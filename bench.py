@@ -1,6 +1,6 @@
 """bench.py -- Envelope-Q gradient updates/sec on synthetic transitions (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 One "step" = one gradient update of Envelope Q-learning (reference envelope.py:269-334, gradient_updates=1) at
@@ -12,16 +12,18 @@ grad clip -> Adam (+ target sync every 200 steps).
            Envelope.update() with the replay store resident in HBM (per step 9 KB of indices + weights in, 4 KB of priorities + loss out).
   e2e    : updates/s through the same call with a HOST-resident replay buffer: per step the gathered minibatch (pinned, 283 KB) crosses
            host->device and the priorities + loss come back device->host; the loss is read as a python float every update.
-  roofline     : the dominant kernel of the step -- the chained hidden-layer launch (layers 2..4 of both Q-networks, 6 f16x2 tcgen05 products in
+  roofline     : the dominant kernel of the step -- the chained hidden-layer launch (layers 2..4 of both Q-networks, 6 f16x2 wgmma products in
                  one persistent kernel) -- against its binding roofline, the measured dense 16-bit tensor peak (HBM view inside);
                  roofline_gemm_layer: the per-layer kernel it replaces.
   roofline_envelope : the fused envelope-TD kernel north_star names, in the form the update runs it (output layers of both nets + envelope
                  operator + Bellman line in one kernel, Q never in HBM), against the measured HBM bandwidth, timed alone in a CUDA graph on
                  rotating buffer sets larger than L2; roofline_envelope_operator: the standalone operator on Q tensors in HBM.
-  cpu_baseline : the reference's CPU implementation (oracle port, or the unmodified reference when mounted) at the SAME full config,
+  cpu_baseline : the reference's CPU implementation (its PyTorch-CPU port, oracle/envelope_update_port.py) at the SAME full config,
                  a bounded NUMBER of updates (not a bounded batch); cpu_dedup_restatement: the de-duplicated CPU restatement for context.
 N > 1: every rank runs an independent update stream (weak scaling, no data-path collective); the ranks exchange their non-dominated
 fronts with ONE NCCL all-gather per evaluation round, which is timed separately (config.ms_eval_round_*), not inside the updates.
+--dump-outputs DIR: after the timed updates, what the last of them produced (loss, priorities of its minibatch, the online network's
+parameters) is written as DIR/<name>.npy (float32); with the same arguments the inputs, and so these arrays, are the same from run to run.
 """
 
 from __future__ import annotations
@@ -48,8 +50,8 @@ def _peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         p = json.load(open(path))
-        return float(p["hbm_gbs"]), float(p.get("bf16_tflops", 1590.0)), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1590.0, "fallback (B200_PROFILING.md)"
+        return float(p["hbm_gbs"]), float(p.get("bf16_tflops", 989.0)), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, 989.0, "data sheet (H100 SXM at 700 W: 3.35 TB/s HBM3, 989 TFLOP/s dense FP16/BF16), not a measurement"
 
 
 class ClockSampler(threading.Thread):
@@ -120,7 +122,7 @@ def _make_agent(dev, seed, on_device):
 
 def time_envelope_kernel(dev, replays=25):
     """Average launch duration of morl_envelope_td_f32 at the north-star shape: 16 launches on 16 rotating input sets
-    (16 x 13.4 MB = 214 MB > 126 MB L2, so every launch streams its Q tensors from HBM) captured in ONE CUDA graph -- the way the
+    (16 x 13.4 MB = 214 MB > 50 MB L2, so every launch streams its Q tensors from HBM) captured in ONE CUDA graph -- the way the
     update issues it -- and the graph replayed `replays` times between two CUDA events on the launching stream.  (A python launch
     loop measures the host's ctypes call, ~12 us, not the kernel.)"""
     import torch as th
@@ -359,14 +361,12 @@ def _pick_cpu_threads():
 
 def cpu_reference_arm(max_steps, warmup, budget_s, dedup=False):
     """Time the reference's CPU update at the FULL metric configuration (B = 1024 transitions, |W| = 64, net 4x256, per=True: both Q-nets
-    run on B*|W|^2 = 4,194,304 rows, ~3.6 TFLOP and ~11 GB per update) -- no batch sub-sampling, no scaling.  The unmodified reference
-    when /root/reference is mounted (kind "reference"), else its PyTorch-CPU port (kind "port", oracle/envelope_update_port.py, pinned
-    bit-for-bit to the reference by tests/test_port_vs_reference.py).  `dedup=True` times the de-duplicated restatement instead
+    run on B*|W|^2 = 4,194,304 rows, ~3.6 TFLOP and ~11 GB per update) -- no batch sub-sampling, no scaling.  Its PyTorch-CPU
+    port (kind "port", oracle/envelope_update_port.py, pinned to the reference's frozen outputs by tests/test_port_vs_reference.py).  `dedup=True` times the de-duplicated restatement instead
     (B*|W| rows; NOT the reference's code path, reported for context only).  The number of timed steps is bounded by `budget_s`
     (at least 1); the per-step times are returned so the caller can report the median."""
     import torch as th
 
-    from oracle import ref_harness as rh
     from oracle.envelope_update_port import EnvelopeUpdatePort
     from morl_baselines_b200.testing import synthetic_store
 
@@ -374,28 +374,15 @@ def cpu_reference_arm(max_steps, warmup, budget_s, dedup=False):
     n_store = 16384
     store = synthetic_store(n_store, OBS, A, D, seed=0)
     rng = np.random.default_rng(0)
-    if rh.reference_available() and not dedup:
-        kind = "reference"
-        envm = rh.import_reference("morl_baselines.multi_policy.envelope.envelope")
-        agent = envm.Envelope(rh.FakeEnv(obs_dim=OBS, n_actions=A, reward_dim=D), batch_size=B, num_sample_w=W, per=True,
-                              buffer_size=n_store, net_arch=NET, log=False, seed=0, device="cpu")
-        rb = agent.replay_buffer
-        rb.obs[:n_store], rb.next_obs[:n_store], rb.actions[:n_store], rb.rewards[:n_store], rb.dones[:n_store] = (
-            store[k] for k in ("obs", "next_obs", "actions", "rewards", "dones"))
-        rb.size, rb.ptr = n_store, 0
-        rb.tree.batch_set(np.arange(n_store), np.full(n_store, rb.min_priority))
-        agent.global_step = 1
-        step = agent.update
-    else:
-        kind = "dedup-restatement" if dedup else "port"
-        port = EnvelopeUpdatePort(OBS, A, D, NET, seed=0)
+    kind = "dedup-restatement" if dedup else "port"
+    port = EnvelopeUpdatePort(OBS, A, D, NET, seed=0)
 
-        def step():
-            idx = rng.integers(0, n_store, size=B)
-            wset = np.abs(rng.standard_normal((W, D)))
-            wset = th.from_numpy((wset / wset.sum(1, keepdims=True)).astype(np.float32))
-            port.update(th.from_numpy(store["obs"][idx]), th.from_numpy(store["actions"][idx]), th.from_numpy(store["rewards"][idx]),
-                        th.from_numpy(store["next_obs"][idx]), th.from_numpy(store["dones"][idx]), wset, dedup=dedup)
+    def step():
+        idx = rng.integers(0, n_store, size=B)
+        wset = np.abs(rng.standard_normal((W, D)))
+        wset = th.from_numpy((wset / wset.sum(1, keepdims=True)).astype(np.float32))
+        port.update(th.from_numpy(store["obs"][idx]), th.from_numpy(store["actions"][idx]), th.from_numpy(store["rewards"][idx]),
+                    th.from_numpy(store["next_obs"][idx]), th.from_numpy(store["dones"][idx]), wset, dedup=dedup)
 
     t_begin = time.perf_counter()
     t_warm = []
@@ -417,7 +404,7 @@ def cpu_reference_arm(max_steps, warmup, budget_s, dedup=False):
 
 
 def run_reference_arm(args, rank):
-    """`--impl reference`: the reference's own CPU implementation of the update on this box's host cores, SAME config as the B200 arm
+    """`--impl reference`: the reference's own CPU implementation of the update on the host cores, SAME config as the GPU arm
     (full batch, full weight set).  Warm-up is capped at one full update and the number of timed updates by a wall-clock budget
     (MORL_CPU_BUDGET_S, default 240 s) -- `steps` in the line is the number actually timed, `steps_requested` what was asked for."""
     if rank != 0:
@@ -440,6 +427,20 @@ def run_reference_arm(args, rank):
     print(json.dumps(line), flush=True)
 
 
+def _dump_outputs(out_dir, agent):
+    """What the last timed Envelope.update() handed back: its loss, the new priorities of its minibatch and the online network it left."""
+    import torch as th
+
+    os.makedirs(out_dir, exist_ok=True)
+    th.cuda.synchronize()
+    s = agent._ensure_static()
+    arrays = {"loss": np.asarray([agent.last_loss_host()]), "priorities": s["prio"].detach().cpu().numpy()}
+    for name, p in agent.q_net.named_parameters():
+        arrays["q_net." + name] = p.detach().cpu().numpy()
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
+
+
 def run_b200(args, rank, local_rank, world):
     import torch as th
     import torch.distributed as dist
@@ -454,7 +455,8 @@ def run_b200(args, rank, local_rank, world):
         dist.init_process_group("nccl", device_id=dev)
     K, Wm = args.steps, args.warmup
     store = synthetic_store(STORE, OBS, A, D, seed=0)
-    np.random.seed(1000 + rank)
+    np.random.seed(1000 + rank)  # replay indices
+    th.manual_seed(1000 + rank)  # network initialisation: with the same arguments every run starts from the same parameters
 
     # ---------------- `value`: the full update of SURVEY 8(d) -- PER sample + targets + forward/backward + optimiser + priority write-back --
     # through the public API with the replay store RESIDENT IN HBM: per step the host walks the sum-tree, 9 KB of indices + weights go
@@ -514,6 +516,8 @@ def run_b200(args, rank, local_rank, world):
     ms, ms_eval_max = float(t_ms[0]), float(t_ms[1])
     value = world * K / (ms * 1e-3)
     loss_dev = agent.last_loss_host()
+    if args.dump_outputs and rank == 0:
+        _dump_outputs(args.dump_outputs, agent)
     h2d_value = B * 8 + 16 + W * D * 4
     del ev_plan
 
@@ -554,13 +558,7 @@ def run_b200(args, rank, local_rank, world):
     t_gemm, gemm_flops, gemm_nprod, gemm_bpe = time_gemm_kernel(dev)
     alg_bytes = 2 * B * W * A * D * 4 + W * D * 4 + B * D * 4 + B * 4 + W * B * D * 4  # SURVEY.md 8(d): 13,386,496 B
     achieved = alg_bytes / t_kernel / 1e9
-    traffic = gemm_traffic = None
-    tpath = os.path.join(ROOT, "profiles", "envelope_td_traffic.json")
-    if os.path.exists(tpath):
-        traffic = json.load(open(tpath)).get("dram_bytes_per_launch")
-    tpath = os.path.join(ROOT, "profiles", "gemm_traffic.json")
-    if os.path.exists(tpath):
-        gemm_traffic = json.load(open(tpath)).get("dram_bytes_per_launch")
+    traffic = gemm_traffic = None  # DRAM bytes per launch from a hardware counter: not measured
     gemm_alg_bytes = 2 * gemm_bpe * B * W * NET[0] + gemm_bpe * NET[0] * NET[0]  # A planes read + C planes written + weight planes
     # fused output layers + envelope + Bellman (the form Envelope.update uses when the shape is inside the kernel): the last hidden
     # activation planes of both nets are its HBM input (the Q tensors never exist in HBM), plus the small operands and the targets
@@ -570,11 +568,10 @@ def run_b200(args, rank, local_rank, world):
     if agent.tensor_core_format == "f16x2" and _ops.qhead_envelope_supported(_ops.FMT_F16X2, B, W, A, D, NET[-1]):
         t_fused = time_qhead_kernel(dev)
         fused_bytes = 2 * 4 * B * W * NET[-1] + 2 * 4 * 32 * NET[-1] + W * D * 4 + B * D * 4 + B * 4 + W * B * D * 4
-        tf = os.path.join(ROOT, "profiles", "qhead_envelope_traffic.json")
-        fused = {"bound": "hbm", "kernel": "qhead_envelope_kernel<f16x2, 3, UNFUSED> (output layers of both Q-nets 65536x24x256 on tcgen05 + envelope "
-                                           "operator + Bellman line; Q tiles in tensor / shared memory only)",
+        fused = {"bound": "hbm", "kernel": "qhead_envelope_kernel<f16x2, 3, UNFUSED> (output layers of both Q-nets 65536x24x256 on wgmma + envelope "
+                                           "operator + Bellman line; Q tiles in registers / shared memory only)",
                  "achieved": fused_bytes / t_fused / 1e9, "peak": hbm_peak, "unit": "GB/s", "frac": fused_bytes / t_fused / 1e9 / hbm_peak,
-                 "traffic": json.load(open(tf)).get("dram_bytes_per_launch") if os.path.exists(tf) else None, "algorithmic_bytes": fused_bytes,
+                 "traffic": None, "algorithmic_bytes": fused_bytes,
                  "us_per_launch": t_fused * 1e6, "peak_source": peak_src, "in_update": bool(getattr(agent, "fused_head_active", False)),
                  "replaces": "2 x morl_gemm_planes_f32 (N = 24) + morl_envelope_td_f32",
                  "timing": "8 launches on 4 rotating pairs of activation-plane tensors (4 x 2 x 67 MB > L2) in one CUDA graph, 12 replays, CUDA events"}
@@ -583,32 +580,29 @@ def run_b200(args, rank, local_rank, world):
                       "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak, "traffic": traffic, "algorithmic_bytes": alg_bytes,
                       "us_per_launch": t_kernel * 1e6, "peak_source": peak_src,
                       "timing": "16 launches on rotating input sets (214 MB > L2) in one CUDA graph, 25 replays, CUDA events"}
-    gemm_layer = {"kernel": "gemm_planes_kernel<pair, f16x2> (ONE hidden layer 65536x256x256 per launch: the per-layer form the chained launch replaces)",
+    gemm_layer = {"kernel": "gemm_planes_kernel<f16x2> (ONE hidden layer 65536x256x256 per launch: the per-layer form the chained launch replaces)",
                   "us_per_launch": t_gemm * 1e6, "hbm_frac": gemm_alg_bytes / t_gemm / 1e9 / hbm_peak, "tensor_frac": gemm_flops / t_gemm / 1e12 / bf16_peak}
     chain_roofline = None
     if agent.tensor_core_format == "f16x2" and _ops.gemm_chain_supported(_ops.FMT_F16X2, B * W, NET[0]) and os.environ.get("MORL_GEMM_CHAIN", "1") == "1":
         t_ch, n_prod, ch_flops, ch_bytes = time_chain_kernel(dev)
-        # dominant kernel of the step: the chained hidden layers (3 launches per update, ~45 % of it).  Floors of the 6-product launch: tensor pipe
-        # 6 x 3 x 8.6 GFLOP / 1687 TFLOP/s = 91.6 us, HBM (2 inputs read + 6 outputs written, intermediates re-read from L2) 537 MB / 6.48 TB/s
-        # = 82.9 us -> the binding roofline is the tensor pipe; the HBM view is reported next to it
+        # dominant kernel of the step: the chained hidden layers (3 launches per update).  Floors of the 6-product launch at the H100 SXM data-sheet
+        # rates: tensor pipe 6 x 3 x 8.6 GFLOP / 989 TFLOP/s = 156 us, HBM (2 inputs read + 6 outputs written, intermediates re-read from L2)
+        # 537 MB / 3.35 TB/s = 160 us -> the two floors are about equal; the tensor view is the headline, the HBM view is reported next to it
         chain_roofline = {"bound": "tensor", "kernel": f"gemm_chain_kernel<f16x2> (hidden layers 2..4 of both Q-networks, {n_prod} products 65536x256x256 in ONE persistent "
-                                                       "launch, 3 fp16 tcgen05 MMAs per fp32 product, CTA pairs, bias + ReLU + re-split epilogue, intermediates re-read from L2)",
+                                                       "launch, 3 fp16 wgmma MMAs per fp32 product, bias + ReLU + re-split epilogue, intermediates re-read from L2)",
                           "achieved": ch_flops / t_ch / 1e12, "peak": bf16_peak, "unit": "TFLOP/s", "frac": ch_flops / t_ch / 1e12 / bf16_peak,
                           "traffic": None, "algorithmic_flops": ch_flops // 3, "algorithmic_tflops": ch_flops / 3 / t_ch / 1e12,
                           "fp32_accurate_peak_tflops": bf16_peak / 3, "us_per_launch": t_ch * 1e6, "us_per_layer_product": t_ch * 1e6 / n_prod,
                           "peak_source": peak_src,
                           "hbm": {"algorithmic_bytes": ch_bytes, "achieved_gbs": ch_bytes / t_ch / 1e9, "peak": hbm_peak, "frac": ch_bytes / t_ch / 1e9 / hbm_peak},
                           "timing": "4 launches on 2 rotating sets of activation buffers (2 x 8 x 67 MB > L2) captured in one CUDA graph, 10 replays, CUDA events"}
-        tf = os.path.join(ROOT, "profiles", "gemm_chain_traffic.json")
-        if os.path.exists(tf):
-            chain_roofline["traffic"] = json.load(open(tf)).get("dram_bytes_per_launch")
     line = {
         "metric": METRIC, "value": value, "unit": "updates/s", "n_gpus": world, "steps": K, "warmup": Wm, "ms_per_step": ms / K,
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {
             "workload": f"Envelope-Q gradient update obs={OBS} |A|={A} d={D} |W|={W} batch={B} net=4x256 per=True, store {STORE} transitions",
             "parallelism": f"replicas x{world} + 1 front all-gather per evaluation round" if world > 1 else "single GPU",
-            "l2": "no explicit flush: each step streams ~0.7 GB of activation planes (65,536 x 256 x 4 B per layer), far above the 126 MB L2",
+            "l2": "no explicit flush: each step streams ~0.7 GB of activation planes (65,536 x 256 x 4 B per layer), far above the 50 MB L2",
             "value_definition": "Envelope.update() with the replay store resident in HBM: PER sum-tree walk, H2D of indices + weights "
                                 f"({h2d_value} B), one CUDA-graph replay, D2H of priorities + loss ({B * 4 + 4} B), priority write-back -- all inside the timed region",
             "e2e_definition": "the same call with a HOST-resident replay buffer: the gathered minibatch crosses PCIe every update",
@@ -620,15 +614,15 @@ def run_b200(args, rank, local_rank, world):
         "e2e": {"value": e2e_value, "unit": "updates/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
         "gpu_launches": int(gpu_launches),
         "clocks": clocks,
-        # dominant kernel of the step (58 % of it, profiles/r02_launches.txt): one hidden layer of the pair batch.  With the f16x2 operand
+        # dominant kernel of the step: one hidden layer of the pair batch.  With the f16x2 operand
         # format its HBM floor (plane bytes in + out) is above its tensor floor, so the binding roofline is HBM: `achieved` = algorithmic
         # plane bytes / time against the measured bandwidth; the tensor-pipe view (MMA flops actually issued against the measured dense
         # 16-bit peak; SURVEY 8(d)'s "FP32-accurate peak actually used" = peak / products) is reported under "tensor".
-        "roofline": chain_roofline if chain_roofline is not None else {"bound": "hbm", "kernel": f"gemm_planes_kernel<pair, {agent.tensor_core_format}> (65536x256x256: one hidden layer of the pair batch, "
-                                                f"{gemm_nprod} 16-bit tcgen05 products per fp32 product, CTA pairs, bias + ReLU + re-split epilogue)",
+        "roofline": chain_roofline if chain_roofline is not None else {"bound": "hbm", "kernel": f"gemm_planes_kernel<{agent.tensor_core_format}> (65536x256x256: one hidden layer of the pair batch, "
+                                                f"{gemm_nprod} 16-bit wgmma products per fp32 product, bias + ReLU + re-split epilogue)",
                      "achieved": gemm_alg_bytes / t_gemm / 1e9, "peak": hbm_peak, "unit": "GB/s", "frac": gemm_alg_bytes / t_gemm / 1e9 / hbm_peak,
                      "traffic": gemm_traffic, "algorithmic_bytes": gemm_alg_bytes, "us_per_launch": t_gemm * 1e6, "peak_source": peak_src,
-                     "why_hbm": "floors of this launch: HBM 134.5 MB / 6.48 TB/s = 20.7 us, tensor pipe 3 x 8.6 GFLOP / 1687 TFLOP/s = 15.3 us",
+                     "why_hbm": "floors of this launch at the H100 SXM data-sheet rates: HBM 134.5 MB / 3.35 TB/s = 40.1 us, tensor pipe 3 x 8.6 GFLOP / 989 TFLOP/s = 26.1 us",
                      "tensor": {"issued_tflops": gemm_flops / t_gemm / 1e12, "peak": bf16_peak, "frac": gemm_flops / t_gemm / 1e12 / bf16_peak,
                                 "algorithmic_flops": gemm_flops // gemm_nprod, "algorithmic_tflops": gemm_flops / gemm_nprod / t_gemm / 1e12,
                                 "fp32_accurate_peak_tflops": bf16_peak / gemm_nprod},
@@ -641,11 +635,11 @@ def run_b200(args, rank, local_rank, world):
         "roofline_envelope": fused if (fused is not None and fused["in_update"]) else standalone_env,
         "roofline_envelope_operator": standalone_env,
         "mlp": {"flop_per_step": mlp_flops, "fp32_equivalent_tflops": mlp_flops / (ms / K * 1e-3) / 1e12,
-                "path": "layer 1 separable (one fp32 kernel on B + |W| rows), layers 2.. tcgen05 split-operand GEMMs forward and backward",
+                "path": "layer 1 separable (one fp32 kernel on B + |W| rows), layers 2.. wgmma split-operand GEMMs forward and backward",
                 "note": "whole-step time used, so this is a lower bound on the dense-layer rate"},
         "loss": loss_dev, "loss_e2e_last": loss_host,
     }
-    if world == 1 and os.environ.get("MORL_SKIP_CPU_BASELINE", "0") != "1":  # (development runs only: the driver's line always carries it)
+    if world == 1 and os.environ.get("MORL_SKIP_CPU_BASELINE", "0") != "1":  # (development runs only)
         # the reference's CPU update at the SAME config (full batch, full weight set), bounded to ~1 minute of CPU work: 1 warm-up + up to 3
         # timed updates; next to it the de-duplicated CPU restatement (not reference code; BASELINE.md section 2) for context
         times, kind, threads, info = cpu_reference_arm(max_steps=3, warmup=1, budget_s=float(os.environ.get("MORL_CPU_BASELINE_BUDGET_S", "60")))
@@ -682,6 +676,7 @@ def run_morld(args, rank, local_rank, world):
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
     POP, OBS_H, ACT_H, D_H, N_BUF = 64, 11, 3, 3, 16384
+    th.manual_seed(0)  # identical initial population on every rank and in every run
     env = FakeEnv(obs_dim=OBS_H, continuous_action_dim=ACT_H, reward_dim=D_H)
     algo = MORLD(env, pop_size=POP, update_passes=1, log=False, device=dev, seed=0, weight_init_method="random", shared_buffer=True,
                  neighborhood_size=1, policy_args={"learning_starts": 0, "buffer_size": N_BUF})
@@ -822,8 +817,11 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default="envelope", choices=["envelope", "morld", "envelope_dp"])
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the outputs of the last timed update as DIR/<name>.npy (envelope workload)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
+    if args.dump_outputs and (args.impl != "b200" or args.workload != "envelope"):
+        ap.error("--dump-outputs is implemented for the envelope workload of the GPU implementation only")
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

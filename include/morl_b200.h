@@ -1,5 +1,5 @@
 /*
- * morl_b200.h -- C-ABI of libmorl_b200.so: the B200 (sm_100a) update engine for the batched
+ * morl_b200.h -- C-ABI of libmorl_b200.so: the H100 (sm_90a) update engine for the batched
  * multi-objective value-update hot path of LucasAlegre/morl-baselines (reference @ a8acdbb).
  *
  * The reference has NO plugin / FFI layer (SURVEY.md section 8(b)): its boundary is the Python class API.
@@ -74,7 +74,7 @@ extern "C" {
 
 MORL_API int morl_version(void);
 MORL_API const char* morl_last_error(void);
-/* number of SMs of the current device (148 on B200), or a negative MORL_ERR_* */
+/* number of SMs of the current device (132 on H100 SXM), or a negative MORL_ERR_* */
 MORL_API int morl_device_sm_count(void);
 
 /* ------------------------------------------------------------------------------------------------
@@ -255,10 +255,10 @@ MORL_API int morl_sumtree_set_f64(double* tree, int n_levels, long long index, d
 MORL_API int morl_per_priority_f32(const float* raw, int n, float alpha, double* min_priority, double* prio64, float* prio32, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * FP32-accurate dense layers on the tcgen05 tensor cores.  Replace the fp32 GEMMs behind the reference's nn.Linear layers
+ * FP32-accurate dense layers on the Hopper tensor cores (wgmma).  Replace the fp32 GEMMs behind the reference's nn.Linear layers
  * (common/networks.py:10-48; called from envelope.py:59-77 / :300, :420, :429 on the 65,536-row effective batch).
  * Every fp32 operand is carried as P 16-bit planes [P][rows][ld] (`plane_stride` elements between planes) whose sum reproduces it;
- * a product is the sum of the significant plane-by-plane MMAs with fp32 accumulation in tensor memory (csrc/gemm_planes.cu):
+ * a product is the sum of the significant plane-by-plane MMAs with fp32 accumulation in registers (csrc/gemm_planes.cu):
  *   MORL_FMT_F16X2  : P = 2 fp16 planes of  scale * x  (scale: a power of two held in a DEVICE float, NULL = 1), 3 MMAs, exact to
  *                     2^-22; |scale * x| must stay below 65,504 -- beyond it the planes hold Inf/NaN (propagating to every output)
  *                     and morl_plane_overflow_count() becomes non-zero.  4 bytes / element.
@@ -284,12 +284,11 @@ MORL_API int morl_per_priority_f32(const float* raw, int n, float alpha, double*
  *                     morl_pairs_relu_split_planes) zeroes the outputs whose bit is clear, i.e. relu'(x) = [x > 0] exactly as
  *                     torch's ReLU backward (reference networks.py:10-48 under autograd).  Both nullable, 16-byte aligned.
  *                     reverse_tiles != 0 walks the 128-row tiles from the last to the first: alternate it between the layers of
- *                     a chain so that a layer starts on the rows its producer wrote last (still in the 126 MB L2).
- *                     split_accumulators != 0: the leading products A0.B0 and the correction products accumulate in separate TMEM
- *                     buffers and are added once, correctly rounded, in the epilogue -- the tensor cores TRUNCATE their fp32
- *                     accumulation at every MMA, which costs ~2e-6 (f16x2) / ~4e-6 (bf16x3) of systematic relative shrinkage per
- *                     K = 256 layer in one accumulator and ~2.5x less in split mode (profiles/r02_gemm_error.txt); the price is that
- *                     the epilogue of a tile no longer overlaps the MMAs of the next one.
+ *                     a chain so that a layer starts on the rows its producer wrote last (still in the 50 MB L2).
+ *                     split_accumulators != 0: the leading products A0.B0 and the correction products accumulate in separate register
+ *                     accumulators and are added once, correctly rounded, in the epilogue, so that only K/16 accumulations happen at
+ *                     full magnitude; the price is that an output wider than 128 columns is computed as two column units (the
+ *                     A tile is staged twice).
  */
 #define MORL_FMT_BF16X3 0
 #define MORL_FMT_F16X2 1
@@ -316,7 +315,7 @@ MORL_API int morl_gemm_planes_f32(int fmt, const void* a_planes, long long a_pla
  * job (c, l):  act[c][l+1] = f(act[c][l] . W[c][l]^T + bias[c][l]),  planes in / planes out at the scale `act_scale`; f = ReLU (relu != 0:
  * forward chains, optionally recording the ReLU bit masks) or the ReLU-backward mask relu_bits_in[job] (dX chains of the backward pass:
  * G_{l-1} = (G_l . W_l) * relu'(H_{l-1}), biases NULL) --
- * bit-identical to n_chains * n_layers calls of morl_gemm_planes_f32 (c_scale = a_scale) -- but a CTA pair takes each of its 256-row tiles
+ * bit-identical to n_chains * n_layers calls of morl_gemm_planes_f32 (c_scale = a_scale) -- but a CTA takes each of its 128-row tiles
  * through all layers, so every intermediate activation is re-read from the L2 it was just written to instead of from HBM, and the launch
  * prologue / drain is paid once.  Replaces the per-layer launches behind the reference's hidden nn.Linear + ReLU stack (networks.py:10-48) in the
  * no-grad passes (both networks at once: n_chains = 2) and in the training pass (n_chains = 1, with ReLU bit masks).
@@ -348,7 +347,7 @@ MORL_API int morl_ensemble_sample_f32(const float* out, const float* max_logvar,
 /* Output layer of BOTH Q-networks + envelope operator + Bellman line as ONE kernel (csrc/qhead_envelope.cu): replaces, for the two no-grad
  * passes of Envelope.update (reference envelope.py:420, :429, :422-440, :298),
  *     morl_gemm_planes_f32 (online, N = A*D) + morl_gemm_planes_f32 (target) + morl_envelope_td_f32
- * -- the Q tensors live in tensor memory / shared memory only (SURVEY 8(f)2: "envelope operator folded into the last-layer epilogue").
+ * -- the Q tensors live in registers / shared memory only (SURVEY 8(f)2: "envelope operator folded into the last-layer epilogue").
  *   a_on_planes / a_tg_planes : last hidden activations of the online / target net on s', planes [2][B*W][K] (row b*W + j), f16x2;
  *   w_on_planes / w_tg_planes : output-layer weight planes [2][32][K] (rows >= A*D zero), scales as in morl_gemm_planes_f32;
  *   everything from `wset` on  : as morl_envelope_td_f32 (same arithmetic contract, row orders, first-occurrence ties, outputs);

@@ -1,7 +1,7 @@
 """ctypes loader for libmorl_b200.so (the C-ABI of include/morl_b200.h).
 
 There is NO CPU fallback: if the shared library is missing, or a compute entry point is called without a CUDA device,
-the call raises.  The library is built in-tree by ``python -m morl_baselines_b200.csrc.build`` (nvcc, sm_100a) and
+the call raises.  The library is built in-tree by ``python -m morl_baselines_b200.csrc.build`` (nvcc, sm_90a) and
 travels with the repo snapshot to the GPU box.
 """
 
@@ -102,7 +102,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise MorlB200Error(
-            f"{LIB_PATH} not found: build it with `python -m morl_baselines_b200.csrc.build` (nvcc, sm_100a). "
+            f"{LIB_PATH} not found: build it with `python -m morl_baselines_b200.csrc.build` (nvcc, sm_90a). "
             "morl_baselines_b200 has no CPU / eager fallback for its CUDA operators."
         )
     lib = C.CDLL(LIB_PATH)

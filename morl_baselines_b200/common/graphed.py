@@ -1,8 +1,7 @@
-"""CUDA-graph capture of a device-only update step (B200-native replacement of the reference's eager op-by-op updates).
+"""CUDA-graph capture of a device-only update step (replacement of the reference's eager op-by-op updates).
 
 The small actor-critic updates of the reference (MOSAC: mosac_continuous_action.py:429-507; CAPQL: capql.py:321-362;
-GPI-PD continuous: gpi_pd_continuous_action.py:373-452) are ~250 tiny tensor operations -- launch-bound on any GPU (7.7 ms
-eager on a B200 for a 128-row minibatch, 13 ms on the reference's CPU path).  ``GraphedStep`` captures one whole update over
+GPI-PD continuous: gpi_pd_continuous_action.py:373-452) are ~250 tiny tensor operations -- launch-bound on any GPU.  ``GraphedStep`` captures one whole update over
 STATIC input buffers (replay indices, optional injected noise) once and replays it: one host call per update.
 
 Warm-up iterations and the capture pass itself must leave no trace (the number of updates applied to the parameters has to match
@@ -51,7 +50,7 @@ class GraphedStep:
 class PopulationGraph:
     """ONE CUDA graph for the device halves of many independent learners (MORL/D ``__update_others``, reference morld.py:423-433, runs them
     strictly one after the other).  Inside the capture the steps are forked round-robin onto ``n_streams`` side streams and joined again,
-    so the graph has that many parallel branches: the tiny kernels of a 2 x 256, batch-128 actor-critic update leave most of a B200 idle,
+    so the graph has that many parallel branches: the tiny kernels of a 2 x 256, batch-128 actor-critic update leave most of the GPU idle,
     and independent learners fill it.  The result per learner is bit-identical to replaying its own graph (no cross-learner data flow)."""
 
     def __init__(self, steps, mutated, n_streams: int = 8, warmup: int = 3):

@@ -2,7 +2,7 @@
 common/model_based/probabilistic_ensemble.py: same class / parameter / state_dict names, same constructor and ``fit`` arguments, same
 numpy RNG consumption).
 
-B200 form: the training set, the bootstrap index table and the hold-out set live in HBM for the whole ``fit`` (the reference slices
+Device form: the training set, the bootstrap index table and the hold-out set live in HBM for the whole ``fit`` (the reference slices
 numpy arrays and copies every minibatch to the device); a minibatch is a device gather; the five hold-out losses of an epoch come back in ONE
 device-to-host copy (the reference calls ``.item()`` per network); ``sample`` is one batched forward plus ONE fused kernel
 (``morl_ensemble_sample_f32``: logvar clamps, exp, reparameterised sample of the drawn elite, ensemble moments, uncertainty, + obs) instead

@@ -27,9 +27,9 @@ int check_launch(const char* what) {
 }
 
 bool pdl_enabled() {
-    // opt-in: measured on the Envelope update (profiles/r02_bench_ab.txt), the attribute on EVERY kernel of the step costs 4.5 % (1,299 ->
-    // 1,242 updates/s): the early-resident CTAs of the small kernels take issue slots and shared memory from the draining grid.  The
-    // GEMM chain keeps its own switch (MORL_GEMM_PDL, on: +3 %), where the prologue that overlaps is long (TMEM allocation, barriers).
+    // opt-in: with the attribute on EVERY kernel of the step the early-resident CTAs of the small kernels take issue slots and shared memory
+    // from the draining grid (not measured on H100).  The GEMM chain keeps its own switch (MORL_GEMM_PDL, default on), where the prologue
+    // that overlaps (barrier initialisation, tensor-map prefetch) is longer.
     static const bool on = [] { const char* e = getenv("MORL_PDL"); return e && e[0] == '1'; }();
     return on;
 }

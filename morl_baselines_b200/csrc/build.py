@@ -1,9 +1,9 @@
-"""Build libmorl_b200.so in-tree with nvcc for sm_100a (no torch, no JIT cache: the .so travels with the snapshot).
+"""Build libmorl_b200.so in-tree with nvcc for sm_90a (no torch, no JIT cache: the .so travels with the snapshot).
 
     python -m morl_baselines_b200.csrc.build [--force] [--verbose]
 
 Each .cu is compiled to an object (parallel, cached on mtime) and linked into ONE shared library exporting the
-C-ABI of include/morl_b200.h.  Flags: -gencode arch=compute_100a,code=sm_100a -lineinfo -O3; -fmad=false is NOT needed
+C-ABI of include/morl_b200.h.  Flags: -gencode arch=compute_90a,code=sm_90a -lineinfo -O3; -fmad=false is NOT needed
 because every parity-critical operation uses explicit _rn intrinsics.
 """
 
@@ -24,7 +24,7 @@ HEADERS = ["common.cuh", "gemm_tc.cuh", "envelope_wp.cuh", os.path.join(ROOT, "i
 
 NVCC_FLAGS = [
     "-gencode",
-    "arch=compute_100a,code=sm_100a",
+    "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-O3",
     "-std=c++17",
@@ -76,7 +76,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     with cf.ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
         objs = list(ex.map(lambda s: _compile(s, verbose), SOURCES))
     if _stale(LIB, objs):
-        cmd = [_nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+        cmd = [_nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers + argument checking for libmorl_b200.so (sm_100a only).
+// common.cuh -- shared device helpers + argument checking for libmorl_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>

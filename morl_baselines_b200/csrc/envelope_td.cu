@@ -127,14 +127,14 @@ __global__ void __launch_bounds__(512) envelope_td_kernel(const float* __restric
 
 
 // =================================================================================================================
-// v2 fast path: packed-FP32 (FMUL2 / FFMA2) scalarisation, 3-input FMNMX3 max tree, persistent CTAs with a
+// v2 fast path: pairwise scalarisation (two weights per register pair), max tree, persistent CTAs with a
 // register-prefetched double buffer.  Bit-identical to the scalar arithmetic above:
 //   * mul.rn.f32x2 is two IEEE multiplies; the unfused add is issued as fma.rn.f32x2(acc, ONE, p) with ONE = 1.0f passed
-//     as a RUNTIME kernel argument -- ptxas contracts mul.rn.f32x2 + add.rn.f32x2 into FFMA2 even with -fmad=false
+//     as a RUNTIME kernel argument -- ptxas may contract a multiply and a dependent add into an FMA even with -fmad=false
 //     (observed with CUDA 12.9), but it cannot fold a multiplier it does not know; fl(acc * 1 + p) == fl(acc + p);
 //   * the Q_on[b] block is transposed once into shared memory as SoA planes Qs[r][c] (c = j*A + a), so one LDS.128 yields
 //     the r-th objective of four consecutive candidates already sitting in aligned register pairs;
-//   * candidates are scanned in groups of 8: four packed dot products, max of 8 with FMNMX3, and only the GROUP index of
+//   * candidates are scanned in groups of 8: four packed dot products, max of 8, and only the GROUP index of
 //     the running maximum is tracked (strict '>' keeps the first group); the exact (first) position inside the winning
 //     group is recovered afterwards by re-evaluating its 8 scores with the scalar path and testing equality.
 // =================================================================================================================
@@ -145,21 +145,22 @@ __device__ __forceinline__ u64 pk2(float lo, float hi) {
     return r;
 }
 __device__ __forceinline__ void upk2(u64 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
+// Hopper has no packed-fp32 arithmetic and no 3-input max: the pair forms below are two scalar IEEE operations on the halves of the
+// register pair (the same values a packed instruction would give), the 3-input max two FMNMX
 __device__ __forceinline__ u64 mul2(u64 a, u64 b) {
-    u64 r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    upk2(a, a0, a1);
+    upk2(b, b0, b1);
+    return pk2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
-    u64 r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
+    float a0, a1, b0, b1, c0, c1;
+    upk2(a, a0, a1);
+    upk2(b, b0, b1);
+    upk2(c, c0, c1);
+    return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
-__device__ __forceinline__ float max3(float a, float b, float c) {
-    float r;
-    asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-    return r;
-}
+__device__ __forceinline__ float max3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 
 // packed w . q for two candidates; `one2` = (1.0f, 1.0f) built from the runtime kernel argument
 template <int D, int MODE>
@@ -436,7 +437,7 @@ __global__ void __launch_bounds__(256) envelope_td_v3_kernel(const float* __rest
 // =================================================================================================================
 // v5 kernel ("weight pairs"): the same FMA-chain filter + exact re-check as v3, re-blocked so that
 //   * a thread owns TWO scalarising weights packed in f32x2 registers and the candidate value is the scalar operand of the packed
-//     FMUL2 / FFMA2 (SASS form  FFMA2 Rd, Rw.F32x2, Rq.F32, Rc.F32x2): one LDS.128 of the AoS block feeds two weights, so the
+//     a multiply / FMA pair per candidate: one LDS.128 of the AoS block feeds two weights, so the
 //     shared-memory traffic per score halves and Q_on[b] is consumed exactly as the bulk copy (TMA) delivered it -- the
 //     AoS -> SoA transposition pass of v3 (and its barrier) disappears;
 //   * a warp covers all 64 weights of a weight block (lane = weight pair) and one quarter of the candidates, so every
@@ -721,9 +722,7 @@ static EnvelopePlan plan_envelope(int B, int W, int A, int D) {
 }
 
 // Path selection, read on every call: MORL_ENVELOPE_PATH = "v1" (generic kernel), "v3" (CUDA-core fast path), "wp" (v5, weight-pair
-// re-blocking of v3; the default whenever the shape fits, then v3, then v1).  (A tensor-core scoring path existed in round 1; it was
-// bit-identical but measured SLOWER on B200 -- reading the 128 KB score tile back from tensor memory is limited to 64 B/clk per SM,
-// profiles/r01_s3_envelope_tc_ncu.txt -- and has been removed from the library; DESIGN.md section 4.1.)  MORL_ENVELOPE_FORCE_V1 is the
+// re-blocking of v3; the default whenever the shape fits, then v3, then v1).  MORL_ENVELOPE_FORCE_V1 is the
 // older spelling of "v1".
 static int envelope_path_override() {
     if (getenv("MORL_ENVELOPE_FORCE_V1") != nullptr) return 1;
@@ -761,7 +760,7 @@ extern "C" int morl_envelope_td_f32(const float* q_online, const float* q_target
             sm_count_cached = n;
         else {
             (void)cudaGetLastError();
-            sm_count_cached = 148;
+            sm_count_cached = 132;
         }
     }
     const int path = envelope_path_override();
@@ -782,9 +781,8 @@ extern "C" int morl_envelope_td_f32(const float* q_online, const float* q_target
                             long long gx = (long long)sm_count_cached * occ / gy;
                             if (gx < 1) gx = 1;
                             if (gx > B) gx = B;
-                            // measured (profiles/r01_s3_pdl_ab.txt): helps when one CTA per SM is resident (B = 148: 3.8 -> 3.35 us) and in
-                            // launch-bound python loops, hurts at the north-star shape where the next grid's early CTAs compete with the
-                            // 7 resident CTAs per SM of the running grid (9.85 -> 10.65 us); whole step unchanged -> opt-in only
+                            // opt-in only: it can help when one CTA per SM is resident and in launch-bound python loops, but at the north-star
+                            // shape the next grid's early CTAs compete with the resident CTAs of the running grid (not measured on H100)
                             static const bool want_pdl = [] { const char* e = getenv("MORL_ENVELOPE_PDL"); return e && e[0] == '1'; }();
                             if (want_pdl) {
                                 // programmatic stream serialisation: the grid may start (barrier init, CTA residency) while the previous

@@ -22,21 +22,22 @@ __device__ __forceinline__ u64 pk2(float lo, float hi) {
     return r;
 }
 __device__ __forceinline__ void upk2(u64 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
+// Hopper has no packed-fp32 arithmetic and no 3-input max: the pair forms below are two scalar IEEE operations on the halves of the
+// register pair (the same values a packed instruction would give), the 3-input max two FMNMX
 __device__ __forceinline__ u64 mul2(u64 a, u64 b) {
-    u64 r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    upk2(a, a0, a1);
+    upk2(b, b0, b1);
+    return pk2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
-    u64 r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
+    float a0, a1, b0, b1, c0, c1;
+    upk2(a, a0, a1);
+    upk2(b, b0, b1);
+    upk2(c, c0, c1);
+    return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
-__device__ __forceinline__ float max3(float a, float b, float c) {
-    float r;
-    asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-    return r;
-}
+__device__ __forceinline__ float max3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 
 // per-group scratch in shared memory: [4][64] best group maximum, runner-up, group of best; [4] max |Q| bits per warp
 struct Scratch {

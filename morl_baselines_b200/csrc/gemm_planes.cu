@@ -1,9 +1,9 @@
-// gemm_planes.cu -- FP32-accurate dense layers on the 5th-generation tensor cores (tcgen05 + TMEM + TMA), sm_100a.
+// gemm_planes.cu -- FP32-accurate dense layers on the Hopper tensor cores (wgmma + TMA + mbarrier), sm_90a.
 //
 // Replaces the cuBLAS SIMT sgemm calls behind the reference's nn.Linear layers (common/networks.py:10-48, called from
 // multi_policy/envelope/envelope.py:59-77, 300, 420, 429) on the 65,536-row effective batch.  The 1e-5 parity bar rules out
 // plain TF32/BF16/FP16, so every fp32 operand is carried as a small number of 16-bit PLANES whose sum reproduces it, and a product
-// A.B^T is the sum of the significant plane-by-plane tensor-core MMAs, accumulated in fp32 in tensor memory.  Two operand formats:
+// A.B^T is the sum of the significant plane-by-plane tensor-core MMAs, accumulated in fp32 in the registers of a warpgroup.  Two operand formats:
 //
 //   MORL_FMT_F16X2  (default of the update path)   s x = h0 + h1: two fp16 planes (11 + 11 significand bits) of the operand scaled
 //       by a power of two s (device-resident, per tensor) -- exact to 2^-22 relative; THREE MMAs  A1B0 + A0B1 + A0B0  per product
@@ -15,14 +15,15 @@
 //       exact to 2^-24; SIX MMAs  A2B0 + A0B2 + A1B1 + A1B0 + A0B1 + A0B0, 6 bytes per element.
 // Either way the result differs from an fp32 GEMM only at the level of its own accumulation-order noise (tests/test_gemm_gpu.py).
 //
-// K-major kernel anatomy (persistent, one CTA per SM -- or one CTA PAIR per TPC with tcgen05 cta_group::2 --, 320 threads):
-//   warp 0   : TMA producer   -- cp.async.bulk.tensor.3d of a [P planes x 128 rows x BK] A box and a [P x BN x BK] B box per stage
-//              (f16x2: BK = 64, 128-byte swizzle, 3 x 64 KB stages; bf16x3: BK = 32, 64-byte swizzle, 3 x 48 KB stages), mbarrier ring;
-//   warp 1   : MMA issuer     -- one elected thread issues NPROD x BK/16 tcgen05.mma.kind::f16 (M=128/256, N=BN, K=16) per stage and
-//              commits the stage back to the producer; accumulators live in TMEM (2 x BN columns, double buffered);
-//   warps 2-9: epilogue       -- tcgen05.ld (32 lanes x 32 columns per warp-instruction), x 2^-(sA+sB), + bias, ReLU / ReLU-mask, then
-//              an fp32 row-major store and/or a re-split into planes (the operand format of the next layer) through a TMA store, so
-//              intermediate activations never exist in fp32 in HBM.
+// K-major kernel anatomy (persistent, one CTA per SM, 288 threads):
+//   warps 0-7: two consumer warpgroups -- each owns 64 of the tile's 128 rows: waits for a stage, issues NPROD x BK/16
+//              wgmma.mma_async (M = 64, N = unit width, K = 16) from the staged boxes and hands the stage back to the producer once the
+//              MMAs that read it have completed; the accumulators (N / 2 fp32 registers per thread) then go through the epilogue in place:
+//              x 2^-(sA+sB), + bias, ReLU / ReLU-mask, then an fp32 row-major store and/or a re-split into planes (the operand format
+//              of the next layer) through a TMA store, so intermediate activations never exist in fp32 in HBM;
+//   warp 8   : TMA producer    -- cp.async.bulk.tensor.3d of a [P planes x 128 rows x BK] A box and P x N/32 [32 rows x BK] B boxes per stage
+//              (f16x2: BK = 64, 128-byte swizzle, 2 x 96 KB stages at N = 256; bf16x3: BK = 32, 64-byte swizzle, 2 x 72 KB), mbarrier
+//              ring; it keeps loading the next tile while the consumers are in their epilogue.
 // Operands: A [P][M][K] (K-major), B [P][N_pad][K] (K-major), K % BK == 0, N_pad % 32 == 0, N_pad <= 256.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -36,7 +37,8 @@
 namespace morl {
 
 constexpr int kGemmBM = 128;
-constexpr int kGemmThreads = 320;  // warp 0 TMA, warp 1 MMA, warps 2-9 epilogue (two warps per TMEM lane quadrant)
+constexpr int kGemmThreads = 288;  // warps 0-7: two consumer warpgroups (wgmma + epilogue), warp 8: TMA producer
+constexpr int kGemmBoxN = 32;      // B rows per TMA box (one plane): any unit width that is a multiple of 32 is a sequence of them
 
 __device__ unsigned int g_plane_overflow;  // number of kernel launches (approx.) that saw an f16x2 element out of fp16 range
 
@@ -55,7 +57,7 @@ __device__ __forceinline__ void note_overflow(float amax) {
 
 
 struct GemmArgs {
-    int M, N, N_pad, K;          // N_pad = B rows covered by the tensor map box (multiple of 16, <= 256)
+    int M, N, N_pad, K;          // N_pad = B rows covered (multiple of 32, <= 256)
     const float* bias;           // [N] or nullptr
     float* c_f32;                // [M, ldc] or nullptr
     int ldc;
@@ -66,32 +68,31 @@ struct GemmArgs {
     int ld_mask;
     const uint32_t* bits_in;     // ReLU-backward mask as BITS [M][8] words (see morl_b200.h "ReLU bit masks"), or nullptr
     uint32_t* bits_out;          // forward: bit = (output > 0) per column, same layout, or nullptr
-    int n_stages;                // depth of the TMA ring: as many (A box + B box) stages as fit (3 at N_pad = 256, more for narrow outputs)
-    uint32_t b_stage;            // bytes of one B stage slot (the B box rounded up to 1 KB)
+    int n_stages;                // depth of the TMA ring: as many (A box + B boxes) stages as fit (2 at N_pad = 256, more for narrow outputs)
+    uint32_t b_stage;            // bytes of one B stage slot (the B rows of a stage rounded up to 1 KB)
     int relu;
     const float* a_scale;        // device scalars (powers of two) the A / B planes were scaled by; nullptr = 1
     const float* b_scale;
     const float* c_scale;        // scale applied to the output before it is re-split into c_planes; nullptr = 1
     int l2_hint;                 // L2 eviction hints on the operand loads (MORL_GEMM_L2HINT=1, default off): A evict_first, B evict_last
-    int skip_b;                  // TIMING EXPERIMENT ONLY (MORL_GEMM_SKIPB=1, wrong results): B boxes are loaded for the first tile of a CTA only
     int pdl;                     // launched with programmatic stream serialisation: overlap this grid's prologue with the predecessor's tail
     int reverse;                 // walk the row tiles from the last to the first (see morl_gemm_planes_f32: L2 reuse between chained layers)
-    unsigned long long* stats;   // diagnostics (MORL_GEMM_STATS=1), else nullptr: [0] MMA wait-on-TMA cycles, [1] MMA wait-on-epilogue,
-                                 // [2] MMA loop total, [3] producer wait-on-free-stage, [4] epilogue wait-on-accumulator, [5] epilogue busy
+    unsigned long long* stats;   // diagnostics (MORL_GEMM_STATS=1), else nullptr: [0] consumer wait-on-TMA cycles, [1] consumer loop total,
+                                 // [2] producer wait-on-free-stage, [3] epilogue busy
 };
 
 __device__ unsigned long long g_gemm_stats[8];
 
 // shared-memory plan of the K-major kernel (host and device agree through these)
-template <int NCTA, int FMT>
+template <int FMT>
 struct KPlan {
     using F = PlaneFmt<FMT>;
-    static constexpr int kStages = NCTA == 2 ? F::kStages2 : F::kStages1;  // ring depth at N_pad = 256
+    static constexpr int kStages = F::kStages;                                    // ring depth at N_pad = 256
     static constexpr int kMaxStages = 8;                                          // barrier slots (narrow outputs run a deeper ring)
     static constexpr uint32_t kRowB = F::BK * 2;                                  // bytes per staged row = swizzle span
     static constexpr uint32_t kAStage = F::P * kGemmBM * kRowB;                   // A box bytes
-    static constexpr uint32_t kBStage = F::P * (256 / NCTA) * kRowB;              // B box bytes at N_pad = 256
-    static constexpr uint32_t kStageC = F::P * 2048;                              // per-epilogue-warp TMA-store tile: P x 32 rows x 64 B
+    static constexpr uint32_t kBStage = F::P * 256 * kRowB;                       // B bytes of a stage at N_pad = 256
+    static constexpr uint32_t kStageC = F::P * 1024;                              // per-consumer-warp TMA-store tile: P x 16 rows x 64 B
     static constexpr uint32_t kOffB = kStages * kAStage;
     static constexpr uint32_t kOffC = kOffB + kStages * kBStage;                  // 1024-aligned (all stage sizes are multiples of 1 KB)
     static constexpr uint32_t kOffBar = kOffC + 8 * kStageC;
@@ -99,26 +100,194 @@ struct KPlan {
     static constexpr uint32_t kBytes = kOffBias + 1024 + 1024;                    // + alignment slack of the dynamic segment
 };
 
-// NCTA = 1: one CTA per 128-row tile.  NCTA = 2: a CTA pair (cluster of 2 on one TPC) per 256-row tile, tcgen05 cta_group::2 --
-// each CTA stages its own 128 A rows and HALF of the B (weight) rows, the pair's tensor cores read both halves, so the L2 -> smem
-// traffic of the weight planes is halved.
-// SPLIT = 1 ("split accumulators"): the tensor cores accumulate in fp32 with TRUNCATION (round toward zero) at every MMA, a bias of
-// about -0.5 ulp of the running sum per instruction; with all NPROD x K/16 products in one accumulator that is ~2e-6 (f16x2) to ~4e-6
-// (bf16x3) of systematic shrinkage per layer at K = 256 (measured: scripts/gemm_error_probe.py).  In split mode the LEADING products
-// A0B0 go to accumulator 0 and the correction products (2^-11 / 2^-8 of the magnitude) to accumulator 1, so only K/16 truncations happen
-// at full magnitude; the epilogue adds the two with one correctly rounded fp32 add.  Cost: the two TMEM buffers no longer double-buffer
-// the accumulator, so the epilogue of a tile does not overlap the MMAs of the next one (the TMA ring still runs ahead).
-template <int NCTA, int FMT, int SPLIT>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBh,
-                   const __grid_constant__ CUtensorMap tmC, const GemmArgs g) {
+// One work unit of a consumer warpgroup: D[64 x N] = sum over the K blocks of the staged planes, NPROD products per K step in the order of
+// PlaneFmt (small terms first).  A stage goes back to the producer as soon as the MMAs reading it have completed: one group of
+// wgmma stays in flight while the next stage is awaited.
+// SPLIT = 1 ("split accumulators", N <= 128): the tensor cores accumulate in fp32 with limited-precision alignment at every MMA; with all
+// NPROD x K/16 products in one accumulator the rounding of the correction products happens at the magnitude of the running sum.  In split
+// mode the LEADING products A0B0 go to acc[0, 64) and the correction products (2^-11 / 2^-8 of the magnitude) to acc[64, 128), so only
+// K/16 accumulations happen at full magnitude; the epilogue adds the two with one correctly rounded fp32 add.
+template <int FMT, int N, int SPLIT>
+__device__ __forceinline__ void mma_unit(float (&acc)[128], uint8_t* smA, uint8_t* smB, uint32_t a_stage_bytes, uint32_t b_stage_stride, int n_kblk,
+                                         uint64_t* full, uint64_t* empty, uint32_t& stage, uint32_t& phase, uint32_t n_stages, int wg, int lane,
+                                         long long* wait_cycles) {
     using F = PlaneFmt<FMT>;
-    using L = KPlan<NCTA, FMT>;
+    static_assert(!SPLIT || N <= 128, "split accumulators: two N / 2-register accumulators per thread");
+    constexpr uint32_t ROWB = F::BK * 2;
+    constexpr uint32_t a_plane = kGemmBM * ROWB, b_plane = (uint32_t)N * ROWB;
+    uint32_t prev = 0;
+    for (int kb = 0; kb < n_kblk; ++kb) {
+        const long long c0 = wait_cycles ? clock64() : 0;
+        g_mbar_wait(&full[stage], phase);
+        if (wait_cycles) *wait_cycles += clock64() - c0;
+        wgmma_fence();
+        const uint32_t a0 = g_smem_u32(smA + stage * a_stage_bytes) + (uint32_t)wg * 64u * ROWB;
+        const uint32_t b0 = g_smem_u32(smB + stage * b_stage_stride);
+#pragma unroll
+        for (int ks = 0; ks < F::BK / 16; ++ks) {
+#pragma unroll
+            for (int t = 0; t < F::NPROD; ++t) {
+                const uint64_t ad = make_desc_k<ROWB>(a0 + F::pa(t) * a_plane + ks * 32);
+                const uint64_t bd = make_desc_k<ROWB>(b0 + F::pb(t) * b_plane + ks * 32);
+                const bool lead = t == F::NPROD - 1;  // the last product of the list is the leading one (A0B0)
+                float* d = (SPLIT && !lead) ? acc + 64 : acc;
+                const uint32_t accumulate = SPLIT ? ((lead ? (kb | ks) : (kb | ks | t)) != 0 ? 1u : 0u) : ((kb | ks | t) != 0 ? 1u : 0u);
+                Wgmma<N>::template mma<FMT, 0, 0>(d, ad, bd, accumulate);
+            }
+        }
+        wgmma_commit();
+        if (kb > 0) {
+            wgmma_wait<1>();  // the MMAs of the previous stage have read it
+            if (lane == 0) g_mbar_arrive(&empty[prev]);
+        }
+        prev = stage;
+        if (++stage == n_stages) {
+            stage = 0;
+            phase ^= 1u;
+        }
+    }
+    wgmma_wait<0>();
+    if (n_kblk > 0 && lane == 0) g_mbar_arrive(&empty[prev]);
+}
+
+struct EpiArgs {
+    int M, N;                    // valid rows / columns of the output
+    float k_acc;                 // accumulator multiplier (operand scales and folded output scale)
+    float c_mul;                 // output scale applied before the re-split when it is not folded into k_acc
+    const float* bias_s;         // shared memory, indexed by output column
+    int relu;
+    const uint32_t* bits_in;
+    uint32_t* bits_out;
+    const uint16_t* mask;
+    int ld_mask;
+    float* c_f32;
+    int ldc;
+    int planes;                  // re-split the output into planes through tmC
+    int ldp;
+};
+
+// Epilogue of one 32-column chunk of a consumer warp's 16 accumulator rows [rbase, rbase + 16): thread l holds a[4 q + 2 h + e] = column
+// col0 + 8 q + 2 (l % 4) + e of row rbase + l / 4 + 8 h (the wgmma fragment).
+template <int FMT>
+__device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, int rbase, int lane, const EpiArgs& e, const CUtensorMap* tmC,
+                                               uint8_t* my_stage, float& amax) {
+    using F = PlaneFmt<FMT>;
+    constexpr int P = F::P;
+    const int l4 = lane & 3, lr = lane >> 2;
+    // ReLU bit masks: word (c & 1) * 4 + (c >> 1) of the row holds columns [32 c, 32 c + 32)
+    const int wi = ((col0 >> 5) & 1) * 4 + (col0 >> 6);
+    float x[2][8];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                float f = __fmaf_rn(a[4 * q + 2 * h + c], e.k_acc, e.bias_s[col0 + 8 * q + 2 * l4 + c]);
+                if (e.relu) f = (f < 0.f) ? 0.f : f;  // (NaN stays NaN, like torch.relu: an overflow upstream must reach the loss)
+                x[h][2 * q + c] = f;
+            }
+    if (e.bits_in) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = rbase + lr + 8 * h;
+            const uint32_t keep = row < e.M ? __ldg(e.bits_in + (size_t)row * 8 + wi) : 0u;
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+                if (!((keep >> (8 * (j >> 1) + 2 * l4 + (j & 1))) & 1u)) x[h][j] = 0.f;
+        }
+    }
+    if (e.bits_out) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = rbase + lr + 8 * h;
+            uint32_t positive = 0;
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+                if (x[h][j] > 0.f) positive |= 1u << (8 * (j >> 1) + 2 * l4 + (j & 1));
+            positive |= __shfl_xor_sync(0xffffffffu, positive, 1);  // the four threads of a row hold 8 of its 32 columns each
+            positive |= __shfl_xor_sync(0xffffffffu, positive, 2);
+            if (l4 == 0 && row < e.M) e.bits_out[(size_t)row * 8 + wi] = positive;
+        }
+    }
+    if (e.mask) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = rbase + lr + 8 * h;
+            if (row < e.M) {
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const uint32_t mm = __ldg(reinterpret_cast<const uint32_t*>(e.mask + (size_t)row * e.ld_mask + col0 + 8 * q + 2 * l4));
+                    // (bf16 or fp16) > 0  <=>  sign bit clear and magnitude non-zero (NaN never occurs in a ReLU output)
+                    if ((mm & 0x8000u) || (mm & 0x7FFFu) == 0u) x[h][2 * q] = 0.f;
+                    if ((mm & 0x80000000u) || (mm & 0x7FFF0000u) == 0u) x[h][2 * q + 1] = 0.f;
+                }
+            }
+        }
+    }
+    if (e.c_f32) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = rbase + lr + 8 * h;
+            if (row < e.M) {
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const int col = col0 + 8 * q + 2 * l4;
+                    float* p = e.c_f32 + (size_t)row * e.ldc + col;
+                    if (col + 1 < e.N && (e.ldc & 1) == 0) {
+                        *reinterpret_cast<float2*>(p) = make_float2(x[h][2 * q], x[h][2 * q + 1]);
+                    } else {
+                        if (col < e.N) p[0] = x[h][2 * q];
+                        if (col + 1 < e.N) p[1] = x[h][2 * q + 1];
+                    }
+                }
+            }
+        }
+    }
+    if (e.planes && col0 < e.ldp) {
+        // stage the warp's [16 rows x 32 cols] x P planes in shared memory (TMA SWIZZLE_64B pattern: 16-byte chunk index XOR ((row >> 1) & 3),
+        // bank-conflict free), then ONE bulk tensor store writes it out coalesced and asynchronously
+        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // previous store has read the staging tile
+        __syncwarp();
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int rl = lr + 8 * h;
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const int col = col0 + 8 * q + 2 * l4;
+                // ragged last chunk: columns [N, ldp) are written as zero
+                const float x0 = col < e.N ? x[h][2 * q] * e.c_mul : 0.f, x1 = col + 1 < e.N ? x[h][2 * q + 1] * e.c_mul : 0.f;
+                uint32_t w[P];
+                F::split2(x0, x1, w, amax);  // re-split (c_scale x) into P planes, two columns per word
+                uint8_t* st = my_stage + rl * 64 + ((q ^ ((rl >> 1) & 3)) << 4) + 4 * l4;
+#pragma unroll
+                for (int p = 0; p < P; ++p) *reinterpret_cast<uint32_t*>(st + p * 1024) = w[p];
+            }
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        __syncwarp();
+        if (lane == 0) {
+            asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(tmC), "r"(g_smem_u32(my_stage)),
+                         "r"(col0), "r"(rbase), "r"(0)
+                         : "memory");
+            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        }
+    }
+}
+
+// One CTA per 128-row tile.  SPLIT = 1: see mma_unit; a tile wider than 128 columns is then computed as two column units (the A boxes of the
+// tile are staged once per unit).
+template <int FMT, int SPLIT>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC,
+                   const GemmArgs g) {
+    using F = PlaneFmt<FMT>;
+    using L = KPlan<FMT>;
     constexpr int P = F::P;
     constexpr int BK = F::BK;
     constexpr int kMaxStages = L::kMaxStages;
     constexpr uint32_t ROWB = L::kRowB;
-    const int kStages = g.n_stages;  // runtime: narrow B boxes leave room for a deeper ring (host: plan_stages)
+    const uint32_t kStages = (uint32_t)g.n_stages;  // runtime: narrow outputs leave room for a deeper ring (host: morl_gemm_planes_f32)
     extern __shared__ uint8_t gsmem_raw[];
     // 1 KB alignment by pointer arithmetic ON the shared array (not through an integer cast), so that the compiler keeps every derived
     // pointer in the shared address space: through the cast the bias / staging accesses were generic LD.E / ST.E (long-scoreboard stalls)
@@ -127,73 +296,45 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     constexpr uint32_t a_stage_bytes = L::kAStage;
     const uint32_t b_stage_stride = g.b_stage;
     uint8_t* smA = gsmem;
-    uint8_t* smB = gsmem + (uint32_t)kStages * a_stage_bytes;  // (n_stages * (A + B) <= kOffC, checked on the host)
-    uint8_t* stage_c = gsmem + L::kOffC;  // per-epilogue-warp staging tiles for the TMA store of the re-split activations
+    uint8_t* smB = gsmem + kStages * a_stage_bytes;  // (n_stages * (A + B) <= kOffC, checked on the host)
+    uint8_t* stage_c = gsmem + L::kOffC;  // per-consumer-warp staging tiles for the TMA store of the re-split activations
     uint64_t* full = reinterpret_cast<uint64_t*>(gsmem + L::kOffBar);
     uint64_t* empty = full + kMaxStages;
-    uint64_t* tfull = empty + kMaxStages;
-    uint64_t* tempty = tfull + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
     float* bias_s = reinterpret_cast<float*>(gsmem + L::kOffBias);  // [256]
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const uint32_t cta_rank = NCTA == 2 ? cluster_ctarank() : 0u;
-    const int unit = blockIdx.x / NCTA, n_units = gridDim.x / NCTA;  // a unit = one CTA (NCTA = 1) or one CTA pair
-    const int n_tiles = (g.M + kGemmBM * NCTA - 1) / (kGemmBM * NCTA);
+    const int n_tiles = (g.M + kGemmBM - 1) / kGemmBM;
     const int n_kblk = g.K / BK;
-    // Work units.  A static round-robin over `n_units` workers leaves a tail of L = n_tiles % n_units tiles that costs a whole
-    // extra round (65,536 rows: 256 pair tiles on 74 pairs = 3.46 -> 4 rounds).  When 2L <= n_units the tail tiles are split into
-    // two half-width (N/2) units each, so the tail costs half a round.  All three roles enumerate the same sequence.
-    const int full_units = (n_tiles / n_units) * n_units;
-    const int tail = n_tiles - full_units;
-    const bool split_tail = NCTA == 2 && tail > 0 && 2 * tail <= n_units && (BN % 64) == 0;
-    const int n_work = split_tail ? full_units + 2 * tail : n_tiles;
+    // Work units: a tile, or (split accumulators, more than 128 columns) its two column units [0, 128) and [128, BN).  Both roles enumerate
+    // the same sequence.
+    const int col_units = (SPLIT && BN > 128) ? 2 : 1;
+    const int n_work = n_tiles * col_units;
     auto unit_of = [&](int u, int& tile, int& n_begin, int& n_cnt) {
-        if (!split_tail || u < full_units) {
-            tile = u; n_begin = 0; n_cnt = BN;
-        } else {
-            const int r = u - full_units;
-            tile = full_units + (r >> 1); n_cnt = BN >> 1; n_begin = (r & 1) * n_cnt;
-        }
+        tile = u / col_units;
+        n_begin = (u - tile * col_units) * 128;
+        n_cnt = col_units == 1 ? BN : (BN - n_begin < 128 ? BN - n_begin : 128);
         if (g.reverse) tile = n_tiles - 1 - tile;
     };
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kStages; ++s) {
+        for (uint32_t s = 0; s < kStages; ++s) {
             g_mbar_init(&full[s], 1);
-            g_mbar_init(&empty[s], 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            g_mbar_init(&tfull[s], 1);
-            g_mbar_init(&tempty[s], 8 * NCTA);  // one arrival per epilogue warp (of both CTAs of a pair, on the leader's barrier)
+            g_mbar_init(&empty[s], 8);  // one arrival per consumer warp
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {  // TMEM: 512 columns (two BN-column accumulators); in a pair both CTAs' warp 1 execute the paired allocation
-        if (NCTA == 2) {
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(g_smem_u32(tmem_slot)) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(g_smem_u32(tmem_slot)) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-    }
     if (g.pdl) {
-        // programmatic dependent launch: this grid may have become resident (barrier init, TMEM allocation above) while the previous kernel
+        // programmatic dependent launch: this grid may have become resident (barrier init above) while the previous kernel
         // of the stream was still draining its last tiles; let OUR successor do the same, then wait until the predecessor's results are
         // visible -- nothing above this line reads global memory, everything below may
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
         asm volatile("griddepcontrol.wait;" ::: "memory");
     }
     for (int t = threadIdx.x; t < 256; t += blockDim.x) bias_s[t] = (g.bias && t < g.N) ? g.bias[t] : 0.f;
-    tc_fence_before();
     __syncthreads();
-    if (NCTA == 2) cluster_sync_all();  // the peer's barriers are initialised before any remote arrive / complete_tx
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ================= TMA producer =================
         if (lane == 0) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
@@ -201,331 +342,116 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
             uint32_t stage = 0, phase = 0;
             long long w_empty = 0;
             const uint64_t pol_a = l2_policy_evict_first(), pol_b = l2_policy_evict_last();
-            for (int u = unit; u < n_work; u += n_units) {
+            for (int u = blockIdx.x; u < n_work; u += gridDim.x) {
                 int tile, n_begin, n_cnt;
                 unit_of(u, tile, n_begin, n_cnt);
-                const int row0 = (tile * NCTA + (int)cta_rank) * kGemmBM;
-                const int b_rows = n_cnt / NCTA;  // B rows this CTA stages for the unit
+                const int row0 = tile * kGemmBM;
+                const uint32_t b_plane = (uint32_t)n_cnt * ROWB;
                 for (int kb = 0; kb < n_kblk; ++kb) {
                     const long long c0 = g.stats ? clock64() : 0;
                     g_mbar_wait(&empty[stage], phase ^ 1u);
                     if (g.stats) w_empty += clock64() - c0;
-                    if (NCTA == 2) {
-                        const bool load_b = !(g.skip_b && u != unit);
-                        // one expect_tx (leader) covers the four boxes of the pair; every box completes on the leader's barrier
-                        if (cta_rank == 0) g_mbar_expect_tx(&full[stage], 2u * (a_stage_bytes + (load_b ? (uint32_t)P * (uint32_t)b_rows * ROWB : 0u)));
-                        const uint32_t lbar = mapa_rank0(g_smem_u32(&full[stage]));
-                        if (!load_b) {
-                            tma_load_3d_pair(smA + stage * a_stage_bytes, &tmA, lbar, kb * BK, row0, 0);
-                        } else if (g.l2_hint) {
-                            tma_load_3d_pair_hint(smA + stage * a_stage_bytes, &tmA, lbar, kb * BK, row0, 0, pol_a);
-                            tma_load_3d_pair_hint(smB + stage * b_stage_stride, n_cnt == BN ? &tmB : &tmBh, lbar, kb * BK,
-                                                  n_begin + (int)cta_rank * b_rows, 0, pol_b);
-                        } else {
-                            tma_load_3d_pair(smA + stage * a_stage_bytes, &tmA, lbar, kb * BK, row0, 0);
-                            tma_load_3d_pair(smB + stage * b_stage_stride, n_cnt == BN ? &tmB : &tmBh, lbar, kb * BK,
-                                             n_begin + (int)cta_rank * b_rows, 0);
+                    g_mbar_expect_tx(&full[stage], a_stage_bytes + (uint32_t)P * b_plane);
+                    uint8_t* bs = smB + stage * b_stage_stride;
+                    if (g.l2_hint) tma_load_3d_hint(smA + stage * a_stage_bytes, &tmA, &full[stage], kb * BK, row0, 0, pol_a);
+                    else tma_load_3d(smA + stage * a_stage_bytes, &tmA, &full[stage], kb * BK, row0, 0);
+                    for (int p = 0; p < P; ++p)
+                        for (int r = 0; r < n_cnt; r += kGemmBoxN) {
+                            uint8_t* dst = bs + (uint32_t)p * b_plane + (uint32_t)r * ROWB;
+                            if (g.l2_hint) tma_load_3d_hint(dst, &tmB, &full[stage], kb * BK, n_begin + r, p, pol_b);
+                            else tma_load_3d(dst, &tmB, &full[stage], kb * BK, n_begin + r, p);
                         }
-                    } else {
-                        g_mbar_expect_tx(&full[stage], a_stage_bytes + (uint32_t)P * (uint32_t)BN * ROWB);
-                        tma_load_3d(smA + stage * a_stage_bytes, &tmA, &full[stage], kb * BK, row0, 0);
-                        tma_load_3d(smB + stage * b_stage_stride, &tmB, &full[stage], kb * BK, 0, 0);
-                    }
                     if (++stage == kStages) {
                         stage = 0;
                         phase ^= 1u;
                     }
                 }
             }
-            if (g.stats) atomicAdd(&g.stats[3], (unsigned long long)w_empty);
-        }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        if (lane == 0 && cta_rank == 0) {  // in a pair only the leader issues; its MMAs drive both CTAs' tensor cores
-            // instruction descriptor (cute::UMMA::InstrDescriptor): D=f32, A/B format of the plane type, K-major both, N, M=128 (256 per pair)
-            constexpr uint32_t a_plane = kGemmBM * ROWB;
-            uint32_t stage = 0, phase = 0, it = 0;
-            long long w_full = 0, w_tempty = 0;
-            const long long t_begin = g.stats ? clock64() : 0;
-            for (int u = unit; u < n_work; u += n_units, ++it) {
-                int tile, n_begin, n_cnt;
-                unit_of(u, tile, n_begin, n_cnt);
-                const uint32_t idesc = (1u << 4) | F::kIdescAB | ((uint32_t)(n_cnt >> 3) << 17) | ((uint32_t)((kGemmBM * NCTA) >> 4) << 24);
-                const uint32_t b_plane = (uint32_t)(n_cnt / NCTA) * ROWB;
-                const uint32_t as = SPLIT ? 0u : (it & 1u);
-                long long c0 = g.stats ? clock64() : 0;
-                g_mbar_wait(&tempty[as], SPLIT ? ((it & 1u) ^ 1u) : (((it >> 1) & 1u) ^ 1u));
-                if (g.stats) w_tempty += clock64() - c0;
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + as * 256u;
-                for (int kb = 0; kb < n_kblk; ++kb) {
-                    c0 = g.stats ? clock64() : 0;
-                    g_mbar_wait(&full[stage], phase);
-                    if (g.stats) w_full += clock64() - c0;
-                    tc_fence_after();
-                    const uint32_t a0 = g_smem_u32(smA + stage * a_stage_bytes);
-                    const uint32_t b0 = g_smem_u32(smB + stage * b_stage_stride);
-#pragma unroll
-                    for (int ks = 0; ks < BK / 16; ++ks) {
-#pragma unroll
-                        for (int t = 0; t < F::NPROD; ++t) {
-                            const uint64_t ad = make_desc_k<ROWB>(a0 + F::pa(t) * a_plane + ks * 32);
-                            const uint64_t bd = make_desc_k<ROWB>(b0 + F::pb(t) * b_plane + ks * 32);
-                            // split mode: the last product of the list is the leading one (A0B0) -> accumulator 0, the rest -> accumulator 1
-                            const bool lead = t == F::NPROD - 1;
-                            const uint32_t d = SPLIT ? (lead ? d_tmem : d_tmem + 256u) : d_tmem;
-                            const uint32_t acc = SPLIT ? ((lead ? (kb | ks) : (kb | ks | t)) != 0 ? 1u : 0u) : ((kb | ks | t) != 0 ? 1u : 0u);
-                            if (NCTA == 2)
-                                tc_mma_bf16_pair(d, ad, bd, idesc, acc);
-                            else
-                                tc_mma_bf16(d, ad, bd, idesc, acc);
-                        }
-                    }
-                    // frees the smem stage (in both CTAs of a pair) when the MMAs above have read it
-                    if (NCTA == 2) tc_commit_pair(&empty[stage]); else tc_commit(&empty[stage]);
-                    if (++stage == kStages) {
-                        stage = 0;
-                        phase ^= 1u;
-                    }
-                }
-                if (NCTA == 2) tc_commit_pair(&tfull[as]); else tc_commit(&tfull[as]);  // accumulator complete
-            }
-            if (g.stats) {
-                atomicAdd(&g.stats[0], (unsigned long long)w_full);
-                atomicAdd(&g.stats[1], (unsigned long long)w_tempty);
-                atomicAdd(&g.stats[2], (unsigned long long)(clock64() - t_begin));
-            }
+            if (g.stats) atomicAdd(&g.stats[2], (unsigned long long)w_empty);
         }
     } else {
-        // ================= epilogue warps (2..9) =================
-        // warp w may only touch TMEM lanes [32*(w%4), +32); the two warps of a quadrant take alternating 32-column chunks
-        const int quad = warp & 3;
-        const int half = (warp - 2) >> 2;
-        uint8_t* my_stage = stage_c + (warp - 2) * L::kStageC;
+        // ================= consumer warpgroups (warps 0..7) =================
+        const int wg = warp >> 2;
+        uint8_t* my_stage = stage_c + warp * L::kStageC;
         // x = acc / (sA sB) + bias; when only planes are written (the hidden layers) the output scale is FOLDED into the two constants:
         // fold * x = acc * (fold / (sA sB)) + fold * bias (exact, powers of two), and max / mask commute with a positive factor
         const float c_mul = ld_scale(g.c_scale);
         const bool folded = g.c_f32 == nullptr;
         const float fold = folded ? c_mul : 1.0f;
-        const float k_acc = fold / (ld_scale(g.a_scale) * ld_scale(g.b_scale));
-        if (warp == 2 && folded)  // (bias_s was filled before the CTA barrier; one warp rescales it)
+        if (warp == 0 && folded)  // (bias_s was filled before the CTA barrier; one warp rescales it)
             for (int t = lane; t < 256; t += 32) bias_s[t] *= fold;
-        asm volatile("bar.sync 1, 256;" ::: "memory");  // the 8 epilogue warps only
+        asm volatile("bar.sync 1, 256;" ::: "memory");  // the 8 consumer warps only
+        EpiArgs e;
+        e.M = g.M; e.N = g.N;
+        e.k_acc = fold / (ld_scale(g.a_scale) * ld_scale(g.b_scale));
+        e.c_mul = folded ? 1.0f : c_mul;
+        e.bias_s = bias_s; e.relu = g.relu; e.bits_in = g.bits_in; e.bits_out = g.bits_out; e.mask = g.mask; e.ld_mask = g.ld_mask;
+        e.c_f32 = g.c_f32; e.ldc = g.ldc; e.planes = g.c_planes != nullptr; e.ldp = g.ldp;
         float amax = 0.f;
-        uint4 tile_bits = make_uint4(0u, 0u, 0u, 0u);
-        uint4 out_bits = make_uint4(0u, 0u, 0u, 0u);
-        auto process = [&](const uint32_t (&v)[32], int n0, int row, bool row_ok) {
-            // ReLU bit masks: word (c & 1) * 4 + (c >> 1) of the row holds columns [32 c, 32 c + 32); a thread owns the chunks of one parity
-            // (its `half`), so its words of a tile are the four consecutive ones prefetched into tile_bits before the accumulator wait
-            // (both uses are warp-uniform branches: the no-grad forward passes, 8 of the 16 GEMMs of an update, pay nothing for them -- the
-            // epilogue has ~30 % of slack against the MMAs of the next tile and an unconditional version used it up)
-            float x[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-                float f = __fmaf_rn(__uint_as_float(v[j]), k_acc, bias_s[n0 + j]);
-                if (g.relu) f = (f < 0.f) ? 0.f : f;  // (NaN stays NaN, like torch.relu: an overflow upstream must reach the loss)
-                x[j] = f;
-            }
-            if (g.bits_in) {
-                const int i4 = n0 >> 6;
-                const uint32_t keep = i4 == 0 ? tile_bits.x : (i4 == 1 ? tile_bits.y : (i4 == 2 ? tile_bits.z : tile_bits.w));
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    if (!((keep >> j) & 1u)) x[j] = 0.f;
-            }
-            if (g.bits_out) {
-                // collected per unit and written ONCE after the column loop (one 16-byte store per thread and tile instead of four scattered
-                // 4-byte stores: the forward GEMMs of the training pass ran 37 us against 30 us for the same layer without the mask)
-                uint32_t positive = 0;
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    if (x[j] > 0.f) positive |= 1u << j;
-                const int i4 = n0 >> 6;
-                if (i4 == 0) out_bits.x = positive; else if (i4 == 1) out_bits.y = positive; else if (i4 == 2) out_bits.z = positive; else out_bits.w = positive;
-            }
-            if (g.mask && row_ok) {
-                const uint4* mrow = reinterpret_cast<const uint4*>(g.mask + (size_t)row * g.ld_mask + n0);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const uint4 mm = __ldg(mrow + q);
-                    const uint32_t w4[4] = {mm.x, mm.y, mm.z, mm.w};
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        const uint32_t bits = (e & 1) ? (w4[e >> 1] >> 16) : (w4[e >> 1] & 0xFFFFu);
-                        // (bf16 or fp16) > 0  <=>  sign bit clear and magnitude non-zero (NaN never occurs in a ReLU output)
-                        if ((bits & 0x8000u) || (bits & 0x7FFFu) == 0u) x[8 * q + e] = 0.f;
-                    }
-                }
-            }
-            if (row_ok && g.c_f32) {
-                float* crow = g.c_f32 + (size_t)row * g.ldc + n0;
-                if (n0 + 32 <= g.N && (g.ldc % 4 == 0)) {
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(crow + j) = make_float4(x[j], x[j + 1], x[j + 2], x[j + 3]);
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if (n0 + j < g.N) crow[j] = x[j];
-                }
-            }
-            if (g.c_planes && n0 < g.ldp) {
-                if (n0 + 32 > g.N) {  // ragged last chunk: columns [N, ldp) are written as zero
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if (n0 + j >= g.N) x[j] = 0.f;
-                }
-                // re-split (c_scale x) into P planes, two columns per word
-                uint32_t pw[P][16];
-                if (folded) {
-#pragma unroll
-                    for (int j = 0; j < 32; j += 2) {
-                        uint32_t w[P];
-                        F::split2(x[j], x[j + 1], w, amax);
-#pragma unroll
-                        for (int p = 0; p < P; ++p) pw[p][j / 2] = w[p];
-                    }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 32; j += 2) {
-                        uint32_t w[P];
-                        F::split2(x[j] * c_mul, x[j + 1] * c_mul, w, amax);
-#pragma unroll
-                        for (int p = 0; p < P; ++p) pw[p][j / 2] = w[p];
-                    }
-                }
-                // stage the warp's [32 rows x 32 cols] x P planes in shared memory (TMA SWIZZLE_64B pattern: 16-byte chunk index
-                // XOR ((row >> 1) & 3), bank-conflict free), then ONE bulk tensor store writes it out coalesced and asynchronously
-                if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // previous store has read the staging tile
-                __syncwarp();
-                uint8_t* st = my_stage + lane * 64;
-                const int sw = (lane >> 1) & 3;
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const int off = ((q ^ sw) << 4);
-#pragma unroll
-                    for (int p = 0; p < P; ++p)
-                        *reinterpret_cast<uint4*>(st + p * 2048 + off) = make_uint4(pw[p][4 * q], pw[p][4 * q + 1], pw[p][4 * q + 2], pw[p][4 * q + 3]);
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) {
-                    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(&tmC), "r"(g_smem_u32(my_stage)),
-                                 "r"(n0), "r"(row - lane), "r"(0)
-                                 : "memory");
-                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                }
-            }
-        };
-        uint32_t it = 0;
-        long long w_tfull = 0, busy = 0;
-        for (int u = unit; u < n_work; u += n_units, ++it) {
+        float acc[128];
+        uint32_t stage = 0, phase = 0;
+        long long w_full = 0, busy = 0;
+        long long* wc = g.stats ? &w_full : nullptr;
+        const long long t_begin = g.stats ? clock64() : 0;
+        for (int u = blockIdx.x; u < n_work; u += gridDim.x) {
             int tile, n_begin, n_cnt;
             unit_of(u, tile, n_begin, n_cnt);
-            const uint32_t as = SPLIT ? 0u : (it & 1u);
-            if (g.bits_in) {  // independent of the MMAs: in flight while this warp waits for the accumulator
-                const int prow = (tile * NCTA + (int)cta_rank) * kGemmBM + quad * 32 + lane;
-                tile_bits = prow < g.M ? __ldg(reinterpret_cast<const uint4*>(g.bits_in + (size_t)prow * 8 + half * 4)) : make_uint4(0u, 0u, 0u, 0u);
+#define MORL_UNIT(N_) \
+    case N_: mma_unit<FMT, N_, SPLIT>(acc, smA, smB, a_stage_bytes, b_stage_stride, n_kblk, full, empty, stage, phase, kStages, wg, lane, wc); break;
+            switch (n_cnt) {
+                MORL_UNIT(32) MORL_UNIT(64) MORL_UNIT(96) MORL_UNIT(128)
+                default:
+                    if constexpr (!SPLIT) {
+                        switch (n_cnt) {
+                            MORL_UNIT(160) MORL_UNIT(192) MORL_UNIT(224) MORL_UNIT(256)
+                            default: __trap();
+                        }
+                    } else {
+                        __trap();
+                    }
             }
-            const long long c0 = g.stats ? clock64() : 0;
-            g_mbar_wait(&tfull[as], SPLIT ? (it & 1u) : ((it >> 1) & 1u));
+#undef MORL_UNIT
             const long long c1 = g.stats ? clock64() : 0;
-            w_tfull += c1 - c0;
-            tc_fence_after();
-            const int row = (tile * NCTA + (int)cta_rank) * kGemmBM + quad * 32 + lane;
-            const bool row_ok = row < g.M;
-            const uint32_t t_row = tmem_base + as * 256u + ((uint32_t)(quad * 32) << 16);
-            uint32_t va[32], vb[32];
-            int n0 = 32 * half;  // accumulator column of the unit; the output column is n_begin + n0
-            if constexpr (SPLIT) {
-                // leading + correction accumulators: two TMEM loads per chunk, one correctly rounded add
-                while (n0 < n_cnt) {
-                    tc_ld32(t_row + (uint32_t)n0, va);
-                    tc_ld32(t_row + 256u + (uint32_t)n0, vb);
-                    tc_ld_wait();
+            const int rbase = tile * kGemmBM + wg * 64 + (warp & 3) * 16;
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) va[j] = __float_as_uint(__fadd_rn(__uint_as_float(va[j]), __uint_as_float(vb[j])));
-                    process(va, n_begin + n0, row, row_ok);
-                    n0 += 64;
-                }
-            } else {
-                // software pipeline over this warp's chunks n0 = 32*half, 32*half + 64, ...: the TMEM load of the next chunk is in
-                // flight while the current one is converted and stored
-                if (n0 < n_cnt) {
-                    tc_ld32(t_row + (uint32_t)n0, va);
-                    tc_ld_wait();
-                }
-                while (n0 < n_cnt) {
-                    const int n1 = n0 + 64;
-                    if (n1 < n_cnt) tc_ld32(t_row + (uint32_t)n1, vb);
-                    process(va, n_begin + n0, row, row_ok);
-                    tc_ld_wait();
-                    if (n1 >= n_cnt) break;
-                    const int n2 = n1 + 64;
-                    if (n2 < n_cnt) tc_ld32(t_row + (uint32_t)n2, va);
-                    process(vb, n_begin + n1, row, row_ok);
-                    tc_ld_wait();
-                    n0 = n2;
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if (NCTA == 2) mbar_arrive_remote(mapa_rank0(g_smem_u32(&tempty[as]))); else g_mbar_arrive(&tempty[as]);
-            }
-            if (g.bits_out && row_ok) {
-                // this thread's chunks of the unit: output columns n_begin + 32 half + 64 k < n_begin + n_cnt, i.e. words (n_begin >> 6) ...
-                uint32_t* dst = g.bits_out + (size_t)row * 8 + half * 4;
-                const int w0 = n_begin >> 6, w1 = (n_begin + n_cnt - 32 * half + 63) >> 6;  // [w0, w1) of the four words this thread owns
-                if (w0 == 0 && w1 == 4) {
-                    *reinterpret_cast<uint4*>(dst) = out_bits;
-                } else {
-                    const uint32_t wv[4] = {out_bits.x, out_bits.y, out_bits.z, out_bits.w};
+            for (int c = 0; c < (SPLIT ? 4 : 8); ++c) {
+                if (32 * c < n_cnt) {
+                    float a[16];
 #pragma unroll
-                    for (int q = 0; q < 4; ++q)
-                        if (q >= w0 && q < w1) dst[q] = wv[q];
+                    for (int j = 0; j < 16; ++j) a[j] = SPLIT ? __fadd_rn(acc[16 * c + j], acc[64 + 16 * c + j]) : acc[16 * c + j];
+                    epilogue_chunk<FMT>(a, n_begin + 32 * c, rbase, lane, e, &tmC, my_stage, amax);
                 }
             }
             if (g.stats) busy += clock64() - c1;
         }
-        if (g.stats && warp == 2 && lane == 0) {
-            atomicAdd(&g.stats[4], (unsigned long long)w_tfull);
-            atomicAdd(&g.stats[5], (unsigned long long)busy);
+        if (g.stats && warp == 0 && lane == 0) {
+            atomicAdd(&g.stats[0], (unsigned long long)w_full);
+            atomicAdd(&g.stats[1], (unsigned long long)(clock64() - t_begin));
+            atomicAdd(&g.stats[3], (unsigned long long)busy);
         }
         if (FMT == MORL_FMT_F16X2) note_overflow(amax);
         if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // all bulk stores of this warp have completed
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (NCTA == 2) cluster_sync_all();  // no CTA of a pair exits (or frees TMEM) while its peer can still signal it
-    if (warp == 1) {
-        tc_fence_after();
-        if (NCTA == 2)
-            asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
-        else
-            asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
-    }
 }
 
 // =================================================================================================================
-// CHAIN kernel: several dense hidden layers of one or two networks in ONE persistent launch (CTA pairs, f16x2 / bf16x3 planes, N = 256 wide
-// layers).  A layer's output rows depend only on the same rows of its input, so a CTA pair can take one of its 256-row tiles through ALL
-// layers: the tile it stores for layer l is the tile it loads for layer l+1 a few units later -- by then still in the 126 MB L2, so only the
-// first layer's input is read from HBM (the per-layer launches re-read every intermediate activation from HBM: 6 x 134 MB for the two
-// no-grad passes of an Envelope update against 6 x 67 MB + 2 x 67 MB here), and the launch prologue / drain is paid once instead of per
-// layer.  Work of a pair: its tiles in groups of `lanes / n_chains`; per group, for every layer, one unit per LANE (lane = (chain, tile
+// CHAIN kernel: several dense hidden layers of one or two networks in ONE persistent launch (f16x2 / bf16x3 planes, N = 256 wide
+// layers).  A layer's output rows depend only on the same rows of its input, so a CTA can take one of its 128-row tiles through ALL
+// layers: the tile it stores for layer l is the tile it loads for layer l+1 a few units later -- by then still in the 50 MB L2, so only the
+// first layer's input is read from HBM, and the launch prologue / drain is paid once instead of per layer.  Work of a CTA: its tiles in
+// groups of `lanes / n_chains`; per group, for every layer, one unit per LANE (lane = (chain, tile
 // of the group)): four lanes keep the dependency distance at four units (unit (l, lane) needs the stores of unit (l-1, lane)), so the
-// producer never waits for the epilogue that has just finished.  Same roles, barriers and arithmetic as gemm_planes_kernel<2, FMT, 0>
-// (bit-identical outputs: tests/test_gemm_gpu.py); additional barrier stored[lane]: the epilogue warps of a CTA arrive once their bulk
-// stores of the unit have COMPLETED, the producer of the same CTA waits for it before loading the next layer of that lane.
+// producer never waits for the epilogue that has just finished.  Same roles, barriers and arithmetic as gemm_planes_kernel<FMT, 0>
+// (bit-identical outputs: tests/test_gemm_gpu.py); additional barrier stored[lane]: the consumer warps arrive once their bulk
+// stores of the unit have COMPLETED, the producer waits for it before loading the next layer of that lane.
 // =================================================================================================================
 constexpr int kChainMaxJobs = 8;   // chains x layers
 constexpr int kChainLanes = 4;
 
 struct alignas(64) ChainMaps {
     CUtensorMap A[kChainMaxJobs];  // load map of the INPUT of job (chain c, layer l): [P][M][K], box P x 128 x BK
-    CUtensorMap B[kChainMaxJobs];  // weight planes of the job: [P][256][K], box P x 128 x BK (each CTA of the pair stages half of the rows)
-    CUtensorMap C[kChainMaxJobs];  // store map of the OUTPUT of the job: [P][M][256], box P x 32 x 32 (64-byte swizzle)
+    CUtensorMap B[kChainMaxJobs];  // weight planes of the job: [P][256][K], box 1 x 32 x BK
+    CUtensorMap C[kChainMaxJobs];  // store map of the OUTPUT of the job: [P][M][256], box P x 16 x 32 (64-byte swizzle)
 };
 
 struct ChainArgs {
@@ -546,43 +472,38 @@ template <int FMT>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
     using F = PlaneFmt<FMT>;
-    using L = KPlan<2, FMT>;
+    using L = KPlan<FMT>;
     constexpr int P = F::P;
     constexpr int BK = F::BK;
     constexpr int BN = 256;
     constexpr int kMaxStages = L::kMaxStages;
     constexpr uint32_t ROWB = L::kRowB;
-    const int kStages = g.n_stages;
+    const uint32_t kStages = (uint32_t)g.n_stages;
     extern __shared__ uint8_t gsmem_raw[];
     uint8_t* gsmem = gsmem_raw + ((1024u - (g_smem_u32(gsmem_raw) & 1023u)) & 1023u);
     constexpr uint32_t a_stage_bytes = L::kAStage;
     constexpr uint32_t b_stage_bytes = L::kBStage;
     uint8_t* smA = gsmem;
-    uint8_t* smB = gsmem + (uint32_t)kStages * a_stage_bytes;
+    uint8_t* smB = gsmem + kStages * a_stage_bytes;
     uint8_t* stage_c = gsmem + L::kOffC;
     uint64_t* full = reinterpret_cast<uint64_t*>(gsmem + L::kOffBar);
     uint64_t* empty = full + kMaxStages;
-    uint64_t* tfull = empty + kMaxStages;
-    uint64_t* tempty = tfull + 2;
-    uint64_t* stored = tempty + 2;  // [kChainLanes]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(stored + kChainLanes);
-    float* bias_s = reinterpret_cast<float*>(gsmem + L::kOffBias);  // [256], refilled per unit by the epilogue warps
+    uint64_t* stored = empty + kMaxStages;  // [kChainLanes]
+    float* bias_s = reinterpret_cast<float*>(gsmem + L::kOffBias);  // [256], refilled per unit by the consumer warps
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const uint32_t cta_rank = cluster_ctarank();
-    const int unit = blockIdx.x / 2, n_units = gridDim.x / 2;
-    const int n_tiles = (g.M + 2 * kGemmBM - 1) / (2 * kGemmBM);
+    const int unit = blockIdx.x, n_units = gridDim.x;
+    const int n_tiles = (g.M + kGemmBM - 1) / kGemmBM;
     const int n_kblk_full = g.K / BK, n_kblk_first = g.k_first / BK;
     const int tiles_per_group = kChainLanes / g.n_chains;  // lanes of a group: (tile of the group) x (chain)
-    // Tile t of chain c goes to pair (t + offset_c) mod n_units with a DIFFERENT rotation per chain: 256 tiles on 74 pairs leave 34 pairs with
-    // four tiles and 40 with three; with both chains on the same pairs the launch lasted 4/3.46 of the balanced time (the 3-tile pairs idled
-    // for a quarter of it), rotated by half the pairs every pair gets 4 + 3 or 3 + 3.
+    // Tile t of chain c goes to CTA (t + offset_c) mod n_units with a DIFFERENT rotation per chain: when the tiles do not divide evenly, both
+    // chains on the same CTAs would give some CTAs two extra tiles and others none; rotated by half the grid the remainders spread.
     const int cu0 = unit, cu1 = (unit + n_units / 2) % n_units;
     const int mt0 = cu0 < n_tiles ? (n_tiles - cu0 + n_units - 1) / n_units : 0;
     const int mt1 = g.n_chains > 1 ? (cu1 < n_tiles ? (n_tiles - cu1 + n_units - 1) / n_units : 0) : 0;
     const int n_groups = ((mt0 > mt1 ? mt0 : mt1) + tiles_per_group - 1) / tiles_per_group;
-    // unit (group gi, layer l, lane ln) -> (job, tile) or tile = -1 (no such tile for this pair)
+    // unit (group gi, layer l, lane ln) -> (job, tile) or tile = -1 (no such tile for this CTA)
     auto unit_of = [&](int gi, int l, int ln, int& job, int& tile) {
         const int c = ln % g.n_chains, ti = gi * tiles_per_group + ln / g.n_chains;
         job = c * g.n_layers + l;
@@ -590,32 +511,20 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
     };
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kStages; ++s) {
+        for (uint32_t s = 0; s < kStages; ++s) {
             g_mbar_init(&full[s], 1);
-            g_mbar_init(&empty[s], 1);
+            g_mbar_init(&empty[s], 8);
         }
-        for (int s = 0; s < 2; ++s) {
-            g_mbar_init(&tfull[s], 1);
-            g_mbar_init(&tempty[s], 16);  // one arrival per epilogue warp of both CTAs, on the leader's barrier
-        }
-        for (int s = 0; s < kChainLanes; ++s) g_mbar_init(&stored[s], 8);  // the 8 epilogue warps of THIS CTA
+        for (int s = 0; s < kChainLanes; ++s) g_mbar_init(&stored[s], 8);  // the 8 consumer warps
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(g_smem_u32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
     }
     if (g.pdl) {
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
         asm volatile("griddepcontrol.wait;" ::: "memory");
     }
-    tc_fence_before();
     __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ================= TMA producer =================
         if (lane == 0) {
             uint32_t stage = 0, phase = 0;
@@ -627,196 +536,78 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
                         unit_of(gi, l, ln, job, tile);
                         if (tile < 0) continue;
                         if (l > 0) {
-                            // the input tile of this unit is the output tile of the lane's previous unit: wait until THIS CTA's stores of
+                            // the input tile of this unit is the output tile of the lane's previous unit: wait until the stores of
                             // it have completed (completion number done_on_lane[ln] of stored[ln])
                             g_mbar_wait(&stored[ln], (done_on_lane[ln] - 1u) & 1u);
                             asm volatile("fence.proxy.async.global;" ::: "memory");
                         }
                         ++done_on_lane[ln];
-                        const int row0 = (tile * 2 + (int)cta_rank) * kGemmBM;
+                        const int row0 = tile * kGemmBM;
                         const int n_kblk = l == 0 ? n_kblk_first : n_kblk_full;
                         for (int kb = 0; kb < n_kblk; ++kb) {
                             g_mbar_wait(&empty[stage], phase ^ 1u);
-                            if (cta_rank == 0) g_mbar_expect_tx(&full[stage], 2u * (a_stage_bytes + b_stage_bytes));
-                            const uint32_t lbar = mapa_rank0(g_smem_u32(&full[stage]));
-                            tma_load_3d_pair(smA + stage * a_stage_bytes, &maps.A[job], lbar, kb * BK, row0, 0);
-                            tma_load_3d_pair(smB + stage * b_stage_bytes, &maps.B[job], lbar, kb * BK, (int)cta_rank * (BN / 2), 0);
-                            if (++stage == (uint32_t)kStages) {
+                            g_mbar_expect_tx(&full[stage], a_stage_bytes + b_stage_bytes);
+                            tma_load_3d(smA + stage * a_stage_bytes, &maps.A[job], &full[stage], kb * BK, row0, 0);
+                            for (int p = 0; p < P; ++p)
+                                for (int r = 0; r < BN; r += kGemmBoxN)
+                                    tma_load_3d(smB + stage * b_stage_bytes + (uint32_t)(p * BN + r) * ROWB, &maps.B[job], &full[stage], kb * BK, r, p);
+                            if (++stage == kStages) {
                                 stage = 0;
                                 phase ^= 1u;
                             }
                         }
-                    }
-        }
-    } else if (warp == 1) {
-        // ================= MMA issuer (leader CTA only) =================
-        if (lane == 0 && cta_rank == 0) {
-            constexpr uint32_t idesc = (1u << 4) | F::kIdescAB | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)((kGemmBM * 2) >> 4) << 24);
-            constexpr uint32_t a_plane = kGemmBM * ROWB;
-            constexpr uint32_t b_plane = (uint32_t)(BN / 2) * ROWB;
-            uint32_t stage = 0, phase = 0, it = 0;
-            for (int gi = 0; gi < n_groups; ++gi)
-                for (int l = 0; l < g.n_layers; ++l)
-                    for (int ln = 0; ln < kChainLanes; ++ln) {
-                        int job, tile;
-                        unit_of(gi, l, ln, job, tile);
-                        if (tile < 0) continue;
-                        const uint32_t as = it & 1u;
-                        g_mbar_wait(&tempty[as], ((it >> 1) & 1u) ^ 1u);
-                        tc_fence_after();
-                        const uint32_t d_tmem = tmem_base + as * 256u;
-                        const int n_kblk = l == 0 ? n_kblk_first : n_kblk_full;
-                        for (int kb = 0; kb < n_kblk; ++kb) {
-                            g_mbar_wait(&full[stage], phase);
-                            tc_fence_after();
-                            const uint32_t a0 = g_smem_u32(smA + stage * a_stage_bytes);
-                            const uint32_t b0 = g_smem_u32(smB + stage * b_stage_bytes);
-#pragma unroll
-                            for (int ks = 0; ks < BK / 16; ++ks) {
-#pragma unroll
-                                for (int t = 0; t < F::NPROD; ++t) {
-                                    const uint64_t ad = make_desc_k<ROWB>(a0 + F::pa(t) * a_plane + ks * 32);
-                                    const uint64_t bd = make_desc_k<ROWB>(b0 + F::pb(t) * b_plane + ks * 32);
-                                    tc_mma_bf16_pair(d_tmem, ad, bd, idesc, (kb | ks | t) != 0 ? 1u : 0u);
-                                }
-                            }
-                            tc_commit_pair(&empty[stage]);
-                            if (++stage == (uint32_t)kStages) {
-                                stage = 0;
-                                phase ^= 1u;
-                            }
-                        }
-                        tc_commit_pair(&tfull[as]);
-                        ++it;
                     }
         }
     } else {
-        // ================= epilogue warps (2..9) =================
-        const int quad = warp & 3;
-        const int half = (warp - 2) >> 2;
-        const int et = threadIdx.x - 64;  // 0..255 among the epilogue threads
-        uint8_t* my_stage = stage_c + (warp - 2) * L::kStageC;
+        // ================= consumer warpgroups (warps 0..7) =================
+        const int wg = warp >> 2;
+        uint8_t* my_stage = stage_c + warp * L::kStageC;
         const float s_act = ld_scale(g.a_scale);
         float amax = 0.f;
-        uint32_t it = 0;
+        float acc[128];
+        uint32_t stage = 0, phase = 0;
         for (int gi = 0; gi < n_groups; ++gi)
             for (int l = 0; l < g.n_layers; ++l)
                 for (int ln = 0; ln < kChainLanes; ++ln) {
                     int job, tile;
                     unit_of(gi, l, ln, job, tile);
                     if (tile < 0) continue;
-                    const uint32_t as = it & 1u;
-                    // this unit's bias (times the folded output scale) into shared memory: every epilogue warp has left the previous unit
+                    // this unit's bias (times the folded output scale) into shared memory: every consumer warp has left the previous unit
                     asm volatile("bar.sync 1, 256;" ::: "memory");
-                    bias_s[et] = (g.bias[job] ? __ldg(g.bias[job] + et) : 0.f) * s_act;
+                    bias_s[threadIdx.x] = (g.bias[job] ? __ldg(g.bias[job] + threadIdx.x) : 0.f) * s_act;
                     asm volatile("bar.sync 1, 256;" ::: "memory");
+                    EpiArgs e;
+                    e.M = g.M; e.N = BN;
                     // x * s_act = acc * (s_act / (s_act * sB)) + s_act * bias  (powers of two: exact), as gemm_planes_kernel's folded epilogue
-                    const float k_acc = s_act / (s_act * ld_scale(g.b_scale[job]));
-                    uint32_t* bits_out = g.bits_out[job];
-                    const uint32_t* bits_in = g.bits_in[job];
-                    uint4 out_bits = make_uint4(0u, 0u, 0u, 0u);
-                    const int row = (tile * 2 + (int)cta_rank) * kGemmBM + quad * 32 + lane;
-                    const bool row_ok = row < g.M;
-                    uint4 in_bits = make_uint4(0u, 0u, 0u, 0u);  // (independent of the MMAs: in flight while this warp waits for the accumulator)
-                    if (bits_in && row_ok) in_bits = __ldg(reinterpret_cast<const uint4*>(bits_in + (size_t)row * 8 + half * 4));
-                    g_mbar_wait(&tfull[as], (it >> 1) & 1u);
-                    tc_fence_after();
-                    const uint32_t t_row = tmem_base + as * 256u + ((uint32_t)(quad * 32) << 16);
-                    uint32_t va[32], vb[32];
-                    auto process = [&](const uint32_t (&v)[32], int n0) {
-                        float x[32];
+                    e.k_acc = s_act / (s_act * ld_scale(g.b_scale[job]));
+                    e.c_mul = 1.0f;
+                    e.bias_s = bias_s; e.relu = g.relu; e.bits_in = g.bits_in[job]; e.bits_out = g.bits_out[job]; e.mask = nullptr; e.ld_mask = 0;
+                    e.c_f32 = nullptr; e.ldc = 0; e.planes = 1; e.ldp = BN;
+                    mma_unit<FMT, BN, 0>(acc, smA, smB, a_stage_bytes, b_stage_bytes, l == 0 ? n_kblk_first : n_kblk_full, full, empty, stage, phase, kStages,
+                                         wg, lane, nullptr);
+                    const int rbase = tile * kGemmBM + wg * 64 + (warp & 3) * 16;
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            float f = __fmaf_rn(__uint_as_float(v[j]), k_acc, bias_s[n0 + j]);
-                            if (g.relu) f = (f < 0.f) ? 0.f : f;  // (NaN stays NaN)
-                            x[j] = f;
-                        }
-                        if (bits_in) {
-                            const int i4 = n0 >> 6;
-                            const uint32_t keep = i4 == 0 ? in_bits.x : (i4 == 1 ? in_bits.y : (i4 == 2 ? in_bits.z : in_bits.w));
+                    for (int c = 0; c < 8; ++c) {
+                        float a[16];
 #pragma unroll
-                            for (int j = 0; j < 32; ++j)
-                                if (!((keep >> j) & 1u)) x[j] = 0.f;
-                        }
-                        if (bits_out) {
-                            uint32_t positive = 0;
-#pragma unroll
-                            for (int j = 0; j < 32; ++j)
-                                if (x[j] > 0.f) positive |= 1u << j;
-                            const int i4 = n0 >> 6;
-                            if (i4 == 0) out_bits.x = positive; else if (i4 == 1) out_bits.y = positive; else if (i4 == 2) out_bits.z = positive; else out_bits.w = positive;
-                        }
-                        uint32_t pw[P][16];
-#pragma unroll
-                        for (int j = 0; j < 32; j += 2) {
-                            uint32_t w[P];
-                            F::split2(x[j], x[j + 1], w, amax);
-#pragma unroll
-                            for (int p = 0; p < P; ++p) pw[p][j / 2] = w[p];
-                        }
-                        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                        __syncwarp();
-                        uint8_t* st = my_stage + lane * 64;
-                        const int sw = (lane >> 1) & 3;
-#pragma unroll
-                        for (int q = 0; q < 4; ++q) {
-                            const int off = ((q ^ sw) << 4);
-#pragma unroll
-                            for (int p = 0; p < P; ++p)
-                                *reinterpret_cast<uint4*>(st + p * 2048 + off) = make_uint4(pw[p][4 * q], pw[p][4 * q + 1], pw[p][4 * q + 2], pw[p][4 * q + 3]);
-                        }
-                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                        __syncwarp();
-                        if (lane == 0) {
-                            asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(&maps.C[job]),
-                                         "r"(g_smem_u32(my_stage)), "r"(n0), "r"(row - lane), "r"(0)
-                                         : "memory");
-                            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                        }
-                    };
-                    int n0 = 32 * half;
-                    tc_ld32(t_row + (uint32_t)n0, va);
-                    tc_ld_wait();
-                    while (n0 < BN) {
-                        const int n1 = n0 + 64;
-                        if (n1 < BN) tc_ld32(t_row + (uint32_t)n1, vb);
-                        process(va, n0);
-                        tc_ld_wait();
-                        if (n1 >= BN) break;
-                        const int n2 = n1 + 64;
-                        if (n2 < BN) tc_ld32(t_row + (uint32_t)n2, va);
-                        process(vb, n1);
-                        tc_ld_wait();
-                        n0 = n2;
+                        for (int j = 0; j < 16; ++j) a[j] = acc[16 * c + j];
+                        epilogue_chunk<FMT>(a, 32 * c, rbase, lane, e, &maps.C[job], my_stage, amax);
                     }
-                    tc_fence_before();
+                    // the lane's next layer loads what this unit stored (bit masks included): signal once the bulk stores of this warp have completed
                     __syncwarp();
-                    if (lane == 0) mbar_arrive_remote(mapa_rank0(g_smem_u32(&tempty[as])));
-                    if (bits_out && row_ok) *reinterpret_cast<uint4*>(bits_out + (size_t)row * 8 + half * 4) = out_bits;
-                    // the lane's next layer loads what this unit stored: signal once the bulk stores of this warp have completed
                     if (lane == 0) {
                         asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
                         g_mbar_arrive(&stored[ln]);
                     }
-                    ++it;
                 }
         if (FMT == MORL_FMT_F16X2) note_overflow(amax);
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
     }
 }
 
 // =================================================================================================================
 // MN-major split-K variant: weight gradients  dW[n, k] = sum_m G[m, n] * H[m, k]  (reduction over the 65,536 batch rows).
 // Both operands are the row-major plane tensors the forward/backward GEMMs already produced, read "MN-major" (the MMA's M / N
-// index is the contiguous one), 128-byte swizzle:  A = G^T (M_mma = n, 128 per CTA), B = H^T (N_mma = k <= 256), K_mma = m.
+// index is the contiguous one), 128-byte swizzle:  A = G^T (M_mma = n, 128 per CTA: 64 per warpgroup), B = H^T (N_mma = k <= 256), K_mma = m.
 // One CTA per (128-row block of n, split s of the m range); fp32 partial tiles are summed by reduce_partials_kernel
 // (deterministic, no atomics), which also removes the operand scales.
 // =================================================================================================================
@@ -829,8 +620,7 @@ __device__ __forceinline__ uint64_t make_desc_mn_sw128(uint32_t smem_addr, uint3
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;  // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;  // SWIZZLE_128B
     return d;
 }
 
@@ -843,13 +633,50 @@ struct GemmMnArgs {
     float* colsum_partial;  // [S][n_tiles*128] or nullptr: per-split column sums of G (bias gradient), fused as G^T . ones
 };
 
-// MC = 1 (two column tiles, NB = 256): the two CTAs of a split (column tiles 0 and 1: consecutive blocks) form a CLUSTER; each loads its own
-// 128 G columns and HALF of the H chunks, multicast to both CTAs, so H crosses the L2 -> SM path once per split instead of twice.  The kernel
-// (hypothesis: 67 MB of G + 2 x 67 MB of H per launch through that path at ~6.5 TB/s would explain the 31 us measured.  Built, correct, and
-// measured: no gain, see the launcher -- opt-in.)
-// A stage may be refilled only when BOTH CTAs have consumed it: every MMA commit arrives on the stage's empty barrier of both CTAs.
-template <int FMT, int MC>
-__global__ void __launch_bounds__(192, 1)
+// the K loop of one consumer warpgroup: acc[64 x NB] += G_chunk^T . H over the stages; cs[64 x 16] += G_chunk^T . ones
+template <int FMT, int NB>
+__device__ __forceinline__ void mma_mn_unit(float (&acc)[128], float (&cs)[8], bool colsum, uint8_t* smA, uint8_t* smB, uint32_t a_stage, uint32_t b_stage,
+                                            uint32_t chunk_bytes, uint64_t ones_desc, int n_kblk, uint64_t* full, uint64_t* empty, int wg, int lane) {
+    using F = PlaneFmt<FMT>;
+    constexpr int P = F::P;
+    constexpr uint32_t plane = kMnKT * 128u;  // 4 KB: one plane of one chunk
+    uint32_t stage = 0, phase = 0, prev = 0;
+    for (int kb = 0; kb < n_kblk; ++kb) {
+        g_mbar_wait(&full[stage], phase);
+        wgmma_fence();
+        const uint32_t a0 = g_smem_u32(smA + stage * a_stage) + (uint32_t)wg * chunk_bytes;  // this warpgroup's 64 columns of G
+        const uint32_t b0 = g_smem_u32(smB + stage * b_stage);
+#pragma unroll
+        for (int ks = 0; ks < kMnKT / 16; ++ks) {
+#pragma unroll
+            for (int t = 0; t < F::NPROD; ++t) {
+                const uint64_t ad = make_desc_mn_sw128(a0 + F::pa(t) * plane + ks * 2048u, chunk_bytes);
+                const uint64_t bd = make_desc_mn_sw128(b0 + F::pb(t) * plane + ks * 2048u, chunk_bytes);
+                Wgmma<NB>::template mma<FMT, 1, 1>(acc, ad, bd, (kb | ks | t) != 0 ? 1u : 0u);
+            }
+            if (colsum) {  // (G_{P-1} + ... + G_0)^T . ones -> 16 identical columns
+#pragma unroll
+                for (int pl = P - 1; pl >= 0; --pl)
+                    Wgmma<16>::template mma<FMT, 1, 1>(cs, make_desc_mn_sw128(a0 + pl * plane + ks * 2048u, chunk_bytes), ones_desc,
+                                                       (kb | ks | (P - 1 - pl)) != 0 ? 1u : 0u);
+            }
+        }
+        wgmma_commit();
+        if (kb > 0) {
+            wgmma_wait<1>();
+            if (lane == 0) g_mbar_arrive(&empty[prev]);
+        }
+        prev = stage;
+        if (++stage == (uint32_t)F::kStagesMn) {
+            stage = 0;
+            phase ^= 1u;
+        }
+    }
+    wgmma_wait<0>();
+}
+
+template <int FMT>
+__global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_planes_mn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmMnArgs g) {
     using F = PlaneFmt<FMT>;
     constexpr int P = F::P;
@@ -866,11 +693,9 @@ gemm_planes_mn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     uint8_t* smB = gsmem + kStages * a_stage;
     uint64_t* full = reinterpret_cast<uint64_t*>(smB + kStages * b_stage);
     uint64_t* empty = full + kStages;
-    uint64_t* tfull = empty + kStages;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tfull + 1);
     // 4 KB of 1.0: the B operand of the fused bias-gradient product  colsum(G) = G^T . ones  (N = 16; every element is 1,
     // so the swizzle pattern is irrelevant)
-    uint8_t* ones_b = reinterpret_cast<uint8_t*>(tmem_slot + 4);
+    uint8_t* ones_b = reinterpret_cast<uint8_t*>(empty + kStages);
     uint32_t* ones = reinterpret_cast<uint32_t*>(ones_b + ((1024u - (g_smem_u32(ones_b) & 1023u)) & 1023u));
     for (int t = threadIdx.x; t < 1024; t += blockDim.x) ones[t] = F::kOnes2;
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -885,23 +710,14 @@ gemm_planes_mn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     if (threadIdx.x == 0) {
         for (int s = 0; s < kStages; ++s) {
             g_mbar_init(&full[s], 1);
-            g_mbar_init(&empty[s], MC ? 2 : 1);  // MC: released by the MMA commits of both CTAs of the cluster
+            g_mbar_init(&empty[s], 8);  // one arrival per consumer warp
         }
-        g_mbar_init(tfull, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {  // 256 accumulator columns + 16 for the fused column sums (allocation granularity: power of two)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(g_smem_u32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    if (MC) cluster_sync_all();  // the peer's barriers exist before any multicast copy / remote arrive targets them
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    pdl_enter();  // (nothing above reads or writes global memory: barriers, the tile of ones and the TMEM allocation overlap the predecessor)
+    pdl_enter();  // (nothing above reads or writes global memory: barriers and the tile of ones overlap the predecessor)
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             uint32_t stage = 0, phase = 0;
             for (int kb = 0; kb < n_kblk; ++kb) {
@@ -909,89 +725,38 @@ gemm_planes_mn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                 g_mbar_expect_tx(&full[stage], (2u + (uint32_t)nb_chunks) * chunk_bytes);
                 const int m0 = m_begin + kb * kMnKT;
                 for (int c = 0; c < 2; ++c) tma_load_3d(smA + stage * a_stage + c * chunk_bytes, &tmA, &full[stage], nt * 128 + c * 64, m0, 0);
-                if (MC) {
-                    // this CTA fetches H chunks 2 nt, 2 nt + 1 for BOTH CTAs (same shared-memory offset and barrier offset in each); the other
-                    // two chunks arrive from the peer's multicast -- every full barrier still counts 2 + 4 chunks
-                    for (int c = 2 * nt; c < 2 * nt + 2; ++c)
-                        tma_load_3d_multicast(smB + stage * b_stage + c * chunk_bytes, &tmB, &full[stage], c * 64, m0, 0, (uint16_t)3);
-                } else {
-                    for (int c = 0; c < nb_chunks; ++c) tma_load_3d(smB + stage * b_stage + c * chunk_bytes, &tmB, &full[stage], c * 64, m0, 0);
-                }
+                for (int c = 0; c < nb_chunks; ++c) tma_load_3d(smB + stage * b_stage + c * chunk_bytes, &tmB, &full[stage], c * 64, m0, 0);
                 if (++stage == kStages) {
                     stage = 0;
                     phase ^= 1u;
                 }
             }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // D=f32, A/B of the plane type, both MN-major, N = NB, M = 128
-            const uint32_t idesc = (1u << 4) | F::kIdescAB | (1u << 15) | (1u << 16) | ((uint32_t)(g.NB >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            const uint32_t idesc_ones = (1u << 4) | F::kIdescAB | (1u << 15) | (1u << 16) | ((uint32_t)(16 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            const uint64_t ones_desc = make_desc_mn_sw128(g_smem_u32(ones), chunk_bytes);
-            constexpr uint32_t plane = kMnKT * 128u;  // 4 KB: one plane of one chunk
-            uint32_t stage = 0, phase = 0;
-            for (int kb = 0; kb < n_kblk; ++kb) {
-                g_mbar_wait(&full[stage], phase);
-                tc_fence_after();
-                const uint32_t a0 = g_smem_u32(smA + stage * a_stage);
-                const uint32_t b0 = g_smem_u32(smB + stage * b_stage);
-#pragma unroll
-                for (int ks = 0; ks < kMnKT / 16; ++ks) {
-#pragma unroll
-                    for (int t = 0; t < F::NPROD; ++t) {
-                        const uint64_t ad = make_desc_mn_sw128(a0 + F::pa(t) * plane + ks * 2048u, chunk_bytes);
-                        const uint64_t bd = make_desc_mn_sw128(b0 + F::pb(t) * plane + ks * 2048u, chunk_bytes);
-                        tc_mma_bf16(tmem_base, ad, bd, idesc, (kb | ks | t) != 0 ? 1u : 0u);
-                    }
-                    if (g.colsum_partial) {  // (G_{P-1} + ... + G_0)^T . ones -> 16 identical columns at TMEM column 256
-#pragma unroll
-                        for (int pl = P - 1; pl >= 0; --pl)
-                            tc_mma_bf16(tmem_base + 256u, make_desc_mn_sw128(a0 + pl * plane + ks * 2048u, chunk_bytes), ones_desc, idesc_ones,
-                                        (kb | ks | (P - 1 - pl)) != 0 ? 1u : 0u);
-                    }
-                }
-                if (MC) tc_commit_mc(&empty[stage]); else tc_commit(&empty[stage]);
-                if (++stage == kStages) {
-                    stage = 0;
-                    phase ^= 1u;
-                }
-            }
-            tc_commit(tfull);
         }
     } else {
-        const int quad = warp & 3;
-        g_mbar_wait(tfull, 0);
-        tc_fence_after();
-        const int row = nt * 128 + quad * 32 + lane;  // output row (n)
-        float* prow = g.partial + ((size_t)split * g.n_tiles * 128 + row) * g.NB;
-        const uint32_t t_row = tmem_base + ((uint32_t)(quad * 32) << 16);
-        for (int n0 = 0; n0 < g.NB; n0 += 32) {
-            uint32_t v[32];
-            tc_ld32(t_row + (uint32_t)n0, v);
-            tc_ld_wait();
-            if (n_kblk > 0) {
+        const int wg = warp >> 2, l4 = lane & 3;
+        float acc[128], cs[8];
 #pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                    *reinterpret_cast<float4*>(prow + n0 + j) = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-            } else {
+        for (int i = 0; i < 128; ++i) acc[i] = 0.f;  // (a split without rows writes zeros)
 #pragma unroll
-                for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(prow + n0 + j) = make_float4(0.f, 0.f, 0.f, 0.f);
-            }
+        for (int i = 0; i < 8; ++i) cs[i] = 0.f;
+        const uint64_t ones_desc = make_desc_mn_sw128(g_smem_u32(ones), chunk_bytes);
+        const bool colsum = g.colsum_partial != nullptr;
+#define MORL_UNIT(N_) \
+    case N_: mma_mn_unit<FMT, N_>(acc, cs, colsum, smA, smB, a_stage, b_stage, chunk_bytes, ones_desc, n_kblk, full, empty, wg, lane); break;
+        switch (g.NB) {
+            MORL_UNIT(64) MORL_UNIT(128) MORL_UNIT(192) MORL_UNIT(256)
+            default: __trap();
         }
-        if (g.colsum_partial) {
-            uint32_t v[32];
-            tc_ld32(t_row + 256u, v);
-            tc_ld_wait();
-            g.colsum_partial[(size_t)split * g.n_tiles * 128 + row] = n_kblk > 0 ? __uint_as_float(v[0]) : 0.f;
+#undef MORL_UNIT
+        const int row = nt * 128 + wg * 64 + (warp & 3) * 16 + (lane >> 2);  // output row (n); this thread also holds row + 8
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            float* prow = g.partial + ((size_t)split * g.n_tiles * 128 + row + 8 * h) * g.NB + 2 * l4;
+#pragma unroll
+            for (int j = 0; j < 32; ++j)
+                if (8 * j < g.NB) *reinterpret_cast<float2*>(prow + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+            if (colsum && l4 == 0) g.colsum_partial[(size_t)split * g.n_tiles * 128 + row + 8 * h] = cs[2 * h];
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (MC) cluster_sync_all();  // no CTA exits while its peer may still multicast into it or arrive on its barriers
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
     }
 }
 
@@ -1571,6 +1336,12 @@ static int make_plane_map_mn(CUtensorMap* map, int fmt, const void* base, int ro
     return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
+// CTAs of a split-K weight-gradient launch (one per SM); morl_gemm_mn_workspace_bytes and the launcher must agree on it
+static inline int mn_sm_count() {
+    const int n = morl_device_sm_count();
+    return n > 0 && n <= 256 ? n : 132;
+}
+
 static inline bool fmt_ok(int fmt) { return fmt == MORL_FMT_BF16X3 || fmt == MORL_FMT_F16X2; }
 
 }  // namespace morl
@@ -1596,7 +1367,7 @@ extern "C" int morl_amax_scale_f32(const float* src, long long n, int target_exp
     MORL_REQUIRE(src && scale_out && workspace, MORL_ERR_NULL, "morl_amax_scale_f32: NULL pointer argument");
     MORL_REQUIRE(n > 0 && target_exp >= -14 && target_exp <= 15, MORL_ERR_SHAPE, "morl_amax_scale_f32: bad n=%lld / target_exp=%d", n, target_exp);
     long long blocks = (n / 4 + 255) / 256;
-    if (blocks > 148) blocks = 148;
+    if (blocks > 132) blocks = 132;
     if (blocks < 1) blocks = 1;
     launch_k(amax_scale_kernel, dim3((int)blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), src, n, target_exp, scale_out, static_cast<unsigned int*>(workspace));
     return check_launch("morl_amax_scale_f32");
@@ -1605,7 +1376,7 @@ extern "C" int morl_amax_scale_f32(const float* src, long long n, int target_exp
 extern "C" size_t morl_gemm_mn_workspace_bytes(int M, int a_cols, int b_cols) {
     if (M <= 0 || a_cols <= 0 || b_cols <= 0) return 0;
     const int n_tiles = (a_cols + 127) / 128;
-    int S = 148 / n_tiles;
+    int S = morl::mn_sm_count() / n_tiles;
     if (S < 1) S = 1;
     int rps = ((M + S - 1) / S + 31) / 32 * 32;
     S = (M + rps - 1) / rps;
@@ -1624,7 +1395,7 @@ extern "C" int morl_gemm_planes_mn_f32(int fmt, const void* g_planes, long long 
                  "morl_gemm_planes_mn_f32: plane row lengths must be multiples of 64 (ldg=%d ldh=%d), ldh <= 256", ldg, ldh);
     const int n_tiles = (g_cols + 127) / 128;
     MORL_REQUIRE(n_tiles * 128 <= ldg || ldg % 128 == 0 || n_tiles * 128 - ldg <= 64, MORL_ERR_UNSUPPORTED, "morl_gemm_planes_mn_f32: ldg=%d", ldg);
-    int S = 148 / n_tiles;
+    int S = morl::mn_sm_count() / n_tiles;
     if (S < 1) S = 1;
     const int rps = ((M + S - 1) / S + 31) / 32 * 32;
     S = (M + rps - 1) / rps;
@@ -1636,43 +1407,17 @@ extern "C" int morl_gemm_planes_mn_f32(int fmt, const void* g_planes, long long 
     MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "morl_gemm_planes_mn_f32: cuTensorMapEncodeTiled(H) failed (%d)", rc);
     GemmMnArgs g;
     g.M = M; g.n_tiles = n_tiles; g.NB = NB; g.rows_per_split = rps; g.partial = static_cast<float*>(workspace);
-    g.colsum_partial = colsum_out ? g.partial + (size_t)S * n_tiles * 128 * NB : nullptr;  // S * n_tiles * 128 <= 148 * 128 floats < 256 KB tail
+    g.colsum_partial = colsum_out ? g.partial + (size_t)S * n_tiles * 128 * NB : nullptr;  // S * n_tiles * 128 <= 256 * 128 floats: the 256 KB tail
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     MORL_DISPATCH_FMT(fmt, {
         using F = PlaneFmt<kFmt>;
         const size_t smem = (size_t)F::kStagesMn * (6u * F::P * kMnKT * 128u) + 256 + 1024 + 64 + 1024 + 4096;
-        static bool attr_set = false, attr_set_mc = false;
+        static bool attr_set = false;
         if (!attr_set) {
-            cudaFuncSetAttribute(gemm_planes_mn_kernel<kFmt, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            cudaFuncSetAttribute(gemm_planes_mn_kernel<kFmt>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             attr_set = true;
         }
-        // measured (profiles/r02_bench_ab_mn_multicast.txt): correct, but the update does not get faster (1,558 vs 1,558 / 1,564 updates/s) -- the
-        // kernel is not bound by the L2 -> SM path of H after all -> opt-in (MORL_MN_MULTICAST=1), the single-CTA form stays the default
-        static const bool mc_env = [] { const char* e = getenv("MORL_MN_MULTICAST"); return e && e[0] == '1'; }();
-        if (mc_env && n_tiles == 2 && NB == 256) {
-            if (!attr_set_mc) {
-                cudaFuncSetAttribute(gemm_planes_mn_kernel<kFmt, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                attr_set_mc = true;
-            }
-            cudaLaunchConfig_t cfg;
-            memset(&cfg, 0, sizeof(cfg));
-            cfg.gridDim = dim3(n_tiles * S);
-            cfg.blockDim = dim3(192);
-            cfg.dynamicSmemBytes = smem;
-            cfg.stream = st;
-            cudaLaunchAttribute attr[2];
-            attr[0].id = cudaLaunchAttributeClusterDimension;
-            attr[0].val.clusterDim.x = 2;
-            attr[0].val.clusterDim.y = 1;
-            attr[0].val.clusterDim.z = 1;
-            attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-            attr[1].val.programmaticStreamSerializationAllowed = 1;
-            cfg.attrs = attr;
-            cfg.numAttrs = pdl_enabled() ? 2 : 1;
-            cudaLaunchKernelEx(&cfg, gemm_planes_mn_kernel<kFmt, 1>, tmA, tmB, g);
-        } else {
-            launch_k(gemm_planes_mn_kernel<kFmt, 0>, dim3(n_tiles * S), dim3(192), smem, st, tmA, tmB, g);
-        }
+        launch_k(gemm_planes_mn_kernel<kFmt>, dim3(n_tiles * S), dim3(kGemmThreads), smem, st, tmA, tmB, g);
     });
     rc = check_launch("morl_gemm_planes_mn_f32");
     if (rc) return rc;
@@ -1773,12 +1518,12 @@ extern "C" int morl_split_planes(int fmt, const float* src, int rows, int cols, 
     if (!transpose && (ldp & 7) == 0 && (plane_stride & 7) == 0 && (reinterpret_cast<uintptr_t>(dst_planes) & 15u) == 0) {
         const long long chunks = total >> 3;
         long long vb = (chunks + 255) / 256;
-        if (vb > 148 * 8) vb = 148 * 8;
+        if (vb > 132 * 8) vb = 132 * 8;
         MORL_DISPATCH_FMT(fmt, (launch_k(split_planes_vec8_kernel<kFmt>, dim3((int)vb), dim3(256), 0, st, src, rows, cols, ld_src, dst, rows_pad, ldp, plane_stride, scale)));
         return check_launch("morl_split_planes(vec8)");
     }
     long long blocks = (total + 255) / 256;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     MORL_DISPATCH_FMT(fmt, (split_planes_kernel<kFmt><<<(int)blocks, 256, 0, st>>>(src, rows, cols, ld_src, transpose, dst, rows_pad, ldp, plane_stride, scale)));
     return check_launch("morl_split_planes");
 }
@@ -1804,7 +1549,7 @@ extern "C" int morl_split_planes_multi(int fmt, const MorlSplitJob* jobs, int n_
         if (t > max_total) max_total = t;
     }
     long long bx = (max_total + 255) / 256;
-    if (bx > 148) bx = 148;
+    if (bx > 132) bx = 132;
     bool any_auto = false;
     for (int i = 0; i < n_jobs; ++i) any_auto = any_auto || (jobs[i].auto_scale && jobs[i].scale);
     if (any_auto) {
@@ -1825,7 +1570,7 @@ extern "C" int morl_pairs_relu_split_planes(int fmt, const float* u, const float
                  "morl_pairs_relu_split_planes: bad shape B=%d W=%d H=%d", B, W, H);
     const long long total = (long long)B * W * (H / 8);
     long long blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     if (relu_bits_out)
         MORL_REQUIRE(H % 32 == 0 && H <= 256 && aligned16(relu_bits_out), MORL_ERR_SHAPE,
                      "morl_pairs_relu_split_planes: ReLU bit masks need H %% 32 == 0, H <= 256 (H=%d)", H);
@@ -1857,50 +1602,26 @@ extern "C" int morl_debug_gemm_stats(unsigned long long* out8, int reset) {
 
 namespace morl {
 template <int FMT, int SPLIT>
-static int launch_gemm_planes(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmBh, const CUtensorMap& tmC, const GemmArgs& g, bool pair,
-                              int sms, cudaStream_t st) {
-    constexpr size_t smem1 = KPlan<1, FMT>::kBytes, smem2 = KPlan<2, FMT>::kBytes;
+static int launch_gemm_planes(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmArgs& g, int sms, cudaStream_t st) {
+    constexpr size_t smem = KPlan<FMT>::kBytes;
     static bool attr_set = false;
     if (!attr_set) {
-        cudaFuncSetAttribute(gemm_planes_kernel<1, FMT, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1);
-        cudaFuncSetAttribute(gemm_planes_kernel<2, FMT, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);
+        cudaFuncSetAttribute(gemm_planes_kernel<FMT, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         attr_set = true;
     }
-    if (pair) {
-        const int n_tiles = (g.M + 2 * kGemmBM - 1) / (2 * kGemmBM);
-        const int pairs = n_tiles < sms / 2 ? n_tiles : sms / 2;
-        cudaLaunchConfig_t cfg;
-        memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = dim3(2 * pairs);
-        cfg.blockDim = dim3(kGemmThreads);
-        cfg.dynamicSmemBytes = smem2;
-        cfg.stream = st;
-        cudaLaunchAttribute attr[2];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[1].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = g.pdl ? 2 : 1;
-        cudaLaunchKernelEx(&cfg, gemm_planes_kernel<2, FMT, SPLIT>, tmA, tmB, tmBh, tmC, g);
-    } else {
-        const int n_tiles = (g.M + kGemmBM - 1) / kGemmBM;
-        const int grid = n_tiles < sms ? n_tiles : sms;
-        cudaLaunchConfig_t cfg;
-        memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = dim3(grid);
-        cfg.blockDim = dim3(kGemmThreads);
-        cfg.dynamicSmemBytes = smem1;
-        cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = g.pdl ? 1 : 0;
-        cudaLaunchKernelEx(&cfg, gemm_planes_kernel<1, FMT, SPLIT>, tmA, tmB, tmBh, tmC, g);
-    }
+    const int n_work = (g.M + kGemmBM - 1) / kGemmBM * ((SPLIT && g.N_pad > 128) ? 2 : 1);
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3(n_work < sms ? n_work : sms);
+    cfg.blockDim = dim3(kGemmThreads);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = g.pdl ? 1 : 0;
+    cudaLaunchKernelEx(&cfg, gemm_planes_kernel<FMT, SPLIT>, tmA, tmB, tmC, g);
     return check_launch("morl_gemm_planes_f32");
 }
 }  // namespace morl
@@ -1923,25 +1644,16 @@ extern "C" int morl_gemm_planes_f32(int fmt, const void* a_planes, long long a_p
         MORL_REQUIRE(ldp % 32 == 0 && ldp >= N && ldp <= N_pad && aligned16(c_planes) && c_plane_stride % 8 == 0, MORL_ERR_SHAPE,
                      "morl_gemm_planes_f32: ldp=%d must be a multiple of 32 with N <= ldp <= N_pad", ldp);
     int sms = morl_device_sm_count();
-    if (sms <= 0) sms = 148;
-    // CTA pairs (tcgen05 cta_group::2) whenever there are at least two 128-row tiles; MORL_GEMM_FORCE_1CTA=1 keeps the 1-CTA kernel
-    static const bool force_1cta = [] { const char* e = getenv("MORL_GEMM_FORCE_1CTA"); return e && e[0] == '1'; }();
-    const bool pair = !force_1cta && M > kGemmBM && sms >= 2;
-    const int ncta = pair ? 2 : 1;
+    if (sms <= 0) sms = 132;
     CUtensorMap tmA, tmB;
     int rc = make_plane_map(&tmA, fmt, a_planes, M, K, a_plane_stride, kGemmBM, BK);
     MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "morl_gemm_planes_f32: cuTensorMapEncodeTiled(A) failed (%d)", rc);
-    rc = make_plane_map(&tmB, fmt, b_planes, N_pad, K, b_plane_stride, N_pad / ncta, BK);
+    rc = make_plane_map(&tmB, fmt, b_planes, N_pad, K, b_plane_stride, kGemmBoxN, BK, true);
     MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "morl_gemm_planes_f32: cuTensorMapEncodeTiled(B) failed (%d)", rc);
-    CUtensorMap tmBh = tmB;  // half-width units of the tail split: boxes of N_pad / 4 rows
-    if (pair && N_pad % 64 == 0) {
-        rc = make_plane_map(&tmBh, fmt, b_planes, N_pad, K, b_plane_stride, N_pad / 4, BK);
-        MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "morl_gemm_planes_f32: cuTensorMapEncodeTiled(B half) failed (%d)", rc);
-    }
     CUtensorMap tmC;
     memset(&tmC, 0, sizeof(tmC));
-    if (c_planes) {  // store map of the re-split output: [P][M][ldp], box 32 cols x 32 rows x P planes (64-byte swizzle)
-        rc = make_plane_map(&tmC, fmt, c_planes, M, ldp, c_plane_stride, 32, 32);
+    if (c_planes) {  // store map of the re-split output: [P][M][ldp], box 32 cols x 16 rows x P planes (64-byte swizzle)
+        rc = make_plane_map(&tmC, fmt, c_planes, M, ldp, c_plane_stride, 16, 32);
         MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "morl_gemm_planes_f32: cuTensorMapEncodeTiled(C) failed (%d)", rc);
     }
     GemmArgs g;
@@ -1951,13 +1663,12 @@ extern "C" int morl_gemm_planes_f32(int fmt, const void* a_planes, long long a_p
     g.mask = static_cast<const uint16_t*>(relu_mask_plane0); g.ld_mask = ld_mask; g.relu = relu;
     g.bits_in = static_cast<const uint32_t*>(relu_bits_in); g.bits_out = static_cast<uint32_t*>(relu_bits_out);
     {
-        // TMA ring: A box + B box per stage; a narrow B box (the output layer: N_pad = 32) leaves room for a deeper ring, which is what
+        // TMA ring: A box + B rows per stage; a narrow B (the output layer: N_pad = 32) leaves room for a deeper ring, which is what
         // keeps enough bytes in flight per SM when a tile is four A boxes and almost no tensor work
         const uint32_t rowb = (uint32_t)BK * 2u, P = (uint32_t)fmt_planes(fmt);
         const uint32_t a_box = P * (uint32_t)kGemmBM * rowb;
-        const uint32_t b_box = (P * (uint32_t)(N_pad / ncta) * rowb + 1023u) & ~1023u;
-        const uint32_t room = fmt == MORL_FMT_F16X2 ? (pair ? KPlan<2, MORL_FMT_F16X2>::kOffC : KPlan<1, MORL_FMT_F16X2>::kOffC)
-                                                    : (pair ? KPlan<2, MORL_FMT_BF16X3>::kOffC : KPlan<1, MORL_FMT_BF16X3>::kOffC);
+        const uint32_t b_box = (P * (uint32_t)N_pad * rowb + 1023u) & ~1023u;
+        const uint32_t room = fmt == MORL_FMT_F16X2 ? KPlan<MORL_FMT_F16X2>::kOffC : KPlan<MORL_FMT_BF16X3>::kOffC;
         int n_st = (int)(room / (a_box + b_box));
         if (n_st > 8) n_st = 8;
         static const int st_env = [] { const char* e = getenv("MORL_GEMM_STAGES"); return e ? atoi(e) : 0; }();
@@ -1967,12 +1678,10 @@ extern "C" int morl_gemm_planes_f32(int fmt, const void* a_planes, long long a_p
     }
     g.a_scale = a_scale; g.b_scale = b_scale; g.c_scale = c_scale;
     g.reverse = reverse_tiles ? 1 : 0;
-    // programmatic dependent launch between consecutive GEMMs of a chain (MORL_GEMM_PDL=0 disables it: A/B in profiles/r02_pdl_ab.txt)
+    // programmatic dependent launch between consecutive GEMMs of a chain (MORL_GEMM_PDL=0 disables it)
     static const bool want_pdl = [] { const char* e = getenv("MORL_GEMM_PDL"); return !(e && e[0] == '0'); }();
     g.pdl = want_pdl ? 1 : 0;
-    static const bool want_skip_b = [] { const char* e = getenv("MORL_GEMM_SKIPB"); return e && e[0] == '1'; }();
-    g.skip_b = want_skip_b ? 1 : 0;
-    // measured on B200 (profiles/r01_s3_l2hint_ab.txt): the hints do not help, so they are opt-in (MORL_GEMM_L2HINT=1)
+    // L2 eviction hints on the operand loads are opt-in (MORL_GEMM_L2HINT=1)
     static const bool want_hint = [] { const char* e = getenv("MORL_GEMM_L2HINT"); return e && e[0] == '1'; }();
     g.l2_hint = want_hint ? 1 : 0;
     static const bool want_stats = [] { const char* e = getenv("MORL_GEMM_STATS"); return e && e[0] == '1'; }();
@@ -1987,10 +1696,8 @@ extern "C" int morl_gemm_planes_f32(int fmt, const void* a_planes, long long a_p
     static const int split_env = [] { const char* e = getenv("MORL_GEMM_SPLIT_ACC"); return e ? (e[0] == '0' ? 0 : 1) : -1; }();
     const bool split_acc = split_env >= 0 ? split_env != 0 : split_accumulators != 0;
     if (fmt == MORL_FMT_F16X2)
-        return split_acc ? launch_gemm_planes<MORL_FMT_F16X2, 1>(tmA, tmB, tmBh, tmC, g, pair, sms, st)
-                         : launch_gemm_planes<MORL_FMT_F16X2, 0>(tmA, tmB, tmBh, tmC, g, pair, sms, st);
-    return split_acc ? launch_gemm_planes<MORL_FMT_BF16X3, 1>(tmA, tmB, tmBh, tmC, g, pair, sms, st)
-                     : launch_gemm_planes<MORL_FMT_BF16X3, 0>(tmA, tmB, tmBh, tmC, g, pair, sms, st);
+        return split_acc ? launch_gemm_planes<MORL_FMT_F16X2, 1>(tmA, tmB, tmC, g, sms, st) : launch_gemm_planes<MORL_FMT_F16X2, 0>(tmA, tmB, tmC, g, sms, st);
+    return split_acc ? launch_gemm_planes<MORL_FMT_BF16X3, 1>(tmA, tmB, tmC, g, sms, st) : launch_gemm_planes<MORL_FMT_BF16X3, 0>(tmA, tmB, tmC, g, sms, st);
 }
 
 
@@ -2000,7 +1707,7 @@ extern "C" int morl_gemm_chain_supported(int fmt, int M, int K) {
 }
 
 // Several 256-wide hidden layers (Linear + ReLU, planes in / planes out) of one or two networks in ONE persistent launch: job (c, l) computes
-// act[c][l+1] = relu(act[c][l] . W[c][l]^T + bias[c][l]) exactly as morl_gemm_planes_f32 does (bit-identical), but a CTA pair takes its row tiles
+// act[c][l+1] = relu(act[c][l] . W[c][l]^T + bias[c][l]) exactly as morl_gemm_planes_f32 does (bit-identical), but a CTA takes its row tiles
 // through all layers, so intermediate activations are re-read from L2 instead of HBM (csrc: gemm_chain_kernel).
 extern "C" int morl_gemm_chain_f32(int fmt, int n_chains, int n_layers, const void* const* act_planes, long long act_plane_stride, const float* act_scale,
                                    const void* const* w_planes, long long w_plane_stride, const float* const* w_scales, const float* const* biases,
@@ -2032,9 +1739,9 @@ extern "C" int morl_gemm_chain_f32(int fmt, int n_chains, int n_layers, const vo
             const long long w_stride = l == 0 ? (long long)256 * k_first : w_plane_stride;
             int rc = make_plane_map(&maps.A[job], fmt, a_in, M, kj, a_stride, kGemmBM, BK);
             MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "morl_gemm_chain_f32: cuTensorMapEncodeTiled(A) failed (%d)", rc);
-            rc = make_plane_map(&maps.B[job], fmt, w_planes[job], 256, kj, w_stride, 128, BK);
+            rc = make_plane_map(&maps.B[job], fmt, w_planes[job], 256, kj, w_stride, kGemmBoxN, BK, true);
             MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "morl_gemm_chain_f32: cuTensorMapEncodeTiled(B) failed (%d)", rc);
-            rc = make_plane_map(&maps.C[job], fmt, a_out, M, 256, act_plane_stride, 32, 32);
+            rc = make_plane_map(&maps.C[job], fmt, a_out, M, 256, act_plane_stride, 16, 32);
             MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "morl_gemm_chain_f32: cuTensorMapEncodeTiled(C) failed (%d)", rc);
             g.bias[job] = biases ? biases[job] : nullptr;
             g.b_scale[job] = w_scales ? w_scales[job] : nullptr;
@@ -2042,29 +1749,24 @@ extern "C" int morl_gemm_chain_f32(int fmt, int n_chains, int n_layers, const vo
             g.bits_in[job] = relu_bits_in ? static_cast<const uint32_t*>(relu_bits_in[job]) : nullptr;
             MORL_REQUIRE(aligned16(g.bits_out[job]) && aligned16(g.bits_in[job]), MORL_ERR_ALIGN, "morl_gemm_chain_f32: ReLU bit masks must be 16-byte aligned");
         }
-    g.n_stages = fmt == MORL_FMT_F16X2 ? KPlan<2, MORL_FMT_F16X2>::kStages : KPlan<2, MORL_FMT_BF16X3>::kStages;
+    g.n_stages = fmt == MORL_FMT_F16X2 ? KPlan<MORL_FMT_F16X2>::kStages : KPlan<MORL_FMT_BF16X3>::kStages;
     static const bool want_pdl = [] { const char* e = getenv("MORL_GEMM_PDL"); return !(e && e[0] == '0'); }();
     g.pdl = want_pdl ? 1 : 0;
     int sms = morl_device_sm_count();
-    if (sms <= 0) sms = 148;
-    const int n_tiles = (M + 2 * kGemmBM - 1) / (2 * kGemmBM);
-    const int pairs = n_tiles < sms / 2 ? n_tiles : sms / 2;
+    if (sms <= 0) sms = 132;
+    const int n_tiles = (M + kGemmBM - 1) / kGemmBM;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(2 * pairs);
+    cfg.gridDim = dim3(n_tiles < sms ? n_tiles : sms);
     cfg.blockDim = dim3(kGemmThreads);
     cfg.stream = static_cast<cudaStream_t>(stream);
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = g.pdl ? 2 : 1;
+    cfg.numAttrs = g.pdl ? 1 : 0;
     if (fmt == MORL_FMT_F16X2) {
-        constexpr size_t smem = KPlan<2, MORL_FMT_F16X2>::kBytes;
+        constexpr size_t smem = KPlan<MORL_FMT_F16X2>::kBytes;
         static bool attr_set = false;
         if (!attr_set) {
             cudaFuncSetAttribute(gemm_chain_kernel<MORL_FMT_F16X2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -2073,7 +1775,7 @@ extern "C" int morl_gemm_chain_f32(int fmt, int n_chains, int n_layers, const vo
         cfg.dynamicSmemBytes = smem;
         cudaLaunchKernelEx(&cfg, gemm_chain_kernel<MORL_FMT_F16X2>, maps, g);
     } else {
-        constexpr size_t smem = KPlan<2, MORL_FMT_BF16X3>::kBytes;
+        constexpr size_t smem = KPlan<MORL_FMT_BF16X3>::kBytes;
         static bool attr_set = false;
         if (!attr_set) {
             cudaFuncSetAttribute(gemm_chain_kernel<MORL_FMT_BF16X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -1,5 +1,5 @@
-// gemm_tc.cuh -- tcgen05 / TMEM / TMA / mbarrier PTX wrappers, the split-operand plane formats and the tensor-map helpers shared by
-// the tensor-core kernels of libmorl_b200.so (gemm_planes.cu, qhead_envelope.cu).  sm_100a only.
+// gemm_tc.cuh -- wgmma / TMA / mbarrier PTX wrappers, the split-operand plane formats and the tensor-map helpers shared by
+// the tensor-core kernels of libmorl_b200.so (gemm_planes.cu, qhead_envelope.cu).  sm_90a only.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -42,36 +42,6 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
         "l"(map), "r"(g_smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
         : "memory");
 }
-// ---- CTA-pair (cta_group::2) flavours: the pair's TMA loads signal the LEADER's (cluster rank 0) mbarrier, the leader's MMA
-// commit is multicast to the same barrier offset in both CTAs, the peer's epilogue releases the accumulator remotely ----
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_rank0(uint32_t smem_addr) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, 0;" : "=r"(r) : "r"(smem_addr));
-    return r;
-}
-__device__ __forceinline__ void tma_load_3d_pair(void* dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
-            g_smem_u32(dst)),
-        "l"(map), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-// same, with an L2 eviction-priority hint (createpolicy): activations are read once (evict_first), weight planes by every tile (evict_last)
-__device__ __forceinline__ void tma_load_3d_pair_hint(void* dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1, int c2, uint64_t policy) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(
-            g_smem_u32(dst)),
-        "l"(map), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2), "l"(policy)
-        : "memory");
-}
 __device__ __forceinline__ uint64_t l2_policy_evict_first() {
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
@@ -82,61 +52,80 @@ __device__ __forceinline__ uint64_t l2_policy_evict_last() {
     asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
     return p;
 }
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_bar) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
-}
-__device__ __forceinline__ void tc_commit_pair(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(g_smem_u32(bar)),
-                 "h"((uint16_t)3)
-                 : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// same, with an L2 eviction-priority hint (createpolicy): activations are read once (evict_first), weight planes by every tile (evict_last)
+__device__ __forceinline__ void tma_load_3d_hint(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, uint64_t policy) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(g_smem_u32(dst)),
+        "l"(map), "r"(g_smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "l"(policy)
         : "memory");
 }
-// one box for several CTAs of the cluster (mask: bit r = CTA rank r): written at the same shared-memory offset in each of them, completing on the
-// mbarrier at the same offset in each of them
-__device__ __forceinline__ void tma_load_3d_multicast(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, uint16_t mask) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(
-            g_smem_u32(dst)),
-        "l"(map), "r"(g_smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(mask)
-        : "memory");
-}
-// commit of a CTA's own (cta_group::1) MMAs, arriving on the barrier at this offset in BOTH CTAs of a 2-CTA cluster
-__device__ __forceinline__ void tc_commit_mc(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(g_smem_u32(bar)),
-                 "h"((uint16_t)3)
-                 : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(g_smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, "
-        "%20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]),
-          "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-          "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]),
-          "=r"(v[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tc_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+
+// ---- warpgroup MMA (wgmma.mma_async, sm_90a): D[64 x N] (+)= A[64 x 16] . B[N x 16]^T, both operands through shared-memory descriptors, fp32
+// accumulators in the registers of the 128 threads of the warpgroup.  Thread t = 32 w + l of the warpgroup holds, for every 8-column group j,
+// d[4 j + {0, 1}] = D[16 w + l / 4][8 j + 2 (l % 4) + {0, 1}] and d[4 j + {2, 3}] = the same columns of row + 8.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int PENDING>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
+
+#define MORL_WG_R16_0 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+#define MORL_WG_R16_1 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+#define MORL_WG_R16_2 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
+#define MORL_WG_R16_3 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+#define MORL_WG_R16_4 "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79"
+#define MORL_WG_R16_5 "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+#define MORL_WG_R16_6 "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111"
+#define MORL_WG_R16_7 "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+#define MORL_WG_A8(d, o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+#define MORL_WG_A16(d, o) MORL_WG_A8(d, o), MORL_WG_A8(d, o + 8)
+#define MORL_WG_REGS_16 "%0, %1, %2, %3, %4, %5, %6, %7"
+#define MORL_WG_ACCS_16 MORL_WG_A8(d, 0)
+#define MORL_WG_REGS_32 MORL_WG_R16_0
+#define MORL_WG_ACCS_32 MORL_WG_A16(d, 0)
+#define MORL_WG_REGS_64 MORL_WG_R16_0 ", " MORL_WG_R16_1
+#define MORL_WG_ACCS_64 MORL_WG_A16(d, 0), MORL_WG_A16(d, 16)
+#define MORL_WG_REGS_96 MORL_WG_R16_0 ", " MORL_WG_R16_1 ", " MORL_WG_R16_2
+#define MORL_WG_ACCS_96 MORL_WG_A16(d, 0), MORL_WG_A16(d, 16), MORL_WG_A16(d, 32)
+#define MORL_WG_REGS_128 MORL_WG_R16_0 ", " MORL_WG_R16_1 ", " MORL_WG_R16_2 ", " MORL_WG_R16_3
+#define MORL_WG_ACCS_128 MORL_WG_A16(d, 0), MORL_WG_A16(d, 16), MORL_WG_A16(d, 32), MORL_WG_A16(d, 48)
+#define MORL_WG_REGS_160 MORL_WG_R16_0 ", " MORL_WG_R16_1 ", " MORL_WG_R16_2 ", " MORL_WG_R16_3 ", " MORL_WG_R16_4
+#define MORL_WG_ACCS_160 MORL_WG_A16(d, 0), MORL_WG_A16(d, 16), MORL_WG_A16(d, 32), MORL_WG_A16(d, 48), MORL_WG_A16(d, 64)
+#define MORL_WG_REGS_192 MORL_WG_R16_0 ", " MORL_WG_R16_1 ", " MORL_WG_R16_2 ", " MORL_WG_R16_3 ", " MORL_WG_R16_4 ", " MORL_WG_R16_5
+#define MORL_WG_ACCS_192 MORL_WG_A16(d, 0), MORL_WG_A16(d, 16), MORL_WG_A16(d, 32), MORL_WG_A16(d, 48), MORL_WG_A16(d, 64), MORL_WG_A16(d, 80)
+#define MORL_WG_REGS_224 MORL_WG_R16_0 ", " MORL_WG_R16_1 ", " MORL_WG_R16_2 ", " MORL_WG_R16_3 ", " MORL_WG_R16_4 ", " MORL_WG_R16_5 ", " MORL_WG_R16_6
+#define MORL_WG_ACCS_224 MORL_WG_A16(d, 0), MORL_WG_A16(d, 16), MORL_WG_A16(d, 32), MORL_WG_A16(d, 48), MORL_WG_A16(d, 64), MORL_WG_A16(d, 80), MORL_WG_A16(d, 96)
+#define MORL_WG_REGS_256 MORL_WG_R16_0 ", " MORL_WG_R16_1 ", " MORL_WG_R16_2 ", " MORL_WG_R16_3 ", " MORL_WG_R16_4 ", " MORL_WG_R16_5 ", " MORL_WG_R16_6 ", " MORL_WG_R16_7
+#define MORL_WG_ACCS_256 MORL_WG_A16(d, 0), MORL_WG_A16(d, 16), MORL_WG_A16(d, 32), MORL_WG_A16(d, 48), MORL_WG_A16(d, 64), MORL_WG_A16(d, 80), MORL_WG_A16(d, 96), MORL_WG_A16(d, 112)
+// TYPE_: "f16" / "bf16"; the N / 2 accumulator registers come first, IA_.. are the operand numbers after them.  `accumulate` = 0 overwrites D.
+#define MORL_WGMMA_ASM(N_, TYPE_, IA_, IB_, IP_, ITA_, ITB_)                                                                     \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #IP_ ", 0;\n\t"                                                       \
+                 "wgmma.mma_async.sync.aligned.m64n" #N_ "k16.f32." TYPE_ "." TYPE_ " {" MORL_WG_REGS_##N_ "}, %" #IA_ ", %" #IB_   \
+                 ", p, 1, 1, %" #ITA_ ", %" #ITB_ ";\n\t}"                                                                        \
+                 : MORL_WG_ACCS_##N_                                                                                             \
+                 : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB))
+template <int N>
+struct Wgmma;
+// FMT: plane format (f16x2 -> f16 operands, bf16x3 -> bf16); TA / TB = 1: the operand is MN-major ("transposed") in shared memory
+#define MORL_WGMMA_DEF(N_, IA_, IB_, IP_, ITA_, ITB_)                                                          \
+    template <>                                                                                                \
+    struct Wgmma<N_> {                                                                                         \
+        template <int FMT, int TA, int TB>                                                                     \
+        __device__ __forceinline__ static void mma(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {  \
+            if (FMT == MORL_FMT_F16X2)                                                                         \
+                MORL_WGMMA_ASM(N_, "f16", IA_, IB_, IP_, ITA_, ITB_);                                          \
+            else                                                                                               \
+                MORL_WGMMA_ASM(N_, "bf16", IA_, IB_, IP_, ITA_, ITB_);                                         \
+        }                                                                                                      \
+    };
+MORL_WGMMA_DEF(16, 8, 9, 10, 11, 12)
+MORL_WGMMA_DEF(32, 16, 17, 18, 19, 20)
+MORL_WGMMA_DEF(64, 32, 33, 34, 35, 36)
+MORL_WGMMA_DEF(96, 48, 49, 50, 51, 52)
+MORL_WGMMA_DEF(128, 64, 65, 66, 67, 68)
+MORL_WGMMA_DEF(160, 80, 81, 82, 83, 84)
+MORL_WGMMA_DEF(192, 96, 97, 98, 99, 100)
+MORL_WGMMA_DEF(224, 112, 113, 114, 115, 116)
+MORL_WGMMA_DEF(256, 128, 129, 130, 131, 132)
 
 // ---- operand formats ------------------------------------------------------------------------------------------------------
 template <int FMT>
@@ -146,9 +135,8 @@ template <>
 struct PlaneFmt<MORL_FMT_BF16X3> {
     static constexpr int P = 3, NPROD = 6;
     static constexpr int BK = 32;                                  // 16-bit elements per K-major stage row (64-byte swizzle)
-    static constexpr uint32_t kIdescAB = (1u << 7) | (1u << 10);   // instruction descriptor: a_format = b_format = BF16
     static constexpr uint32_t kOnes2 = 0x3F803F80u;                // two packed 1.0
-    static constexpr int kStages1 = 2, kStages2 = 3, kStagesMn = 3;
+    static constexpr int kStages = 2, kStagesMn = 3;
     // small terms first: A2B0, A0B2, A1B1, A1B0, A0B1, A0B0
     __device__ static constexpr int pa(int t) { return t == 0 ? 2 : (t == 2 || t == 3) ? 1 : 0; }
     __device__ static constexpr int pb(int t) { return t == 1 ? 2 : (t == 2 || t == 4) ? 1 : 0; }
@@ -184,9 +172,8 @@ template <>
 struct PlaneFmt<MORL_FMT_F16X2> {
     static constexpr int P = 2, NPROD = 3;
     static constexpr int BK = 64;                                  // 128-byte swizzle rows
-    static constexpr uint32_t kIdescAB = 0u;                       // a_format = b_format = F16
     static constexpr uint32_t kOnes2 = 0x3C003C00u;
-    static constexpr int kStages1 = 2, kStages2 = 3, kStagesMn = 4;
+    static constexpr int kStages = 2, kStagesMn = 4;
     // small terms first: A1B0, A0B1, A0B0
     __device__ static constexpr int pa(int t) { return t == 0 ? 1 : 0; }
     __device__ static constexpr int pb(int t) { return t == 1 ? 1 : 0; }
@@ -218,7 +205,7 @@ struct PlaneFmt<MORL_FMT_F16X2> {
 
 __device__ __forceinline__ float ld_scale(const float* p) { return p ? __ldg(p) : 1.0f; }
 
-// Shared-memory matrix descriptor, K-major canonical layout (cute::UMMA::SmemDescriptor, version 1) with ROWB-byte rows = the swizzle
+// Shared-memory matrix descriptor of wgmma, K-major canonical layout with ROWB-byte rows = the swizzle
 // span (64 B -> SWIZZLE_64B, 128 B -> SWIZZLE_128B); 8-row groups are contiguous: SBO = 8 * ROWB; LBO unused (1).  A K step of 16
 // elements inside the swizzle span is a +32 B advance of the start address.
 template <int ROWB>
@@ -228,8 +215,7 @@ __device__ __forceinline__ uint64_t make_desc_k(uint32_t smem_addr) {
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);        // start address, 16-byte units
     d |= (uint64_t)1 << 16;                            // leading byte offset (ignored for swizzled K-major), 16-byte units
     d |= (uint64_t)((8 * ROWB) >> 4) << 32;            // stride byte offset: 8 rows x ROWB
-    d |= (uint64_t)1 << 46;                            // descriptor version (Blackwell)
-    d |= (uint64_t)(ROWB == 64 ? 4 : 2) << 61;         // layout type: SWIZZLE_64B = 4, SWIZZLE_128B = 2
+    d |= (uint64_t)(ROWB == 64 ? 2 : 1) << 62;         // swizzle mode: 128 B = 1, 64 B = 2
     return d;
 }
 
@@ -253,14 +239,15 @@ static inline EncodeTiledFn get_encode_fn() {
 static inline int fmt_planes(int fmt) { return fmt == MORL_FMT_F16X2 ? 2 : 3; }
 static inline CUtensorMapDataType fmt_tm_type(int fmt) { return fmt == MORL_FMT_F16X2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16; }
 
-// [P][rows][K] plane tensor, box = P x box_rows x box_k elements, swizzle span = box_k * 2 bytes (64 or 128)
-static inline int make_plane_map(CUtensorMap* map, int fmt, const void* base, int rows, int K, long long plane_stride_elems, int box_rows, int box_k) {
+// [P][rows][K] plane tensor, box = P (or one plane) x box_rows x box_k elements, swizzle span = box_k * 2 bytes (64 or 128)
+static inline int make_plane_map(CUtensorMap* map, int fmt, const void* base, int rows, int K, long long plane_stride_elems, int box_rows, int box_k,
+                                 bool one_plane = false) {
     EncodeTiledFn enc = get_encode_fn();
     if (!enc) return -1;
     const cuuint32_t P = (cuuint32_t)fmt_planes(fmt);
     const cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)rows, P};
     const cuuint64_t strides[2] = {(cuuint64_t)K * 2, (cuuint64_t)plane_stride_elems * 2};
-    const cuuint32_t box[3] = {(cuuint32_t)box_k, (cuuint32_t)box_rows, P};
+    const cuuint32_t box[3] = {(cuuint32_t)box_k, (cuuint32_t)box_rows, one_plane ? 1u : P};
     const cuuint32_t estr[3] = {1, 1, 1};
     const CUresult r = enc(map, fmt_tm_type(fmt), 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                            box_k == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,

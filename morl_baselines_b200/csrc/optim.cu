@@ -35,7 +35,7 @@ extern "C" int morl_polyak_f32(const float* const* params, float* const* targets
                  n_tensors, (long long)max_size);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     long long bx = (max_size + 255) / 256;
-    if (bx > 148 * 4) bx = 148 * 4;
+    if (bx > 132 * 4) bx = 132 * 4;
     const dim3 grid((unsigned)bx, (unsigned)n_tensors, 1);
     // (1 - tau) is formed in double then rounded, like Python's `1.0 - tau` handed to Tensor.mul_
     const float omt = (float)(1.0 - tau);

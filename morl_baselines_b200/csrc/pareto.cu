@@ -79,8 +79,8 @@ static int pareto_launch(const char* fn, const T* pts, int N, int D, int remove_
     if (N == 0) return MORL_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int itiles = (N + kParetoTile - 1) / kParetoTile;
-    // enough CTAs for ~4 waves of 148 SMs, but never split j finer than one pass of the CTA's 8 warps
-    int jsplits = (4 * 148 + itiles - 1) / itiles;
+    // enough CTAs for ~4 waves of 132 SMs, but never split j finer than one pass of the CTA's 8 warps
+    int jsplits = (4 * 132 + itiles - 1) / itiles;
     const int max_splits = (N + kParetoThreads - 1) / kParetoThreads;
     if (jsplits > max_splits) jsplits = max_splits;
     if (jsplits < 1) jsplits = 1;
@@ -248,7 +248,7 @@ extern "C" int morl_front_unpack_f64(const double* gathered, int world, int d, i
                  cap, n_extra);
     const int rec_len = 1 + cap * d + n_extra;
     long long blocks = ((long long)world * cap * d + 255) / 256;
-    if (blocks > 148 * 4) blocks = 148 * 4;
+    if (blocks > 132 * 4) blocks = 132 * 4;
     front_unpack_kernel<<<(int)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(gathered, world, rec_len, d, cap, n_extra, pts_out, meta_out);
     return check_launch("morl_front_unpack_f64");
 }

@@ -1,21 +1,20 @@
-// qhead_envelope.cu -- the output layer of BOTH Q-networks, the envelope operator and the vector Bellman target as ONE kernel, sm_100a.
+// qhead_envelope.cu -- the output layer of BOTH Q-networks, the envelope operator and the vector Bellman target as ONE kernel, sm_90a.
 //
 // Replaces, for the two no-grad passes of Envelope.update (reference multi_policy/envelope/envelope.py:420 online net on s', :429 target
 // net on s', :422-440 einsum -> max -> argmax -> gather x2, :298 Bellman line), the chain
 //     Q_on = h_on . W_on^T + b_on   (GEMM, 6.3 MB written)      Q_tg = h_tg . W_tg^T + b_tg   (GEMM, 6.3 MB written)
 //     target = envelope_td(Q_on, Q_tg, ...)                     (12.6 MB read)
-// by one pass over the last hidden activations: the Q tiles live in tensor memory and shared memory only (SURVEY 8(f)2, hypothesis H1).
+// by one pass over the last hidden activations: the Q tiles live in registers and shared memory only (SURVEY 8(f)2, hypothesis H1).
 //
-// One persistent CTA per SM, 320 threads, a tile = 128 pair rows (b*W + j) = 128 / W whole transitions:
-//   warp 0   : TMA producer  -- the output-layer weight planes of both nets ONCE per CTA (resident: 2 x K/64 boxes of [2 x 32 x 64]
+// One persistent CTA per SM, 288 threads, a tile = 128 pair rows (b*W + j) = 128 / W whole transitions:
+//   warp 8   : TMA producer  -- the output-layer weight planes of both nets ONCE per CTA (resident: 2 x K/64 boxes of [2 x 32 x 64]
 //              fp16), then per tile and per net K/64 activation boxes [2 planes x 128 rows x 64] through a ring (128-byte swizzle);
-//   warp 1   : MMA issuer    -- per net 3 x K/16 tcgen05.mma.kind::f16 (M = 128, N = 32, K = 16; products A1B0 + A0B1 + A0B0 in the order of
-//              gemm_planes_kernel, so the accumulators are bit-identical to the unfused output-layer GEMM); Q_on in TMEM columns
-//              [0, 32), Q_tg in [32, 64) of one of two accumulator sets (the MMAs of tile n+1 overlap the epilogue + scan of tile n);
-//   warps 2-5: group 0       -- tcgen05.ld of Q_on (one row per thread), x 1/(sA sB) + bias, fp32 rows into the shared Q tile (AoS
-//   warps 6-9: group 1          [j][a][d], exactly the layout of Q[b] in HBM); same for Q_tg.  Then each group runs the envelope scan
+//   warps 0-3: group 0       -- the warpgroup issues, for Q_on, 2 (row halves) x 3 x K/16 wgmma.mma_async (M = 64, N = 32, K = 16; products
+//   warps 4-7: group 1          A1B0 + A0B1 + A0B0 in the order of gemm_planes_kernel, so the accumulators are bit-identical to the unfused
+//              output-layer GEMM), then x 1/(sA sB) + bias, fp32 rows into the shared Q tile (AoS [j][a][d], exactly the layout of Q[b]
+//              in HBM); same for Q_tg in group 1.  Then each group runs the envelope scan
 //              (envelope_wp.cuh: weight-pair FMA-chain filter + exact re-check, first-occurrence ties) of the transitions t = group,
-//              group + 2, ... of the tile and writes  r + (1 - done) gamma Q_tg[b, j*, a*, :].
+//              group + 2, ... of the tile and writes  r + (1 - done) gamma Q_tg[b, j*, a*, :].  The producer stages the next tile meanwhile.
 // HBM traffic: the activation planes of both nets (2 x 4 B x B W x K), read once; roofline = HBM (DESIGN.md section 4.1b).
 #include <stdlib.h>
 
@@ -24,7 +23,7 @@
 
 namespace morl {
 
-constexpr int kQhThreads = 320;
+constexpr int kQhThreads = 288;   // warps 0-7: two warpgroups (one per network), warp 8: TMA producer
 constexpr int kQhBM = 128;
 constexpr int kQhBN = 32;       // accumulator columns per net (N = A*D <= 32)
 constexpr int kQhMaxStages = 6;
@@ -77,11 +76,10 @@ qhead_envelope_kernel(const __grid_constant__ CUtensorMap tmA_on, const __grid_c
                       const __grid_constant__ CUtensorMap tmB_tg, const QHeadArgs g) {
     using F = PlaneFmt<FMT>;
     using L = QhPlan<FMT>;
-    constexpr int P = F::P;
     constexpr int BK = F::BK;
     constexpr uint32_t ROWB = L::kRowB;
     const L plan(g.K, g.N, g.n_stages);
-    const int kStages = g.n_stages;
+    const uint32_t kStages = (uint32_t)g.n_stages;
     const int n_kblk = g.K / BK;
     extern __shared__ uint8_t qsmem_raw[];
     uint8_t* sm = qsmem_raw + ((1024u - (g_smem_u32(qsmem_raw) & 1023u)) & 1023u);  // (pointer arithmetic on the shared array: see gemm_planes.cu)
@@ -93,28 +91,17 @@ qhead_envelope_kernel(const __grid_constant__ CUtensorMap tmA_on, const __grid_c
     uint64_t* full = reinterpret_cast<uint64_t*>(sm + plan.off_bar);
     uint64_t* empty = full + kQhMaxStages;
     uint64_t* bfull = empty + kQhMaxStages;
-    uint64_t* tfull = bfull + 1;
-    uint64_t* tempty = tfull + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int N = g.N;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kStages; ++s) {
+        for (uint32_t s = 0; s < kStages; ++s) {
             g_mbar_init(&full[s], 1);
-            g_mbar_init(&empty[s], 1);
+            g_mbar_init(&empty[s], 8);  // one arrival per consumer warp (both groups walk every stage)
         }
         g_mbar_init(bfull, 1);
-        for (int s = 0; s < 2; ++s) {
-            g_mbar_init(&tfull[s], 1);
-            g_mbar_init(&tempty[s], 8);  // one arrival per epilogue warp
-        }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {  // two accumulator sets x (Q_on | Q_tg) x 32 columns
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 128;" ::"r"(g_smem_u32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     if (g.pdl) {  // nothing above reads global memory; everything below may (see gemm_planes_kernel)
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -124,12 +111,9 @@ qhead_envelope_kernel(const __grid_constant__ CUtensorMap tmA_on, const __grid_c
         const int net = threadIdx.x >> 5, n = threadIdx.x & 31;
         bias_s[threadIdx.x] = (g.bias[net] && n < N) ? g.bias[net][n] : 0.f;
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ================= TMA producer =================
         if (lane == 0) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA_on) : "memory");
@@ -146,60 +130,19 @@ qhead_envelope_kernel(const __grid_constant__ CUtensorMap tmA_on, const __grid_c
                         g_mbar_wait(&empty[stage], phase ^ 1u);
                         g_mbar_expect_tx(&full[stage], L::kAStage);
                         tma_load_3d(smA + stage * L::kAStage, net ? &tmA_tg : &tmA_on, &full[stage], kb * BK, tile * kQhBM, 0);
-                        if (++stage == (uint32_t)kStages) {
+                        if (++stage == kStages) {
                             stage = 0;
                             phase ^= 1u;
                         }
                     }
                 }
-            }
-        }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        if (lane == 0) {
-            // instruction descriptor: D = f32, A / B = the plane type, both K-major, N = 32, M = 128
-            constexpr uint32_t idesc = (1u << 4) | F::kIdescAB | ((uint32_t)(kQhBN >> 3) << 17) | ((uint32_t)(kQhBM >> 4) << 24);
-            constexpr uint32_t a_plane = kQhBM * ROWB, b_plane = kQhBN * ROWB;
-            g_mbar_wait(bfull, 0);
-            tc_fence_after();
-            uint32_t stage = 0, phase = 0, it = 0;
-            for (int u = blockIdx.x; u < g.n_tiles; u += gridDim.x, ++it) {
-                const uint32_t as = it & 1u;
-                g_mbar_wait(&tempty[as], ((it >> 1) & 1u) ^ 1u);
-                tc_fence_after();
-                for (int net = 0; net < g.n_nets; ++net) {
-                    const uint32_t d_tmem = tmem_base + as * (2u * kQhBN) + (uint32_t)net * kQhBN;
-                    for (int kb = 0; kb < n_kblk; ++kb) {
-                        g_mbar_wait(&full[stage], phase);
-                        tc_fence_after();
-                        const uint32_t a0 = g_smem_u32(smA + stage * L::kAStage);
-                        const uint32_t b0 = g_smem_u32(smB + (uint32_t)(net * n_kblk + kb) * L::kBChunk);
-#pragma unroll
-                        for (int ks = 0; ks < BK / 16; ++ks) {
-#pragma unroll
-                            for (int t = 0; t < F::NPROD; ++t) {
-                                const uint64_t ad = make_desc_k<ROWB>(a0 + F::pa(t) * a_plane + ks * 32);
-                                const uint64_t bd = make_desc_k<ROWB>(b0 + F::pb(t) * b_plane + ks * 32);
-                                tc_mma_bf16(d_tmem, ad, bd, idesc, (kb | ks | t) != 0 ? 1u : 0u);
-                            }
-                        }
-                        tc_commit(&empty[stage]);  // frees the activation stage when the MMAs above have read it
-                        if (++stage == (uint32_t)kStages) {
-                            stage = 0;
-                            phase ^= 1u;
-                        }
-                    }
-                }
-                tc_commit(&tfull[as]);  // both accumulators of the set are complete
             }
         }
     } else {
-        // ================= epilogue + envelope scan (warps 2..9) =================
-        const int e = warp - 2;
-        const int grp = e >> 2;                      // 0: stages Q_on, 1: stages Q_tg; scans the transitions t = grp, grp + 2, ...
-        const int quad = warp & 3;                   // TMEM lane quadrant this warp may read
-        const int tid_g = (e & 3) * 32 + lane;       // index in the group (scan / finish roles)
-        const int row = quad * 32 + lane;            // tile row staged by this thread
+        // ================= MMA + epilogue + envelope scan (warpgroups 0 and 1) =================
+        const int grp = warp >> 2;                   // 0: computes and stages Q_on, 1: Q_tg; scans the transitions t = grp, grp + 2, ...
+        const int tid_g = (warp & 3) * 32 + lane;    // index in the group (scan / finish roles)
+        const int l4 = lane & 3;
         const float k_acc = 1.0f / (ld_scale(g.a_scale[grp]) * ld_scale(g.b_scale[grp]));
         const int W = g.W, A = g.A, C = W * A, T = kQhBM / W;
         const bool fused = g.n_nets == 2;
@@ -207,60 +150,94 @@ qhead_envelope_kernel(const __grid_constant__ CUtensorMap tmA_on, const __grid_c
         if (fused) wp::load_role<D>(role, g.wset, W, tid_g);
         const int part = tid_g & 1;
         auto sync_g = [&]() { bar_sync_named(2 + grp, 128); };
-        uint32_t it = 0;
-        for (int u = blockIdx.x; u < g.n_tiles; u += gridDim.x, ++it) {
+        constexpr uint32_t a_plane = kQhBM * ROWB, b_plane = kQhBN * ROWB;
+        if (grp < g.n_nets) g_mbar_wait(bfull, 0);
+        uint32_t stage = 0, phase = 0;
+        for (int u = blockIdx.x; u < g.n_tiles; u += gridDim.x) {
             const int tile = g.reverse ? g.n_tiles - 1 - u : u;
-            const uint32_t as = it & 1u;
-            g_mbar_wait(&tfull[as], (it >> 1) & 1u);
-            tc_fence_after();
-            uint32_t v[32];
-            tc_ld32(tmem_base + as * (2u * kQhBN) + (uint32_t)grp * kQhBN + ((uint32_t)(quad * 32) << 16), v);
-            tc_ld_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) g_mbar_arrive(&tempty[as]);  // the accumulator set is free for tile it + 2
-            float x[32];
+            // acc[mh]: rows [64 mh, 64 mh + 64) of the tile, 32 columns: the products of a K step in the order of gemm_planes_kernel, so the
+            // accumulators are bit-identical to the unfused output-layer GEMM.  Both groups walk EVERY stage of the ring in order (a parity
+            // wait is only meaningful one phase ahead) and release it; a group issues MMAs on the stages of its own net only.
+            float acc[2][16];
+            for (int net = 0; net < g.n_nets; ++net) {
+                uint32_t prev = 0;
+                for (int kb = 0; kb < n_kblk; ++kb) {
+                    g_mbar_wait(&full[stage], phase);
+                    if (net == grp) {
+                        wgmma_fence();
+                        const uint32_t a0 = g_smem_u32(smA + stage * L::kAStage);
+                        const uint32_t b0 = g_smem_u32(smB + (uint32_t)(grp * n_kblk + kb) * L::kBChunk);
 #pragma unroll
-            for (int j = 0; j < 32; ++j) x[j] = __fmaf_rn(__uint_as_float(v[j]), k_acc, bias_s[grp * kQhBN + j]);
-            if (!fused) {
-                // output layer of one net: the rows go straight to HBM (16-byte stores when the row length allows)
-                if (grp == 0) {
-                    float* orow = g.q_out[0] + ((size_t)tile * kQhBM + row) * N;
-                    if ((N & 3) == 0) {
+                        for (int mh = 0; mh < 2; ++mh) {
 #pragma unroll
-                        for (int j = 0; j < 32; j += 4)
-                            if (j < N) *reinterpret_cast<float4*>(orow + j) = make_float4(x[j], x[j + 1], x[j + 2], x[j + 3]);
-                    } else {
+                            for (int ks = 0; ks < BK / 16; ++ks) {
 #pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (j < N) orow[j] = x[j];
+                                for (int t = 0; t < F::NPROD; ++t) {
+                                    const uint64_t ad = make_desc_k<ROWB>(a0 + F::pa(t) * a_plane + (uint32_t)mh * 64u * ROWB + ks * 32);
+                                    const uint64_t bd = make_desc_k<ROWB>(b0 + F::pb(t) * b_plane + ks * 32);
+                                    Wgmma<kQhBN>::template mma<FMT, 0, 0>(acc[mh], ad, bd, (kb | ks | t) != 0 ? 1u : 0u);
+                                }
+                            }
+                        }
+                        wgmma_commit();
+                        if (kb > 0) {
+                            wgmma_wait<1>();
+                            if (lane == 0) g_mbar_arrive(&empty[prev]);  // frees the activation stage when the MMAs above have read it
+                        }
+                        prev = stage;
+                    } else if (lane == 0) {
+                        g_mbar_arrive(&empty[stage]);  // the other group's operand
                     }
+                    if (++stage == kStages) {
+                        stage = 0;
+                        phase ^= 1u;
+                    }
+                }
+                if (net == grp) {
+                    wgmma_wait<0>();
+                    if (lane == 0) g_mbar_arrive(&empty[prev]);
+                }
+            }
+            if (!fused) {
+                // output layer of one net: the rows go straight to HBM
+                if (grp == 0) {
+#pragma unroll
+                    for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const int row = mh * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+                            float* orow = g.q_out[0] + ((size_t)tile * kQhBM + row) * N;
+#pragma unroll
+                            for (int q = 0; q < 4; ++q)
+#pragma unroll
+                                for (int c = 0; c < 2; ++c) {
+                                    const int col = 8 * q + 2 * l4 + c;
+                                    if (col < N) orow[col] = __fmaf_rn(acc[mh][4 * q + 2 * h + c], k_acc, bias_s[col]);
+                                }
+                        }
                 }
                 continue;
             }
             bar_sync_named(1, 256);  // every scan of the previous tile has finished reading the Q tile
-            float* qrow = Qst + ((size_t)grp * kQhBM + row) * N;
-            if ((N & 3) == 0) {
 #pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                    if (j < N) *reinterpret_cast<float4*>(qrow + j) = make_float4(x[j], x[j + 1], x[j + 2], x[j + 3]);
-            } else {
+            for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    if (j < N) qrow[j] = x[j];
-            }
-            if (g.q_out[grp]) {
-                float* orow = g.q_out[grp] + ((size_t)tile * kQhBM + row) * N;
-                if ((N & 3) == 0) {
+                for (int h = 0; h < 2; ++h) {
+                    const int row = mh * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+                    float* qrow = Qst + ((size_t)grp * kQhBM + row) * N;
+                    float* orow = g.q_out[grp] ? g.q_out[grp] + ((size_t)tile * kQhBM + row) * N : nullptr;
 #pragma unroll
-                    for (int j = 0; j < 32; j += 4)
-                        if (j < N) *reinterpret_cast<float4*>(orow + j) = make_float4(x[j], x[j + 1], x[j + 2], x[j + 3]);
-                } else {
+                    for (int q = 0; q < 4; ++q)
 #pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if (j < N) orow[j] = x[j];
+                        for (int c = 0; c < 2; ++c) {
+                            const int col = 8 * q + 2 * l4 + c;
+                            if (col < N) {
+                                const float x = __fmaf_rn(acc[mh][4 * q + 2 * h + c], k_acc, bias_s[grp * kQhBN + col]);
+                                qrow[col] = x;
+                                if (orow) orow[col] = x;
+                            }
+                        }
                 }
-            }
             bar_sync_named(1, 256);  // both Q tiles are staged
             for (int t = grp; t < T; t += 2) {
                 const int b = tile * T + t;
@@ -286,13 +263,6 @@ qhead_envelope_kernel(const __grid_constant__ CUtensorMap tmA_on, const __grid_c
                 if (t + 2 < T) sync_g();  // the group's scratch is rewritten by its next transition
             }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 128;" ::"r"(tmem_base) : "memory");
     }
 }
 
@@ -386,7 +356,7 @@ extern "C" int morl_qhead_envelope_td_f32(int fmt, const void* a_on_planes, cons
     g.n_stages = n_st;
     const size_t smem = QhPlan<kFmt>(K, g.N, n_st).bytes;
     int sms = morl_device_sm_count();
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
     const int grid = g.n_tiles < sms ? g.n_tiles : sms;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     bool launched = false;
@@ -440,7 +410,7 @@ extern "C" int morl_qhead_gemm_f32(int fmt, const void* a_planes, long long a_pl
     g.n_stages = n_st;
     const size_t smem = QhPlan<kFmt>(K, N, n_st).bytes;
     int sms = morl_device_sm_count();
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
     const int grid = g.n_tiles < sms ? g.n_tiles : sms;
     return launch_qhead<kFmt, 3, MORL_DOT_UNFUSED>(tmA, tmA, tmB, tmB, g, smem, grid, static_cast<cudaStream_t>(stream));
 }

@@ -80,7 +80,7 @@ extern "C" int morl_replay_gather(const float* obs_store, const float* next_obs_
     const long long work = (long long)B * (vec4 ? obs_dim / 4 : obs_dim);
     long long blocks = (work + 255) / 256;
     if (blocks < 1) blocks = 1;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     if (vec4)
         launch_k(replay_gather_kernel<true>, dim3((int)blocks), dim3(256), 0, st, obs_store, next_obs_store, act_store, rew_store, done_store, idx, B, obs_dim,
                                                                 act_dim, rew_dim, act_is_u8, capacity, obs_out, next_obs_out, act_out,

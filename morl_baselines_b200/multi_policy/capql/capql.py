@@ -1,4 +1,4 @@
-"""CAPQL on the B200 update engine -- drop-in for reference morl_baselines/multi_policy/capql/capql.py (same classes
+"""CAPQL on the CUDA update engine -- drop-in for reference morl_baselines/multi_policy/capql/capql.py (same classes
 ``ReplayMemory / WeightSamplerAngle / Policy / QNetwork / CAPQL`` and method names).
 
 Hot-path row a12 of SURVEY.md section 8: the SAC vector target with the per-objective minimum over the critics and the
@@ -6,7 +6,7 @@ entropy term, stack -> min -> (alpha * logp) broadcast -> Bellman (capql.py:326-
 (morl_actor_critic_td_f32, variant ELEMENTWISE_MIN); the target sync of all critics is one multi-tensor launch per net.
 The transition store keeps the reference's semantics (python ``random.sample`` over the stored tuples, capql.py:51-58) but
 lives in preallocated arrays mirrored in HBM, so a minibatch is one index gather instead of six np.stack + six copies.
-The reference's update is ~200 tiny tensor operations (8.4 ms on its CPU path, 3.9 ms eager on a B200, launch bound): the device side
+The reference's update is ~200 tiny tensor operations (launch bound): the device side
 of one gradient update -- gather, target, critic step, policy step, target syncs -- is captured in a CUDA graph over static index /
 noise buffers (``use_cuda_graph``, common/graphed.py) and replayed with one host call per update.
 """

@@ -1,4 +1,4 @@
-"""Envelope Q-Learning on the B200 update engine (drop-in for reference
+"""Envelope Q-Learning on the CUDA update engine (drop-in for reference
 morl_baselines/multi_policy/envelope/envelope.py: same constructor, attributes, ``update / eval / act / max_action /
 envelope_target / ddqn_target / train / save / load / get_config``).
 
@@ -11,7 +11,7 @@ What changes under the API (SURVEY.md section 8, rows a1-a6, a14-a17, a20):
     gather -> MSE -> homotopy loss -> d loss/d q -> PER priorities (envelope.py:301-313, 329-331) is ONE kernel
     (morl_td_mse_priority_f32); the minibatch gather reads a replay store resident in HBM (morl_replay_gather);
     the target sync is one multi-tensor launch (morl_polyak_f32);
-  * the dense layers (forward on the three passes, hand-written backward) run on the tcgen05 tensor cores with fp32-accurate split
+  * the dense layers (forward on the three passes, hand-written backward) run on the tensor cores (wgmma) with fp32-accurate split
     operands (tc_mlp.py, csrc/gemm_bf16x3.cu); the update does not go through autograd: the loss kernel emits d loss / d Q, the
     backward GEMMs write straight into persistent ``.grad`` buffers, clip + Adam is one fused multi-tensor step;
   * the whole gradient update is captured in a CUDA graph and replayed (no host sync inside, no library kernel in the graph); the
@@ -40,8 +40,8 @@ from ...common.prioritized_buffer import PrioritizedReplayBuffer
 from ...common.utils import linearly_decaying_value
 from ...common.weights import equally_spaced_weights, random_weights
 
-# output layers + envelope operator + Bellman line as one kernel (csrc/qhead_envelope.cu: 29.4 us against 57.7 us for the three-launch chain at
-# the north-star shape, bit-identical -- profiles/r02_qhead_time.txt); MORL_FUSED_HEAD=0 keeps the three-launch chain (A/B runs)
+# output layers + envelope operator + Bellman line as one kernel (csrc/qhead_envelope.cu; bit-identical to the
+# three-launch chain, tests/test_qhead_envelope_gpu.py); MORL_FUSED_HEAD=0 keeps the three-launch chain (A/B runs)
 _FUSED_HEAD = os.environ.get("MORL_FUSED_HEAD", "1") != "0"
 _PRE_REFRESH = os.environ.get("MORL_PRE_REFRESH", "1") == "1"  # weight-plane refresh on a side branch, under the tree walk + gather (+1.4 %)
 _HEAD_REVERSE = os.environ.get("MORL_HEAD_REVERSE", "1") == "1"  # the fused head walks the tiles from the last one after a chained pass (L2; +1.2 %)
@@ -211,7 +211,7 @@ class Envelope(MOPolicy, MOAgent):
                                               device=self.device if replay_on_device else None)
         self.dot_mode = ops.DOT_UNFUSED
         self.use_cuda_graph = use_cuda_graph
-        # dense layers of all three passes on the tcgen05 tensor cores (split operands, fp32-accurate).  No silent library fallback: a
+        # dense layers of all three passes on the tensor cores (wgmma, split operands, fp32-accurate).  No silent library fallback: a
         # network the tensor-core path does not cover is an error unless the caller explicitly opts into the validation path.
         # operand format of the tensor-core dense layers: "f16x2" (default: 3 MMAs / 4 B per element, fp16 exponent range with device-resident
         # power-of-two scales) or "bf16x3" (6 MMAs / 6 B per element, fp32 exponent range) -- tc_mlp.py
@@ -220,8 +220,8 @@ class Envelope(MOPolicy, MOAgent):
             raise ValueError(f"tensor_core_format must be 'f16x2' or 'bf16x3', got {fmt_name!r}")
         if tensor_core_accumulators not in ("single", "split"):
             raise ValueError(f"tensor_core_accumulators must be 'single' or 'split', got {tensor_core_accumulators!r}")
-        # "split": leading and correction products of the forward GEMMs in separate TMEM accumulators (csrc/gemm_planes.cu): the tensor cores
-        # truncate their fp32 accumulation; Q error vs float64 1.1e-6 instead of 2.7e-6 (both inside the 1e-5 bar), ~8 % slower update
+        # "split": leading and correction products of the forward GEMMs in separate register accumulators (csrc/gemm_planes.cu), added
+        # once with a correctly rounded fp32 add: fewer accumulations at full magnitude; a 256-wide layer then runs as two column units
         self.tensor_core_accumulators = tensor_core_accumulators
         self.tensor_core_format = fmt_name
         self._tc_fmt = ops.FMT_F16X2 if fmt_name == "f16x2" else ops.FMT_BF16X3
@@ -429,7 +429,7 @@ class Envelope(MOPolicy, MOAgent):
                     # output layers of both nets + envelope operator + Bellman line in ONE kernel: Q_on / Q_tg (envelope.py:420, :429) exist
                     # in tensor / shared memory only (csrc/qhead_envelope.cu; bit-identical to the three-launch chain below)
                     if self._tc_on.chain_supported() and self._tc_tg.chain_supported():
-                        # hidden layers 2.. of BOTH nets in one persistent launch: a CTA pair takes each of its row tiles through all layers of
+                        # hidden layers 2.. of BOTH nets in one persistent launch: a CTA takes each of its row tiles through all layers of
                         # both nets, re-reading every intermediate activation from L2 (csrc/gemm_planes.cu: gemm_chain_kernel)
                         if self._nograd_chain is None:
                             self._nograd_chain = TCPairMlp.make_chain([self._tc_on, self._tc_tg])
@@ -505,9 +505,9 @@ class Envelope(MOPolicy, MOAgent):
                 raw = (s["raw_prio"] if device_per else s["prio"]) if self.per else None
                 ops.td_mse_priority(q_values, act.reshape(-1), target_q, wset_t, 0.0, B, Wt, ops.ROWS_BMAJOR, want_grad=True, want_prio=self.per,
                                     workspace=s["ws"], loss_out=s["loss1"], grad_out=self._dq, prio_out=raw, lambda_dev=s["lam"])
-                # device-resident PER: the priority / sum-tree branch (a 63 us single-block kernel with 45 KB of shared memory) is forked only
-                # AFTER the last persistent GEMM of the backward pass -- forked right here it kept one SM, hence one CTA pair of every GEMM
-                # that overlapped it, waiting (the first dX GEMM ran 46 us instead of 32); the host-tree modes keep the early hand-off
+                # device-resident PER: the priority / sum-tree branch (a single-block kernel with 45 KB of shared memory) is forked only
+                # AFTER the last persistent GEMM of the backward pass -- forked right here it keeps one SM, hence one persistent CTA of every GEMM
+                # that overlaps it, waiting; the host-tree modes keep the early hand-off
                 defer_ship = dp is None and device_per and _DEFER_TREE
                 if dp is None and not defer_ship:
                     self._ship_results(raw, device_per)

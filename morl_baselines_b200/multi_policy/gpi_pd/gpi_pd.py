@@ -1,4 +1,4 @@
-"""GPI-LS / GPI-PD (discrete actions) on the B200 update engine -- drop-in for reference
+"""GPI-LS / GPI-PD (discrete actions) on the CUDA update engine -- drop-in for reference
 morl_baselines/multi_policy/gpi_pd/gpi_pd.py (same constructor incl. the Dyna arguments, ``update / gpi_action / eval / max_action /
 _envelope_target / _reset_priorities / _rollout_dynamics / _sample_batch_experiences / set_weight_support / train_iteration / save / load``).
 

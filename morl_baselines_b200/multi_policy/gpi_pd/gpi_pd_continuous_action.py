@@ -1,4 +1,4 @@
-"""GPI-PD / GPI-LS with continuous actions on the B200 update engine -- drop-in for reference
+"""GPI-PD / GPI-LS with continuous actions on the CUDA update engine -- drop-in for reference
 morl_baselines/multi_policy/gpi_pd/gpi_pd_continuous_action.py (same classes ``Policy / QNetwork / GPIPDContinuousAction /
 GPILSContinuousAction``, constructor arguments, method names and checkpoint keys).
 
@@ -10,7 +10,7 @@ Hot-path row a11 of SURVEY.md section 8 (BASELINE.json configs[2]: GPI-PD on mo-
 * the GPI evaluation over the |M| x |M| (critic-conditioning weight, candidate action) pairs (``eval``, :463-478) is one batched
   critic call followed by the fused double-argmax kernel (``morl_gpi_envelope_f32`` with B = 1);
 * target-network syncs are one multi-tensor launch per network (``polyak_update``), Adam steps the fused two-launch optimiser;
-* the reference's update is ~200 tiny tensor operations (13.4 ms on its CPU path, 3.3 ms eager on a B200, launch bound): the device
+* the reference's update is ~200 tiny tensor operations (launch bound): the device
   side of one gradient update -- gather from the HBM replay mirror, weight tiling, target, critic step, priorities, target syncs and
   the delayed actor step -- is captured in CUDA graphs over static index / weight / noise buffers (``use_cuda_graph``,
   common/graphed.py); per update the host only walks the PER sum-tree, replays one graph and writes the priorities back.

@@ -1,4 +1,4 @@
-"""MORL/D (decomposition-based MORL) on the B200 update engine -- drop-in for reference
+"""MORL/D (decomposition-based MORL) on the CUDA update engine -- drop-in for reference
 morl_baselines/multi_policy/morld/morld.py with MOSAC inner learners (config 5 of BASELINE.json).
 
 What changes under the API (SURVEY.md section 8, rows a13, a18, a19 and 8(e)):

@@ -1,7 +1,7 @@
 """Thin PyTorch-facing wrappers over the C-ABI (include/morl_b200.h).
 
 PyTorch is plumbing here: it owns the device buffers and the stream; every operator below is one (or two) launches of a
-hand-written sm_100a kernel from libmorl_b200.so.  All wrappers require CUDA tensors and raise otherwise -- there is
+hand-written sm_90a kernel from libmorl_b200.so.  All wrappers require CUDA tensors and raise otherwise -- there is
 no CPU / eager fallback (the CPU restatement lives in oracle/ and is test-only).
 """
 
@@ -315,7 +315,7 @@ def sm_count() -> int:
     return n
 
 
-# ------------------------------------------------------------------------------------------------ tcgen05 dense layers
+# ------------------------------------------------------------------------------------------------ wgmma dense layers
 def _pad(n: int, m: int) -> int:
     return (n + m - 1) // m * m
 
@@ -405,7 +405,7 @@ def gemm_planes(a_planes: th.Tensor, b_planes: th.Tensor, n_out: int, bias: Opti
                 c_planes: Optional[th.Tensor] = None, reverse_tiles: bool = False, a_scale: Optional[th.Tensor] = None,
                 b_scale: Optional[th.Tensor] = None, c_scale: Optional[th.Tensor] = None, split_acc: bool = False,
                 relu_bits_in: Optional[th.Tensor] = None, relu_bits_out: Optional[th.Tensor] = None):
-    """C = act(A . B^T + bias) on the tcgen05 tensor cores with split operands (fp32-accurate).
+    """C = act(A . B^T + bias) on the tensor cores (wgmma) with split operands (fp32-accurate).
     a_planes [P, M, K], b_planes [P, N_pad, K]; the scales are device floats the planes were multiplied by (None = 1);
     ``split_acc``: leading and correction products in separate accumulators (the tensor cores truncate their fp32 accumulation; ~2.5x
     smaller systematic error, ~20 % slower per launch); False (default): one double-buffered accumulator.

@@ -1,4 +1,4 @@
-"""Multi-objective SAC (continuous actions) on the B200 update engine -- drop-in for reference
+"""Multi-objective SAC (continuous actions) on the CUDA update engine -- drop-in for reference
 morl_baselines/single_policy/ser/mosac_continuous_action.py (``MOSoftQNetwork / MOSACActor / MOSAC`` with the same
 constructor, ``update / eval / train / get_buffer / set_buffer / set_weights / get_policy_net / get_save_dict / load``).
 MOSAC is the inner learner of MORL/D (reference multi_policy/morld/morld.py:30-34).
@@ -6,7 +6,7 @@ MOSAC is the inner learner of MORL/D (reference multi_policy/morld/morld.py:30-3
 Hot-path row a13 of SURVEY.md section 8: scalarise both target critics, min, - alpha * logp, scalarise the reward, Bellman
 (mosac_continuous_action.py:435-442) is ONE kernel (morl_actor_critic_td_f32, variant SCALAR_MIN); the minibatch comes from
 the HBM-resident replay mirror with one gather kernel; both target syncs are multi-tensor launches; clip-free Adam steps are the fused
-two-launch optimiser.  The reference's update is ~250 tiny tensor operations (13 ms on its CPU path, 7.7 ms eager on a B200, launch
+two-launch optimiser.  The reference's update is ~250 tiny tensor operations (launch
 bound); here the whole device side of ``update()`` -- gather, critic step, ``policy_freq`` actor / temperature steps, target syncs --
 is captured in CUDA graphs over static index / noise buffers (``use_cuda_graph``, common/graphed.py) and replayed with one host call.
 """

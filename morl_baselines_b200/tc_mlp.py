@@ -1,13 +1,13 @@
-"""Dense layers of the weight-conditioned Q-network on the tcgen05 tensor cores (csrc/gemm_planes.cu).
+"""Dense layers of the weight-conditioned Q-network on the tensor cores (wgmma; csrc/gemm_planes.cu).
 
 ``TCPairMlp`` runs the reference's ``mlp`` stack (common/networks.py:10-48: Linear -> ReLU ... -> Linear) for every
 (observation b, weight vector j) pair of a minibatch without ever materialising fp32 activations in HBM:
 
     layer 1   : u = feats @ W1[:, :F]^T (B rows), v = wset @ W1[:, F:]^T + b1 (W rows)  -- one launch (morl_pair_layer1_uv_f32) --
                  h1[b*W + j] = relu(u[b] + v[j]) written straight into operand planes (morl_pairs_relu_split_planes);
-    layers 2..: the 256-wide hidden layers of a pass as ONE chained launch (morl_gemm_chain_f32: a CTA pair takes its row tiles through
+    layers 2..: the 256-wide hidden layers of a pass as ONE chained launch (morl_gemm_chain_f32: a CTA takes its row tiles through
                  all layers, intermediate activations re-read from L2; both no-grad nets together) -- or, for other widths, one
-                 morl_gemm_planes_f32 launch per layer (TMA -> tcgen05.mma -> TMEM -> epilogue, activation re-split fused in the epilogue);
+                 morl_gemm_planes_f32 launch per layer (TMA -> wgmma -> register accumulators -> epilogue, activation re-split fused in the epilogue);
                  the last layer writes fp32 Q-values (morl_qhead_gemm_f32 when it is <= 32 wide) or is consumed, together with the other
                  network's, by the fused head (morl_qhead_envelope_td_f32: Q never reaches HBM).
 
@@ -320,7 +320,7 @@ TCPairMlp._backward_chained = _backward_chained
 
 
 class TCPairMlpFn(th.autograd.Function):
-    """Q = mlp(pairs(feats, wset)) with the dense layers on the tcgen05 tensor cores, forward and backward."""
+    """Q = mlp(pairs(feats, wset)) with the dense layers on the tensor cores (wgmma), forward and backward."""
 
     @staticmethod
     def forward(ctx, plan: TCPairMlp, feats: th.Tensor, wset: th.Tensor, *params):

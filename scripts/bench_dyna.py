@@ -1,6 +1,6 @@
 """GPI-PD Dyna path (SURVEY 8(f)3) at the reference's default sizes: time of one `_rollout_dynamics` call (25,000 imagined transitions from a
 64-policy support set, every row accepted: the worst case of the insert) and of one `ProbabilisticEnsemble.fit` epoch on 16,384 transitions.
-    python scripts/bench_dyna.py                   B200 engine (needs a GPU)
+    python scripts/bench_dyna.py                   CUDA engine (needs a GPU)
     python scripts/bench_dyna.py --impl reference  the unmodified reference on CPU through oracle/ref_harness (build container only)
 One JSON object on stdout."""
 import json

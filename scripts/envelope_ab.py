@@ -121,7 +121,7 @@ def timed(path, B, W, A, D, sets, out):
     return t_loop, e0.elapsed_time(e1) * 1e-3 / 400
 
 
-for (B, W, A, D) in [(1024, 64, 8, 3), (148, 64, 8, 3), (2048, 64, 8, 3)]:
+for (B, W, A, D) in [(1024, 64, 8, 3), (132, 64, 8, 3), (2048, 64, 8, 3)]:
     sets = [make(B, W, A, D, "plain", 100 + i) for i in range(16)]
     out = th.empty(W * B, D, device=dev)
     alg = 2 * B * W * A * D * 4 + W * D * 4 + B * D * 4 + B * 4 + W * B * D * 4

@@ -1,5 +1,5 @@
-"""Quick probe of the tcgen05 split-operand GEMM on a real B200: correctness on one shape + timing vs cuBLAS fp32 (CUDA events), both
-operand formats.  Also the ncu target of scripts/gpu_*.sh (`-k regex:gemm_planes`)."""
+"""Quick probe of the wgmma split-operand GEMM on an H100: correctness on one shape + timing vs cuBLAS fp32 (CUDA events), both
+operand formats.  Also a profiler target (`-k regex:gemm_planes`)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch as th
@@ -26,6 +26,6 @@ for fmt, name, nprod in fmts:
     print(name, "max abs err", float((c[:4096].double() - ref).abs().max()), "ref max", float(ref.abs().max()))
     t1 = timeit(lambda: ops.gemm_planes(ap, bp, N, bias=bias, relu=True, out_f32=False, out_planes=True, c_planes=cp, a_scale=sa, b_scale=sb, c_scale=sa))
     t2 = timeit(lambda: ops.gemm_planes(ap, bp, N, bias=bias, relu=True, out_f32=True, out_planes=False, c_f32=c, a_scale=sa, b_scale=sb))
-    print(f"tcgen05 {name} -> planes: {t1:.1f} us ({nprod*fl/t1/1e6:.0f} TFLOP/s issued, {fl/t1/1e6:.1f} fp32-equivalent); -> f32: {t2:.1f} us")
+    print(f"wgmma {name} -> planes: {t1:.1f} us ({nprod*fl/t1/1e6:.0f} TFLOP/s issued, {fl/t1/1e6:.1f} fp32-equivalent); -> f32: {t2:.1f} us")
 t3 = timeit(lambda: th.relu(th.addmm(bias, a, b.t())))
 print(f"cuBLAS fp32 addmm+relu: {t3:.1f} us")

@@ -19,7 +19,7 @@ g = th.Generator(device=dev).manual_seed(0)
 if os.environ.get("SAN_ZERO_PLANES") == "1":
     # initcheck does not see the writes of TMA bulk tensor STORES (cp.async.bulk.tensor ... global.shared::cta): plane tensors produced
     # by the GEMM epilogue then look uninitialised to later readers.  Pre-zeroing every plane allocation separates that tool artefact
-    # from a genuine read of memory nobody wrote (profiles/r02_sanitize_initcheck*.txt).
+    # from a genuine read of memory nobody wrote.
     _empty = ops.empty_planes
     ops.empty_planes = lambda *a, **k: _empty(*a, **k).zero_()
 groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain"}

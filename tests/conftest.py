@@ -1,4 +1,4 @@
-"""pytest configuration: the `gpu` marker selects tests that need a real B200 (run by the driver with `-m gpu`)."""
+"""pytest configuration: the `gpu` marker selects tests that need an H100 (`-m gpu`)."""
 
 import os
 import sys
@@ -11,15 +11,15 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); everything else must pass on a CPU-only host")
-    config.addinivalue_line("markers", "unvalidated: new GPU test that has not passed on a B200 yet -- skipped unless MORL_RUN_UNVALIDATED=1, "
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); everything else must pass on a CPU-only host")
+    config.addinivalue_line("markers", "unvalidated: new GPU test that has not passed on an H100 yet -- skipped unless MORL_RUN_UNVALIDATED=1, "
                                        "so that a bring-up failure cannot take the validated suite down with it; the marker is removed once it has passed")
 
 
 def pytest_collection_modifyitems(config, items):
     if os.environ.get("MORL_RUN_UNVALIDATED", "0") == "1":
         return
-    skip = pytest.mark.skip(reason="not yet validated on a B200 (set MORL_RUN_UNVALIDATED=1 to run)")
+    skip = pytest.mark.skip(reason="not yet validated on an H100 (set MORL_RUN_UNVALIDATED=1 to run)")
     for item in items:
         if "unvalidated" in item.keywords:
             item.add_marker(skip)

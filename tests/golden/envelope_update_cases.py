@@ -1,5 +1,5 @@
 """Inputs shared by tests/golden/make_golden_envelope_update.py (run against the unmodified reference in the build container) and
-tests/test_envelope_update_golden_gpu.py (run on the B200): everything derives from numpy PCG64 / MT19937 streams, which are
+tests/test_envelope_update_golden_gpu.py (run on the GPU): everything derives from numpy PCG64 / MT19937 streams, which are
 bit-reproducible across machines, so the fixture stores the reference's initial parameters and outputs only."""
 
 from __future__ import annotations
@@ -21,7 +21,7 @@ CASES = {
 
 
 def fill_agent(agent, c):
-    """Load the synthetic transitions into ``agent.replay_buffer`` (reference or B200 class) with NON-uniform priorities, so the
+    """Load the synthetic transitions into ``agent.replay_buffer`` (reference or engine class) with NON-uniform priorities, so the
     sum-tree walk matters."""
     store = synthetic_store(c["N"], c["obs"], c["A"], c["D"], seed=c["seed"])
     rb = agent.replay_buffer

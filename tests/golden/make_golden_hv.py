@@ -1,7 +1,7 @@
 """Hypervolume-parity reference run (SURVEY.md section 8(d), "HV parity protocol"): the UNMODIFIED reference Envelope is trained on
 CPU on the stand-in MDP (tests/golden/standin_env.py) for a fixed number of environment steps / gradient updates per seed; the
 discounted returns of its greedy policy for a fixed list of evaluation weights, the non-dominated front and its hypervolume are
-frozen into tests/golden/hv_parity.json.  tests/test_hv_parity_gpu.py trains the B200 engine with the same hyper-parameters, seeds,
+frozen into tests/golden/hv_parity.json.  tests/test_hv_parity_gpu.py trains the CUDA engine with the same hyper-parameters, seeds,
 environment and evaluation weights and requires the mean hypervolume to agree within 1 %.
 
     python tests/golden/make_golden_hv.py         (build container only: needs /root/reference)

@@ -1,6 +1,6 @@
 """Stand-in vector-reward MDP for the hypervolume-parity protocol (SURVEY.md section 8(d): "If mo-gymnasium is unavailable on the
 build box, use an in-repo stand-in vector-reward MDP for *both* engines and say so").  mo-gymnasium is not installed here, so the
-reference (CPU, golden generation) and the B200 engine (GPU test) are both trained on this environment.
+reference (CPU, golden generation) and the CUDA engine (GPU test) are both trained on this environment.
 
 TreasureChain: a 3-objective chain in the spirit of deep-sea-treasure.  Positions x = 0..2; every step costs TIME_COST units of
 time (objective 2).  Actions: 0 = move right (walking off the end of the chain terminates the episode empty-handed), 1 = collect

@@ -1,5 +1,5 @@
 """Host-side model of the work schedule of the chained hidden-layer launch (csrc/gemm_planes.cu: gemm_chain_kernel -- the `unit_of` enumeration
-every role of a CTA pair walks).  Checks, for the shapes the update uses and for ragged ones, what the kernel relies on and what DESIGN.md
+every role of a CTA walks).  Checks, for the shapes the update uses and for ragged ones, what the kernel relies on and what DESIGN.md
 section 4.6 claims:
   * every (chain, tile, layer) unit is processed exactly once over all pairs, all layers of a (chain, tile) by the SAME pair (the next layer
     re-loads what the pair itself stored), in layer order, and the lane of a unit -- the `stored[lane]` barrier its producer waits on -- is the

@@ -2,12 +2,12 @@
 
 tests/golden/envelope_update.npz holds what the reference's ``Envelope.update()`` (multi_policy/envelope/envelope.py:266-367) produced on
 CPU for the north-star shape (obs 32, |A| 8, d 3, |W| 64, B 1024, 4x256), for BASELINE configs[1] (minecart dims, |W| 32, B 256) and
-for a homotopy-schedule run (tests/golden/make_golden_envelope_update.py).  Here the CUDA engine -- device replay gather, tcgen05 dense
+for a homotopy-schedule run (tests/golden/make_golden_envelope_update.py).  Here the CUDA engine -- device replay gather, tensor-core dense
 layers on the B*|W| distinct rows (74-pair persistent schedule, tail split, snake order at the north-star shape), fused envelope-TD,
 fused loss / priorities, hand-written backward, fused clip + Adam, CUDA-graph replay -- runs the same updates from the same initial
 parameters, replay store, sum-tree and RNG streams.
 
-Bounds (BASELINE.json north_star: "Q-values and losses within 1e-5 relative fp32"; measured values: profiles/r02_golden_diag*.txt):
+Bounds (BASELINE.json north_star: "Q-values and losses within 1e-5 relative fp32"):
   * sampled indices, weight sets            : identical (host RNG mirror: global numpy RNG for the sum-tree walk, agent.np_random for the weights)
   * critic loss                             : 1e-5 relative (measured 0 .. 7e-7)
   * priorities (|w . td| + min_p)^alpha     : |p - p_ref| <= 1e-5 |p_ref| + 2e-6 on >= 99 % of the B rows (measured: 0 .. 7 of 1024 rows outside).
@@ -108,5 +108,5 @@ def test_north_star_update_bf16x3_operand_format(cuda):
 
 
 def test_north_star_update_split_accumulators(cuda):
-    """The higher-accuracy accumulator mode of the forward GEMMs (leading / correction products in separate TMEM buffers)."""
+    """The higher-accuracy accumulator mode of the forward GEMMs (leading / correction products in separate accumulators)."""
     _run_case("north_star", cuda, True, True, tensor_core_accumulators="split")

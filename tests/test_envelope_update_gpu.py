@@ -1,5 +1,5 @@
 """Whole-update parity of morl_baselines_b200.Envelope (CUDA: device replay gather, Q on B*|W| rows, fused envelope-TD, fused
-loss, CUDA-graph replay, optional tcgen05 dense layers) against the PyTorch-CPU port of the reference update
+loss, CUDA-graph replay, optional tensor-core dense layers) against the PyTorch-CPU port of the reference update
 (oracle/envelope_update_port.py, itself pinned bit-for-bit to the unmodified reference in tests/test_port_vs_reference.py).
 
 Tolerance (BASELINE.json north_star): losses and parameters within 1e-5 relative; priorities within 1e-5 relative (they are
@@ -69,7 +69,7 @@ def test_envelope_update_matches_reference_port(cuda, per, tc, graph):
 
 @pytest.mark.parametrize("graph", [False, True])
 def test_envelope_update_single_tile_shape(cuda, graph):
-    """B * |W| = 128 rows: exactly one 128-row tile, the ONE-CTA GEMM kernel (the CTA-pair kernel needs two) with every epilogue flavour
+    """B * |W| = 128 rows: exactly one 128-row tile, a one-CTA launch of the GEMM kernel with every epilogue flavour
     of the update -- hidden layers, ReLU mask, fp32 output -- on a 4 x 256 net (the hypervolume-parity training configuration)."""
     # (4 x 256 net: 140k parameters; Adam's first steps turn the ~1e-8 rounding noise of the smallest gradient elements into ~1e-5 parameter
     # differences on a handful of them -- tests/test_envelope_update_golden_gpu.py states the full bound)

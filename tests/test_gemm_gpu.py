@@ -1,4 +1,4 @@
-"""GPU tests of the tcgen05 split-operand GEMMs (csrc/gemm_planes.cu) against a float64 reference, for both operand formats:
+"""GPU tests of the wgmma split-operand GEMMs (csrc/gemm_planes.cu) against a float64 reference, for both operand formats:
 f16x2 (two fp16 planes of a power-of-two-scaled operand, three MMAs) and bf16x3 (three bf16 planes, six MMAs).
 
 Tolerance: the expansions are exact to ~2^-22 (f16x2) / 2^-24 (bf16x3) per product and accumulate in fp32, so the result must agree
@@ -335,10 +335,10 @@ def test_pairs_grad_reduce(cuda, fmt):
         np.testing.assert_allclose(dV.cpu().numpy(), ref.sum(0).cpu().numpy(), rtol=1e-5, atol=1e-5)
 
 
-@pytest.mark.parametrize("env_flags", [{"MORL_GEMM_FORCE_1CTA": "1"}, {"MORL_GEMM_SPLIT_ACC": "1"}, {"MORL_GEMM_FORCE_1CTA": "1", "MORL_GEMM_SPLIT_ACC": "1"}])
+@pytest.mark.parametrize("env_flags", [{"MORL_GEMM_L2HINT": "1"}, {"MORL_GEMM_SPLIT_ACC": "1"}, {"MORL_GEMM_L2HINT": "1", "MORL_GEMM_SPLIT_ACC": "1"}])
 def test_gemm_alternative_kernels_still_correct(cuda, env_flags):
-    """Large shapes use the CTA-pair (cta_group::2) kernel; MORL_GEMM_FORCE_1CTA=1 keeps the one-CTA kernel alive and MORL_GEMM_SPLIT_ACC=1
-    forces the split-accumulator mode on every call (cross-checks).  The switches are read once per process, hence the subprocess."""
+    """MORL_GEMM_L2HINT=1 puts L2 eviction hints on the operand loads and MORL_GEMM_SPLIT_ACC=1
+    forces the split-accumulator mode on every call (a 256-wide output then runs as two 128-column units, a 160-wide one as 128 + 32) -- cross-checks.  The switches are read once per process, hence the subprocess."""
     import os
     import subprocess
     import sys
@@ -354,12 +354,14 @@ def test_gemm_alternative_kernels_still_correct(cuda, env_flags):
         "    sb = ops.scale_tensor(1024.0, 'cuda') if fmt == ops.FMT_F16X2 else None\n"
         "    c, _ = ops.gemm_planes(ops.split_planes(a, fmt, scale=sa), ops.split_planes(b, fmt, scale=sb), 256, a_scale=sa, b_scale=sb)\n"
         "    err = float((c.double() - ref).abs().max()); print('ERR', fmt, err); assert err < 2e-5\n"
+        "    c, _ = ops.gemm_planes(ops.split_planes(a, fmt, scale=sa), ops.split_planes(b[:160].contiguous(), fmt, scale=sb), 160, a_scale=sa, b_scale=sb)\n"
+        "    err = float((c.double() - ref[:, :160]).abs().max()); print('N160', fmt, err); assert err < 2e-5\n"
     )
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     env = dict(os.environ, PYTHONPATH=root, **env_flags)
     r = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stdout + r.stderr
-    assert r.stdout.count("ERR") == 2
+    assert r.stdout.count("ERR") == 2 and r.stdout.count("N160") == 2
 
 
 @pytest.mark.parametrize("fmt", FMTS)

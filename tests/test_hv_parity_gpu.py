@@ -3,7 +3,7 @@ reference after equal updates").
 
 The unmodified reference Envelope was trained on CPU in the build container (tests/golden/make_golden_hv.py -> hv_parity.json) on
 the stand-in vector-reward MDP of tests/golden/standin_env.py (mo-gymnasium is not installed, so BOTH engines use the stand-in, as
-the protocol prescribes).  Here the B200 engine is trained with the same hyper-parameters, seeds, environment, number of
+the protocol prescribes).  Here the CUDA engine is trained with the same hyper-parameters, seeds, environment, number of
 environment steps (= gradient updates) and evaluation-weight list; both fronts go through the same exact hypervolume routine.
 Bar: |mean_seeds HV_b200 - mean_seeds HV_ref| / mean HV_ref <= 1 %  (3 seeds).
 """

@@ -2,11 +2,11 @@
 the last-layer epilogue, reference multi_policy/envelope/envelope.py:420-440 + :298).
 
 The kernel must be BIT-IDENTICAL to the three-launch chain it replaces (morl_gemm_planes_f32 for each net, then morl_envelope_td_f32):
-  * its Q tiles (optional fp32 copies) equal the unfused output-layer GEMM bit for bit (same MMA order in tensor memory, same epilogue fma);
+  * its Q tiles (optional fp32 copies) equal the unfused output-layer GEMM bit for bit (same MMA order, same epilogue fma);
   * targets / preference indices / action indices equal the standalone operator's on those Q tensors AND the CPU oracle's
     (integer outputs and fp32 targets: exact equality, no tolerance);
   * Envelope.update() with the fused head produces exactly the losses, priorities and parameters of the update without it.
-Shapes: the north-star (B=1024, |W|=64, |A|=8, d=3, K=256: 512 tiles on 148 CTAs, every ring / accumulator phase wraps), BASELINE
+Shapes: the north-star (B=1024, |W|=64, |A|=8, d=3, K=256: 512 tiles on 132 CTAs, every ring phase wraps), BASELINE
 configs[1] (minecart dims: |W|=32, |A|=6, N=18 -- ragged Q rows, four transitions per tile), small / odd ones, constant Q (every
 candidate ties: first occurrence), both row orders, the three scalarisation arithmetics."""
 
