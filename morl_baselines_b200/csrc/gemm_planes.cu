@@ -15,15 +15,17 @@
 //       exact to 2^-24; SIX MMAs  A2B0 + A0B2 + A1B1 + A1B0 + A0B1 + A0B0, 6 bytes per element.
 // Either way the result differs from an fp32 GEMM only at the level of its own accumulation-order noise (tests/test_gemm_gpu.py).
 //
-// K-major kernel anatomy (persistent, one CTA per SM, 288 threads):
+// K-major kernel anatomy (persistent, one CTA per SM, 384 threads = three warpgroups; setmaxnreg moves the registers of the producer
+// warpgroup to the consumers: 232 per consumer thread, 40 per producer thread, so the 128 accumulators and the epilogue fit without spills):
 //   warps 0-7: two consumer warpgroups -- each owns 64 of the tile's 128 rows: waits for a stage, issues NPROD x BK/16
 //              wgmma.mma_async (M = 64, N = unit width, K = 16) from the staged boxes and hands the stage back to the producer once the
 //              MMAs that read it have completed; the accumulators (N / 2 fp32 registers per thread) then go through the epilogue in place:
 //              x 2^-(sA+sB), + bias, ReLU / ReLU-mask, then an fp32 row-major store and/or a re-split into planes (the operand format
-//              of the next layer) through a TMA store, so intermediate activations never exist in fp32 in HBM;
-//   warp 8   : TMA producer    -- cp.async.bulk.tensor.3d of a [P planes x 128 rows x BK] A box and P x N/32 [32 rows x BK] B boxes per stage
-//              (f16x2: BK = 64, 128-byte swizzle, 2 x 96 KB stages at N = 256; bf16x3: BK = 32, 64-byte swizzle, 2 x 72 KB), mbarrier
-//              ring; it keeps loading the next tile while the consumers are in their epilogue.
+//              of the next layer) through TMA stores from two staging tiles per warp used in turn, so intermediate activations never
+//              exist in fp32 in HBM;
+//   warps 8-11: producer warpgroup, one lane of warp 8 issues TMA -- cp.async.bulk.tensor.3d of a [P planes x 128 rows x BK] A box and
+//              P x N/32 [32 rows x BK] B boxes per stage (f16x2: BK = 64, 128-byte swizzle, 2 x 96 KB stages at N = 256; bf16x3: BK = 32,
+//              64-byte swizzle, 2 x 72 KB), mbarrier ring; it keeps loading the next tile while the consumers are in their epilogue.
 // Operands: A [P][M][K] (K-major), B [P][N_pad][K] (K-major), K % BK == 0, N_pad % 32 == 0, N_pad <= 256.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -37,7 +39,9 @@
 namespace morl {
 
 constexpr int kGemmBM = 128;
-constexpr int kGemmThreads = 288;  // warps 0-7: two consumer warpgroups (wgmma + epilogue), warp 8: TMA producer
+constexpr int kGemmThreads = 384;  // warps 0-7: two consumer warpgroups (wgmma + epilogue), warps 8-11: producer warpgroup (one lane of warp 8 issues TMA)
+// 2 x 128 x 232 + 128 x 40 = 64,512 <= 65,536 registers: a consumer thread holds 128 fp32 accumulators and the epilogue's working set without spilling
+constexpr int kGemmConsumerRegs = 232, kGemmProducerRegs = 40;
 constexpr int kGemmBoxN = 32;      // B rows per TMA box (one plane): any unit width that is a multiple of 32 is a sequence of them
 
 __device__ unsigned int g_plane_overflow;  // number of kernel launches (approx.) that saw an f16x2 element out of fp16 range
@@ -92,12 +96,13 @@ struct KPlan {
     static constexpr uint32_t kRowB = F::BK * 2;                                  // bytes per staged row = swizzle span
     static constexpr uint32_t kAStage = F::P * kGemmBM * kRowB;                   // A box bytes
     static constexpr uint32_t kBStage = F::P * 256 * kRowB;                       // B bytes of a stage at N_pad = 256
-    static constexpr uint32_t kStageC = F::P * 1024;                              // per-consumer-warp TMA-store tile: P x 16 rows x 64 B
+    static constexpr uint32_t kStageC = F::P * 1024;                              // TMA-store tile: P x 16 rows x 64 B; TWO per consumer warp
     static constexpr uint32_t kOffB = kStages * kAStage;
     static constexpr uint32_t kOffC = kOffB + kStages * kBStage;                  // 1024-aligned (all stage sizes are multiples of 1 KB)
-    static constexpr uint32_t kOffBar = kOffC + 8 * kStageC;
+    static constexpr uint32_t kOffBar = kOffC + 8 * 2 * kStageC;
     static constexpr uint32_t kOffBias = kOffBar + 256;
     static constexpr uint32_t kBytes = kOffBias + 1024 + 1024;                    // + alignment slack of the dynamic segment
+    static_assert(kBytes <= 227 * 1024, "dynamic shared memory of one CTA on sm_90");
 };
 
 // One work unit of a consumer warpgroup: D[64 x N] = sum over the K blocks of the staged planes, NPROD products per K step in the order of
@@ -167,10 +172,11 @@ struct EpiArgs {
 };
 
 // Epilogue of one 32-column chunk of a consumer warp's 16 accumulator rows [rbase, rbase + 16): thread l holds a[4 q + 2 h + e] = column
-// col0 + 8 q + 2 (l % 4) + e of row rbase + l / 4 + 8 h (the wgmma fragment).
+// col0 + 8 q + 2 (l % 4) + e of row rbase + l / 4 + 8 h (the wgmma fragment).  The re-split planes leave through the warp's two staging tiles in
+// turn (n_stored counts the warp's bulk stores): a chunk is staged while the TMA store of the previous one is still reading the other tile.
 template <int FMT>
 __device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, int rbase, int lane, const EpiArgs& e, const CUtensorMap* tmC,
-                                               uint8_t* my_stage, float& amax) {
+                                               uint8_t* my_stage, uint32_t& n_stored, float& amax) {
     using F = PlaneFmt<FMT>;
     constexpr int P = F::P;
     const int l4 = lane & 3, lr = lane >> 2;
@@ -247,7 +253,9 @@ __device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, i
     if (e.planes && col0 < e.ldp) {
         // stage the warp's [16 rows x 32 cols] x P planes in shared memory (TMA SWIZZLE_64B pattern: 16-byte chunk index XOR ((row >> 1) & 3),
         // bank-conflict free), then ONE bulk tensor store writes it out coalesced and asynchronously
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // previous store has read the staging tile
+        uint8_t* tile = my_stage + (n_stored & 1u) * (uint32_t)(P * 1024);
+        ++n_stored;
+        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");  // the store before the previous one has read this tile
         __syncwarp();
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -259,7 +267,7 @@ __device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, i
                 const float x0 = col < e.N ? x[h][2 * q] * e.c_mul : 0.f, x1 = col + 1 < e.N ? x[h][2 * q + 1] * e.c_mul : 0.f;
                 uint32_t w[P];
                 F::split2(x0, x1, w, amax);  // re-split (c_scale x) into P planes, two columns per word
-                uint8_t* st = my_stage + rl * 64 + ((q ^ ((rl >> 1) & 3)) << 4) + 4 * l4;
+                uint8_t* st = tile + rl * 64 + ((q ^ ((rl >> 1) & 3)) << 4) + 4 * l4;
 #pragma unroll
                 for (int p = 0; p < P; ++p) *reinterpret_cast<uint32_t*>(st + p * 1024) = w[p];
             }
@@ -267,7 +275,7 @@ __device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, i
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncwarp();
         if (lane == 0) {
-            asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(tmC), "r"(g_smem_u32(my_stage)),
+            asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(tmC), "r"(g_smem_u32(tile)),
                          "r"(col0), "r"(rbase), "r"(0)
                          : "memory");
             asm volatile("cp.async.bulk.commit_group;" ::: "memory");
@@ -334,9 +342,10 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     for (int t = threadIdx.x; t < 256; t += blockDim.x) bias_s[t] = (g.bias && t < g.N) ? g.bias[t] : 0.f;
     __syncthreads();
 
-    if (warp == 8) {
-        // ================= TMA producer =================
-        if (lane == 0) {
+    if (warp >= 8) {
+        // ================= producer warpgroup: one lane issues TMA =================
+        warpgroup_reg_dec<kGemmProducerRegs>();
+        if (warp == 8 && lane == 0) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
             uint32_t stage = 0, phase = 0;
@@ -371,8 +380,10 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         }
     } else {
         // ================= consumer warpgroups (warps 0..7) =================
+        warpgroup_reg_inc<kGemmConsumerRegs>();
         const int wg = warp >> 2;
-        uint8_t* my_stage = stage_c + warp * L::kStageC;
+        uint8_t* my_stage = stage_c + warp * 2 * L::kStageC;
+        uint32_t n_stored = 0;
         // x = acc / (sA sB) + bias; when only planes are written (the hidden layers) the output scale is FOLDED into the two constants:
         // fold * x = acc * (fold / (sA sB)) + fold * bias (exact, powers of two), and max / mask commute with a positive factor
         const float c_mul = ld_scale(g.c_scale);
@@ -419,7 +430,7 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
                     float a[16];
 #pragma unroll
                     for (int j = 0; j < 16; ++j) a[j] = SPLIT ? __fadd_rn(acc[16 * c + j], acc[64 + 16 * c + j]) : acc[16 * c + j];
-                    epilogue_chunk<FMT>(a, n_begin + 32 * c, rbase, lane, e, &tmC, my_stage, amax);
+                    epilogue_chunk<FMT>(a, n_begin + 32 * c, rbase, lane, e, &tmC, my_stage, n_stored, amax);
                 }
             }
             if (g.stats) busy += clock64() - c1;
@@ -524,9 +535,10 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
     }
     __syncthreads();
 
-    if (warp == 8) {
-        // ================= TMA producer =================
-        if (lane == 0) {
+    if (warp >= 8) {
+        // ================= producer warpgroup: one lane issues TMA =================
+        warpgroup_reg_dec<kGemmProducerRegs>();
+        if (warp == 8 && lane == 0) {
             uint32_t stage = 0, phase = 0;
             uint32_t done_on_lane[kChainLanes] = {0u, 0u, 0u, 0u};  // units already issued on each lane = completions of stored[lane] to expect
             for (int gi = 0; gi < n_groups; ++gi)
@@ -560,8 +572,10 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
         }
     } else {
         // ================= consumer warpgroups (warps 0..7) =================
+        warpgroup_reg_inc<kGemmConsumerRegs>();
         const int wg = warp >> 2;
-        uint8_t* my_stage = stage_c + warp * L::kStageC;
+        uint8_t* my_stage = stage_c + warp * 2 * L::kStageC;
+        uint32_t n_stored = 0;
         const float s_act = ld_scale(g.a_scale);
         float amax = 0.f;
         float acc[128];
@@ -591,7 +605,7 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
                         float a[16];
 #pragma unroll
                         for (int j = 0; j < 16; ++j) a[j] = acc[16 * c + j];
-                        epilogue_chunk<FMT>(a, 32 * c, rbase, lane, e, &maps.C[job], my_stage, amax);
+                        epilogue_chunk<FMT>(a, 32 * c, rbase, lane, e, &maps.C[job], my_stage, n_stored, amax);
                     }
                     // the lane's next layer loads what this unit stored (bit masks included): signal once the bulk stores of this warp have completed
                     __syncwarp();
@@ -633,13 +647,21 @@ struct GemmMnArgs {
     float* colsum_partial;  // [S][n_tiles*128] or nullptr: per-split column sums of G (bias gradient), fused as G^T . ones
 };
 
-// the K loop of one consumer warpgroup: acc[64 x NB] += G_chunk^T . H over the stages; cs[64 x 16] += G_chunk^T . ones
-template <int FMT, int NB>
-__device__ __forceinline__ void mma_mn_unit(float (&acc)[128], float (&cs)[8], bool colsum, uint8_t* smA, uint8_t* smB, uint32_t a_stage, uint32_t b_stage,
+// One consumer warpgroup of the weight-gradient kernel: acc[64 x NB] = G_chunk^T . H over the stages (cs[64 x 16] = G_chunk^T . ones), then the
+// fp32 partial tile of this split.  NB and COLSUM are template parameters and the accumulators live in this function only: a run-time
+// branch between the wgmma of one commit group, or one 128-register accumulator array shared by the instantiations of all widths, makes
+// ptxas serialise the wgmma (its remarks C7519 / C7511).
+template <int FMT, int NB, bool COLSUM>
+__device__ __forceinline__ void mma_mn_unit(const GemmMnArgs& g, int split, int row, uint8_t* smA, uint8_t* smB, uint32_t a_stage, uint32_t b_stage,
                                             uint32_t chunk_bytes, uint64_t ones_desc, int n_kblk, uint64_t* full, uint64_t* empty, int wg, int lane) {
     using F = PlaneFmt<FMT>;
     constexpr int P = F::P;
     constexpr uint32_t plane = kMnKT * 128u;  // 4 KB: one plane of one chunk
+    float acc[NB / 2], cs[8];
+#pragma unroll
+    for (int i = 0; i < NB / 2; ++i) acc[i] = 0.f;  // (a split without rows writes zeros)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) cs[i] = 0.f;
     uint32_t stage = 0, phase = 0, prev = 0;
     for (int kb = 0; kb < n_kblk; ++kb) {
         g_mbar_wait(&full[stage], phase);
@@ -654,7 +676,7 @@ __device__ __forceinline__ void mma_mn_unit(float (&acc)[128], float (&cs)[8], b
                 const uint64_t bd = make_desc_mn_sw128(b0 + F::pb(t) * plane + ks * 2048u, chunk_bytes);
                 Wgmma<NB>::template mma<FMT, 1, 1>(acc, ad, bd, (kb | ks | t) != 0 ? 1u : 0u);
             }
-            if (colsum) {  // (G_{P-1} + ... + G_0)^T . ones -> 16 identical columns
+            if constexpr (COLSUM) {  // (G_{P-1} + ... + G_0)^T . ones -> 16 identical columns
 #pragma unroll
                 for (int pl = P - 1; pl >= 0; --pl)
                     Wgmma<16>::template mma<FMT, 1, 1>(cs, make_desc_mn_sw128(a0 + pl * plane + ks * 2048u, chunk_bytes), ones_desc,
@@ -673,6 +695,14 @@ __device__ __forceinline__ void mma_mn_unit(float (&acc)[128], float (&cs)[8], b
         }
     }
     wgmma_wait<0>();
+    const int l4 = lane & 3;  // this thread holds output rows (n) row and row + 8
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        float* prow = g.partial + ((size_t)split * g.n_tiles * 128 + row + 8 * h) * NB + 2 * l4;
+#pragma unroll
+        for (int j = 0; j < NB / 8; ++j) *reinterpret_cast<float2*>(prow + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        if (COLSUM && l4 == 0) g.colsum_partial[(size_t)split * g.n_tiles * 128 + row + 8 * h] = cs[2 * h];
+    }
 }
 
 template <int FMT>
@@ -717,8 +747,9 @@ gemm_planes_mn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     __syncthreads();
     pdl_enter();  // (nothing above reads or writes global memory: barriers and the tile of ones overlap the predecessor)
 
-    if (warp == 8) {
-        if (lane == 0) {
+    if (warp >= 8) {
+        warpgroup_reg_dec<kGemmProducerRegs>();
+        if (warp == 8 && lane == 0) {
             uint32_t stage = 0, phase = 0;
             for (int kb = 0; kb < n_kblk; ++kb) {
                 g_mbar_wait(&empty[stage], phase ^ 1u);
@@ -733,30 +764,21 @@ gemm_planes_mn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
             }
         }
     } else {
-        const int wg = warp >> 2, l4 = lane & 3;
-        float acc[128], cs[8];
-#pragma unroll
-        for (int i = 0; i < 128; ++i) acc[i] = 0.f;  // (a split without rows writes zeros)
-#pragma unroll
-        for (int i = 0; i < 8; ++i) cs[i] = 0.f;
+        warpgroup_reg_inc<kGemmConsumerRegs>();
+        const int wg = warp >> 2;
         const uint64_t ones_desc = make_desc_mn_sw128(g_smem_u32(ones), chunk_bytes);
         const bool colsum = g.colsum_partial != nullptr;
-#define MORL_UNIT(N_) \
-    case N_: mma_mn_unit<FMT, N_>(acc, cs, colsum, smA, smB, a_stage, b_stage, chunk_bytes, ones_desc, n_kblk, full, empty, wg, lane); break;
+        const int row = nt * 128 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#define MORL_UNIT(N_)                                                                                                                               \
+    case N_:                                                                                                                                        \
+        if (colsum) mma_mn_unit<FMT, N_, true>(g, split, row, smA, smB, a_stage, b_stage, chunk_bytes, ones_desc, n_kblk, full, empty, wg, lane);  \
+        else mma_mn_unit<FMT, N_, false>(g, split, row, smA, smB, a_stage, b_stage, chunk_bytes, ones_desc, n_kblk, full, empty, wg, lane);        \
+        break;
         switch (g.NB) {
             MORL_UNIT(64) MORL_UNIT(128) MORL_UNIT(192) MORL_UNIT(256)
             default: __trap();
         }
 #undef MORL_UNIT
-        const int row = nt * 128 + wg * 64 + (warp & 3) * 16 + (lane >> 2);  // output row (n); this thread also holds row + 8
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            float* prow = g.partial + ((size_t)split * g.n_tiles * 128 + row + 8 * h) * g.NB + 2 * l4;
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-                if (8 * j < g.NB) *reinterpret_cast<float2*>(prow + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-            if (colsum && l4 == 0) g.colsum_partial[(size_t)split * g.n_tiles * 128 + row + 8 * h] = cs[2 * h];
-        }
     }
 }
 

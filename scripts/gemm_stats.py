@@ -28,11 +28,15 @@ e0.record(); run(n); e1.record(); th.cuda.synchronize()
 lib.morl_debug_gemm_stats(buf, 1)
 us = e0.elapsed_time(e1) / n * 1e3
 sm = ops.sm_count()
-pairs = sm // 2
-mhz = 1965.0
-c = [float(x) for x in buf]
-print(f"format {'bf16x3' if fmt == ops.FMT_BF16X3 else 'f16x2'}, accumulators {'split' if os.environ.get('MORL_GEMM_SPLIT_ACC') == '1' else 'single'}")
-print(f"launch {us:.1f} us = {us * mhz:.0f} cycles @ {mhz:.0f} MHz (stats add a little overhead)")
-print(f"MMA thread (per leader, per launch): total {c[2] / pairs / n:.0f} cyc, waiting TMA {c[0] / pairs / n:.0f}, waiting epilogue {c[1] / pairs / n:.0f}")
-print(f"TMA thread (per CTA): waiting for a free stage {c[3] / sm / n:.0f} cyc")
-print(f"epilogue warp (per CTA): waiting for accumulator {c[4] / sm / n:.0f} cyc, busy {c[5] / sm / n:.0f} cyc")
+ctas = min(sm, (M + 127) // 128)
+tiles = (M + 127) // 128 / ctas  # tiles per CTA and launch
+# GemmArgs::stats: [0] consumer cycles waiting for TMA, [1] consumer loop total, [2] producer waiting for a free stage, [3] epilogue busy;
+# [0], [1], [3] are written by consumer warp 0 of every CTA, [2] by the producer thread
+wait_tma, total, wait_free, epi = (float(buf[i]) / ctas / n for i in range(4))
+print(f"format {'bf16x3' if fmt == ops.FMT_BF16X3 else 'f16x2'}, accumulators {'split' if os.environ.get('MORL_GEMM_SPLIT_ACC') == '1' else 'single'}, "
+      f"{th.cuda.get_device_name(0)}")
+print(f"launch {us:.1f} us on {ctas} CTAs, {tiles:.2f} tiles per CTA (the counters add a little overhead)")
+print(f"consumer warp (per CTA, per launch): total {total:.0f} cyc = {total / tiles:.0f} per tile; waiting for TMA {wait_tma:.0f} = {wait_tma / tiles:.0f} per tile "
+      f"({wait_tma / total:.2f}); epilogue busy {epi:.0f} = {epi / tiles:.0f} per tile ({epi / total:.2f}); "
+      f"issuing / waiting for MMAs {(total - wait_tma - epi) / tiles:.0f} per tile ({(total - wait_tma - epi) / total:.2f})")
+print(f"producer thread (per CTA, per launch): waiting for a free stage {wait_free:.0f} cyc = {wait_free / tiles:.0f} per tile ({wait_free / total:.2f} of the consumer total)")
