@@ -73,37 +73,38 @@ def test_forward_and_dx_forms_do_not_depend_on_tile_order(cuda, fmt, M, N, K):
 @pytest.mark.parametrize("n_chains", [1, 2])
 @pytest.mark.parametrize("M", [65536, 32800, 1280])  # 257 tiles (ragged last one); 1280: fewer tiles than CTAs
 def test_dx_chain_equals_per_layer_launches(cuda, fmt, n_chains, M):
-    """The backward form of the chained launch (no ReLU, outputs masked by recorded ReLU bits, first layer reading a 64-wide input) against
-    one launch per layer: every plane tensor bit for bit."""
+    """The backward form of the chained launch (no ReLU, outputs masked by recorded ReLU bits, first layer reading the padded dL/dQ: 64,
+    128 or 256 wide for output layers of <= 64, <= 128 and <= 256 columns) against one launch per layer: every plane tensor bit for bit."""
     from morl_baselines_b200 import ops
 
-    H, K0, n_layers = 256, 64, 3
+    H, n_layers = 256, 3
     g = th.Generator(device=cuda).manual_seed(M + n_chains)
     sa = _scale(fmt, 64.0, cuda)
-    acts, weights, scales, masks, refs = [], [], [], [], []
-    for c in range(n_chains):
-        a0 = ops.split_planes(th.randn(M, K0, device=cuda, generator=g) * 1e-2, fmt, scale=sa)
-        ws, sws, ms = [], [], []
-        for l in range(n_layers):
-            k = K0 if l == 0 else H
-            sw = _scale(fmt, 1024.0 * (1 + l), cuda)
-            ws.append(ops.split_planes(th.randn(H, k, device=cuda, generator=g) / 16, fmt, scale=sw))
-            sws.append(sw)
-            ms.append(th.randint(-2**31, 2**31 - 1, (M, 8), device=cuda, generator=g, dtype=th.int64).to(th.int32))
-        a, ref = a0, []
-        for l in range(n_layers):
-            _, a = ops.gemm_planes(a, ws[l], H, out_f32=False, out_planes=True, a_scale=sa, b_scale=sws[l], c_scale=sa, relu_bits_in=ms[l])
-            ref.append(a)
-        acts.append([a0] + [ops.empty_planes(fmt, M, H, cuda).zero_() for _ in range(n_layers)])
-        weights.append(ws); scales.append(sws); masks.append(ms); refs.append(ref)
-    chain = ops.GemmChain(acts, weights, None, None if fmt != ops.FMT_F16X2 else scales, None, act_scale=sa, relu=False, bits_in=masks, k_first=K0)
-    for _ in range(2):
-        chain()
-    th.cuda.synchronize()
-    for c in range(n_chains):
-        for l in range(n_layers):
-            assert th.equal(acts[c][l + 1].view(th.int16), refs[c][l].view(th.int16)), f"planes differ: chain {c} layer {l}"
-        assert float(refs[c][-1].float().abs().max()) > 0
+    for K0 in (64, 128, 256):
+        acts, weights, scales, masks, refs = [], [], [], [], []
+        for c in range(n_chains):
+            a0 = ops.split_planes(th.randn(M, K0, device=cuda, generator=g) * 1e-2, fmt, scale=sa)
+            ws, sws, ms = [], [], []
+            for l in range(n_layers):
+                k = K0 if l == 0 else H
+                sw = _scale(fmt, 1024.0 * (1 + l), cuda)
+                ws.append(ops.split_planes(th.randn(H, k, device=cuda, generator=g) / 16, fmt, scale=sw))
+                sws.append(sw)
+                ms.append(th.randint(-2**31, 2**31 - 1, (M, 8), device=cuda, generator=g, dtype=th.int64).to(th.int32))
+            a, ref = a0, []
+            for l in range(n_layers):
+                _, a = ops.gemm_planes(a, ws[l], H, out_f32=False, out_planes=True, a_scale=sa, b_scale=sws[l], c_scale=sa, relu_bits_in=ms[l])
+                ref.append(a)
+            acts.append([a0] + [ops.empty_planes(fmt, M, H, cuda).zero_() for _ in range(n_layers)])
+            weights.append(ws); scales.append(sws); masks.append(ms); refs.append(ref)
+        chain = ops.GemmChain(acts, weights, None, None if fmt != ops.FMT_F16X2 else scales, None, act_scale=sa, relu=False, bits_in=masks, k_first=K0)
+        for _ in range(2):
+            chain()
+        th.cuda.synchronize()
+        for c in range(n_chains):
+            for l in range(n_layers):
+                assert th.equal(acts[c][l + 1].view(th.int16), refs[c][l].view(th.int16)), f"planes differ: K0 {K0} chain {c} layer {l}"
+            assert float(refs[c][-1].float().abs().max()) > 0
 
 
 def test_overflow_in_the_epilogue_is_still_flagged(cuda):
