@@ -32,6 +32,19 @@
  *                         north-star shape can be matched bit-for-bit.
  *      MORL_DOT_FMA     : fma(w2,q2, fma(w1,q1, fl(w0*q0)))   the GPU-native chain (what cuBLAS would do).
  *   argmax / argmin are always FIRST-occurrence (th.max / th.argmax / th.argmin semantics).
+ *
+ * Selection rules of the four per-row targets below (greedy_td, critic_min_td, gpi_envelope, actor_critic_td):
+ *   - ties: the argmax over candidates keeps the lowest index among equal scores (for gpi_envelope the joint index
+ *     p*A + a, also when the tied candidates are walked by different lanes); the argmin over nets keeps the lowest net;
+ *   - NaN: the argmax starts from -inf and only a strictly greater score replaces it, so a NaN score never wins.  The
+ *     argmin over nets starts from net 0's score: a NaN at a later net never replaces it, a NaN at net 0 stays and then
+ *     loses the argmax.  (th.argmax / th.argmin would return the NaN; the two differ only once values have diverged.)
+ *     MORL_AC_ELEMENTWISE_MIN and MORL_AC_SCALAR_MIN take fminf, which ignores a NaN operand;
+ *   - -inf: a row whose every score is -inf or NaN takes candidate 0 (action 0; for critic_min_td / gpi_envelope with
+ *     the critic-min net of that candidate), as th.argmax does for an all -inf row;
+ *   - w_map / r_map address w [w_rows, D] and reward / done [r_rows] by the row-index maps above: TILE row k % rows,
+ *     BLOCK row k / (N / rows) (N = B for gpi_envelope); rows must divide N, and rows == N or rows == 1 mean the same
+ *     under both maps.
  */
 #ifndef MORL_B200_H_
 #define MORL_B200_H_
@@ -161,6 +174,8 @@ MORL_API int morl_td_mse_priority_f32(const float* q_values, const int32_t* acti
  *   target_q_gpi : f32 [N, D] or NULL (gpi_pd=True -> priorities from the GPI envelope target)
  *   loss_out : f32 [1] = (1/n_nets) * sum_n mean( where(|d|<mp, 0.5 d^2, mp |d|) )   (common/networks.py:90-100)
  *   grad_q   : f32 [n_nets, N, A, D] or NULL;   prio_out : f32 [p_rows] (first p_rows rows), raw |w . err| before clip/pow
+ *   |d| == min_priority exactly takes the linear branch (mp |d|; the gradient is +-mp either way); d == +-0 adds nothing and
+ *   has a zero gradient.  action row k is action[k % a_rows]; the priority weight of row k is w[TILE or BLOCK map of w_map].
  */
 MORL_API int morl_td_huber_priority_f32(const float* q_values, int n_nets, const int32_t* action, int a_rows,
                                const float* target_q, const float* target_q_gpi, const float* w, int w_rows,

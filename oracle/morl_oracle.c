@@ -108,21 +108,26 @@ void oracle_envelope_td(const float* q_on, const float* q_tg, const float* wset,
     }
 }
 
+/* The three per-row targets below take the first argmax with a strict `>` from -inf, as the kernels do
+ * (include/morl_b200.h): a NaN score never wins, and a row whose every score is -inf or NaN falls back to candidate 0.
+ * th.argmax would return the first NaN instead; the two differ only on rows with a NaN score. */
+
 /* Envelope.ddqn_target, envelope.py:442-463 (+ :298 when reward != NULL); GPIPD._reset_priorities non-GPI branch gpi_pd.py:648-656 */
 void oracle_greedy_td(const float* q_sel, const float* q_eval, const float* w, int w_rows, int w_map, const float* reward,
                       const float* done, int r_rows, int r_map, float gamma, int N, int A, int D, int mode, float* out,
                       int32_t* act) {
     for (int k = 0; k < N; ++k) {
         const float* wv = w + (size_t)map_row(k, w_rows, N, w_map) * D;
-        float mval = 0.f;
-        int marg = 0;
+        float mval = -INFINITY;
+        int marg = -1;
         for (int a = 0; a < A; ++a) {
             float s = dotw(wv, q_sel + ((size_t)k * A + a) * D, D, mode);
-            if (a == 0 || s > mval) {
+            if (s > mval) {
                 mval = s;
                 marg = a;
             }
         }
+        if (marg < 0) marg = 0; /* every score -inf or NaN */
         const float* qe = q_eval + ((size_t)k * A + marg) * D;
         if (reward) {
             int ri = map_row(k, r_rows, N, r_map);
@@ -142,8 +147,8 @@ void oracle_critic_min_td(const float* q_nets, int n_nets, const float* w, int w
     size_t stride = (size_t)N * A * D;
     for (int k = 0; k < N; ++k) {
         const float* wv = w + (size_t)map_row(k, w_rows, N, w_map) * D;
-        float best = 0.f;
-        int ba = 0, bn = 0;
+        float best = -INFINITY;
+        int ba = -1, bn = 0;
         for (int a = 0; a < A; ++a) {
             float smin = 0.f;
             int nmin = 0;
@@ -154,13 +159,15 @@ void oracle_critic_min_td(const float* q_nets, int n_nets, const float* w, int w
                     nmin = n;
                 }
             }
+            if (a == 0) bn = nmin;
             /* max_q = einsum(w, gathered) recomputes the same scalarisation of the selected net */
-            if (a == 0 || smin > best) {
+            if (smin > best) {
                 best = smin;
                 ba = a;
                 bn = nmin;
             }
         }
+        if (ba < 0) ba = 0; /* every score -inf or NaN: action 0 with its critic-min net */
         const float* qe = q_nets + bn * stride + ((size_t)k * A + ba) * D;
         if (reward) {
             int ri = map_row(k, r_rows, N, r_map);
@@ -180,10 +187,10 @@ void oracle_gpi_envelope(const float* q_nets, int n_nets, const float* w, int w_
     size_t stride = (size_t)B * P * A * D;
     for (int b = 0; b < B; ++b) {
         const float* wv = w + (size_t)map_row(b, w_rows, B, w_map) * D;
-        float bestp = 0.f;
-        int bp = 0, bpa = 0, bpn = 0;
+        float bestp = -INFINITY;
+        int bp = -1, bpa = 0, bpn = 0, n00 = 0;
         for (int p = 0; p < P; ++p) {
-            float besta = 0.f;
+            float besta = -INFINITY;
             int ba = 0, bn = 0;
             for (int a = 0; a < A; ++a) {
                 float smin = 0.f;
@@ -195,18 +202,24 @@ void oracle_gpi_envelope(const float* q_nets, int n_nets, const float* w, int w_
                         nmin = n;
                     }
                 }
-                if (a == 0 || smin > besta) {
+                if (p == 0 && a == 0) n00 = nmin;
+                if (smin > besta) {
                     besta = smin;
                     ba = a;
                     bn = nmin;
                 }
             }
-            if (p == 0 || besta > bestp) {
+            if (besta > bestp) {
                 bestp = besta;
                 bp = p;
                 bpa = ba;
                 bpn = bn;
             }
+        }
+        if (bp < 0) { /* every score -inf or NaN: candidate (0, 0) with its critic-min net */
+            bp = 0;
+            bpa = 0;
+            bpn = n00;
         }
         const float* qe = q_nets + bpn * stride + ((((size_t)b * P + bp) * A) + bpa) * D;
         if (out) {
