@@ -288,14 +288,18 @@ MORL_API int morl_per_priority_f32(const float* raw, int n, float alpha, double*
  *                     one launch; a job with auto_scale != 0 derives its scale from the largest magnitude of its own matrix
  *                     (scale * amax in [2^(target_exp-1), 2^target_exp)) and stores it in *scale.
  * morl_gemm_planes_f32 : C = act(A . B^T + bias),  A planes [P][M][K] (K-major), B planes [P][N_pad][K] (K-major weights);
- *                     K % 64 == 0 (f16x2) / K % 32 == 0 (bf16x3), N_pad % 32 == 0, N_pad <= 256.  The accumulator is multiplied by
+ *                     K % 64 == 0 (f16x2) / K % 32 == 0 (bf16x3), N_pad % 32 == 0, N_pad <= 512 (wider than 256: two column units
+ *                     [0, 256) and [256, N_pad) of a row tile, each bit-identical to a launch over that half).  The accumulator is multiplied by
  *                     1 / (a_scale * b_scale) before the bias.  Outputs: c_f32 [M, ldc] and/or c_planes [P][M][ldp] holding
  *                     c_scale * C (the operand format of the next layer).  relu != 0 applies max(x, 0); relu_mask_plane0 (plane 0 of
  *                     a forward activation, [M][ld_mask] 16-bit) zeroes the outputs where that activation was <= 0 (ReLU backward).
  *                     ReLU bit masks (the form the update uses; relu_mask_plane0 stays for callers that only hold planes):
- *                     relu_bits_out [M][8] uint32 receives bit j of word (c & 1) * 4 + (c >> 1) = (C[m, 32 c + j] > 0) -- 32 bytes per
- *                     row instead of the 512-byte activation row, words ordered so that the four chunks one epilogue thread owns
- *                     are one 16-byte load; relu_bits_in (same layout, written by the forward call of the layer or by
+ *                     relu_bits_out [M][8] uint32 (N_pad <= 256) receives bit j of word (c & 1) * 4 + (c >> 1) = (C[m, 32 c + j] > 0) -- 32
+ *                     bytes per row instead of the 512-byte activation row, words ordered so that the four chunks one epilogue thread
+ *                     owns are one 16-byte load.  N_pad > 256: [M][16] words (the row pitch follows N_pad, not N: every 32-column
+ *                     chunk below N_pad has a word, padding chunks included), bit j of word 8 * (c >> 3) + (c & 1) * 4 + ((c >> 1) & 3):
+ *                     each 256-column half of the row keeps the 8-word order above, the second half's words after the first's.
+ *                     relu_bits_in (same layout, written by the forward call of the layer or by
  *                     morl_pairs_relu_split_planes) zeroes the outputs whose bit is clear, i.e. relu'(x) = [x > 0] exactly as
  *                     torch's ReLU backward (reference networks.py:10-48 under autograd).  Both nullable, 16-byte aligned.
  *                     reverse_tiles != 0 walks the 128-row tiles from the last to the first: alternate it between the layers of
@@ -385,14 +389,16 @@ MORL_API int morl_qhead_envelope_td_f32(int fmt, const void* a_on_planes, const 
                                         int B, int W, int A, int D, int dot_mode, int row_order, int reverse_tiles, float* target_out,
                                         int32_t* pref_out, int32_t* act_out, float* q_on_out, float* q_tg_out, void* stream);
 /* h[b*W + j, :] = relu(u[b, :] + v[j, :]) written directly as planes [P][B*W][H] of scale * h (separable first layer of the
- * weight-conditioned Q-network: W1 [s || w] + b1 = W1_s s + (W1_w w + b1); reference envelope.py:75 builds the concat). */
+ * weight-conditioned Q-network: W1 [s || w] + b1 = W1_s s + (W1_w w + b1); reference envelope.py:75 builds the concat).
+ * relu_bits_out (nullable): the ReLU bit mask of h in the layout of morl_gemm_planes_f32 ([B*W][8] words for H <= 256, [B*W][16] for
+ * H <= 512; H % 32 == 0). */
 MORL_API int morl_pairs_relu_split_planes(int fmt, const float* u, const float* v, int B, int W, int H, void* dst_planes,
                                           long long plane_stride, const float* scale, void* relu_bits_out, void* stream);
 
 
 /* Weight-gradient GEMM (reduction over the batch rows), split-K, deterministic:
  *   out[n, k] = sum_m G[m, n] * H[m, k]      G planes [P][M][ldg] (n < g_cols, scaled by *g_scale), H planes [P][M][ldh] (k < h_cols,
- *   scaled by *h_scale);  ldg, ldh multiples of 64, ldh <= 256;  transpose_out != 0 stores out[k, n] instead.  Replaces the
+ *   scaled by *h_scale);  ldg, ldh multiples of 64, ldh <= 512;  transpose_out != 0 stores out[k, n] instead.  Replaces the
  *   dW = dY^T X products that torch autograd issues for the nn.Linear layers of the reference networks (loss.backward(), envelope.py:316).
  *   colsum_out (nullable, [g_cols]): out_b[n] = sum_m G[m, n], the bias gradient db = colsum(dY), evaluated in the same pass as
  *   G^T . ones on the tensor cores (replaces a separate sweep of the G planes).

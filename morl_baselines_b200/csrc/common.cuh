@@ -98,6 +98,16 @@ __device__ __forceinline__ int map_row(int k, int rows, int n, int map) {
     return map == MORL_MAP_TILE ? (k % rows) : (k / (n / rows));
 }
 
+// ---- ReLU bit masks (include/morl_b200.h "ReLU bit masks"): the one place that knows the layout ---------------------------------
+// A row of an activation `width` columns wide is 8 uint32 words (width <= 256) or 16 (width <= 512).  Column c lies in chunk k = c / 32;
+// within each 256-column half the word order is (k & 1) * 4 + ((k >> 1) & 3), so the four chunks one epilogue thread owns are one
+// 16-byte load; the second half's words follow the first's.
+__host__ __device__ __forceinline__ int relu_bits_words(int width) { return width > 256 ? 16 : 8; }
+__host__ __device__ __forceinline__ int relu_bits_word(int col) {
+    const int k = col >> 5;
+    return 8 * (k >> 3) + (k & 1) * 4 + ((k >> 1) & 3);
+}
+
 // (value desc, index asc) total order used when partial argmaxes are merged: keeps first occurrence.
 __device__ __forceinline__ void argmax_merge(float& v, int& i, float v2, int i2) {
     if (v2 > v || (v2 == v && i2 < i)) {

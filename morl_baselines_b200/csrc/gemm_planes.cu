@@ -26,7 +26,8 @@
 //   warps 8-11: producer warpgroup, one lane of warp 8 issues TMA -- cp.async.bulk.tensor.3d of a [P planes x 128 rows x BK] A box and
 //              P x N/32 [32 rows x BK] B boxes per stage (f16x2: BK = 64, 128-byte swizzle, 2 x 96 KB stages at N = 256; bf16x3: BK = 32,
 //              64-byte swizzle, 2 x 72 KB), mbarrier ring; it keeps loading the next tile while the consumers are in their epilogue.
-// Operands: A [P][M][K] (K-major), B [P][N_pad][K] (K-major), K % BK == 0, N_pad % 32 == 0, N_pad <= 256.
+// Operands: A [P][M][K] (K-major), B [P][N_pad][K] (K-major), K % BK == 0, N_pad % 32 == 0, N_pad <= 512.  An output wider than 256
+// columns runs as two column units [0, 256) and [256, N_pad) of the same tile, each with the shared-memory plan of N_pad = 256.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -61,7 +62,7 @@ __device__ __forceinline__ void note_overflow(float amax) {
 
 
 struct GemmArgs {
-    int M, N, N_pad, K;          // N_pad = B rows covered (multiple of 32, <= 256)
+    int M, N, N_pad, K;          // N_pad = B rows covered (multiple of 32, <= 512)
     const float* bias;           // [N] or nullptr
     float* c_f32;                // [M, ldc] or nullptr
     int ldc;
@@ -70,8 +71,9 @@ struct GemmArgs {
     long long plane_stride;      // elements between planes
     const uint16_t* mask;        // plane 0 of the forward activation [M][ld_mask] for the ReLU-backward mask, or nullptr
     int ld_mask;
-    const uint32_t* bits_in;     // ReLU-backward mask as BITS [M][8] words (see morl_b200.h "ReLU bit masks"), or nullptr
+    const uint32_t* bits_in;     // ReLU-backward mask as BITS [M][relu_bits_words(N_pad)] words (see morl_b200.h "ReLU bit masks"), or nullptr
     uint32_t* bits_out;          // forward: bit = (output > 0) per column, same layout, or nullptr
+    int bits_ld;                 // words per row of bits_in / bits_out: relu_bits_words(N_pad) (the epilogue visits every chunk below N_pad)
     int n_stages;                // depth of the TMA ring: as many (A box + B boxes) stages as fit (2 at N_pad = 256, more for narrow outputs)
     uint32_t b_stage;            // bytes of one B stage slot (the B rows of a stage rounded up to 1 KB)
     int relu;
@@ -163,6 +165,7 @@ struct EpiArgs {
     int relu;
     const uint32_t* bits_in;
     uint32_t* bits_out;
+    int bits_ld;                 // words per bit-mask row (relu_bits_words)
     const uint16_t* mask;
     int ld_mask;
     float* c_f32;
@@ -180,8 +183,8 @@ __device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, i
     using F = PlaneFmt<FMT>;
     constexpr int P = F::P;
     const int l4 = lane & 3, lr = lane >> 2;
-    // ReLU bit masks: word (c & 1) * 4 + (c >> 1) of the row holds columns [32 c, 32 c + 32)
-    const int wi = ((col0 >> 5) & 1) * 4 + (col0 >> 6);
+    // ReLU bit masks: the word of the row that holds columns [col0, col0 + 32)
+    const int wi = relu_bits_word(col0);
     float x[2][8];
 #pragma unroll
     for (int h = 0; h < 2; ++h)
@@ -197,7 +200,7 @@ __device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, i
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int row = rbase + lr + 8 * h;
-            const uint32_t keep = row < e.M ? __ldg(e.bits_in + (size_t)row * 8 + wi) : 0u;
+            const uint32_t keep = row < e.M ? __ldg(e.bits_in + (size_t)row * e.bits_ld + wi) : 0u;
 #pragma unroll
             for (int j = 0; j < 8; ++j)
                 if (!((keep >> (8 * (j >> 1) + 2 * l4 + (j & 1))) & 1u)) x[h][j] = 0.f;
@@ -213,7 +216,7 @@ __device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, i
                 if (x[h][j] > 0.f) positive |= 1u << (8 * (j >> 1) + 2 * l4 + (j & 1));
             positive |= __shfl_xor_sync(0xffffffffu, positive, 1);  // the four threads of a row hold 8 of its 32 columns each
             positive |= __shfl_xor_sync(0xffffffffu, positive, 2);
-            if (l4 == 0 && row < e.M) e.bits_out[(size_t)row * 8 + wi] = positive;
+            if (l4 == 0 && row < e.M) e.bits_out[(size_t)row * e.bits_ld + wi] = positive;
         }
     }
     if (e.mask) {
@@ -283,8 +286,9 @@ __device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, i
     }
 }
 
-// One CTA per 128-row tile.  SPLIT = 1: see mma_unit; a tile wider than 128 columns is then computed as two column units (the A boxes of the
-// tile are staged once per unit).
+// One CTA per 128-row tile.  SPLIT = 1: see mma_unit; a tile wider than 128 columns is then computed as column units of 128 (the A boxes of
+// the tile are staged once per unit).  SPLIT = 0 and N_pad > 256: two column units [0, 256) and [256, N_pad), each with the stage plan of
+// N_pad = 256 and this unit's 256 biases in shared memory.
 template <int FMT, int SPLIT>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC,
@@ -314,14 +318,16 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     const int lane = threadIdx.x & 31;
     const int n_tiles = (g.M + kGemmBM - 1) / kGemmBM;
     const int n_kblk = g.K / BK;
-    // Work units: a tile, or (split accumulators, more than 128 columns) its two column units [0, 128) and [128, BN).  Both roles enumerate
-    // the same sequence.
-    const int col_units = (SPLIT && BN > 128) ? 2 : 1;
+    // Work units: a tile, or its column units of at most kUnitN columns ([0, 128), [128, 256), ... with split accumulators; [0, 256) and
+    // [256, BN) for outputs wider than 256 columns).  Both roles enumerate the same sequence.
+    constexpr int kUnitN = SPLIT ? 128 : 256;
+    const int col_units = (BN + kUnitN - 1) / kUnitN;
+    const bool wide = BN > 256;  // the biases of one unit at a time in shared memory (bias_s holds 256)
     const int n_work = n_tiles * col_units;
     auto unit_of = [&](int u, int& tile, int& n_begin, int& n_cnt) {
         tile = u / col_units;
-        n_begin = (u - tile * col_units) * 128;
-        n_cnt = col_units == 1 ? BN : (BN - n_begin < 128 ? BN - n_begin : 128);
+        n_begin = (u - tile * col_units) * kUnitN;
+        n_cnt = BN - n_begin < kUnitN ? BN - n_begin : kUnitN;
         if (g.reverse) tile = n_tiles - 1 - tile;
     };
 
@@ -396,8 +402,8 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         e.M = g.M; e.N = g.N;
         e.k_acc = fold / (ld_scale(g.a_scale) * ld_scale(g.b_scale));
         e.c_mul = folded ? 1.0f : c_mul;
-        e.bias_s = bias_s; e.relu = g.relu; e.bits_in = g.bits_in; e.bits_out = g.bits_out; e.mask = g.mask; e.ld_mask = g.ld_mask;
-        e.c_f32 = g.c_f32; e.ldc = g.ldc; e.planes = g.c_planes != nullptr; e.ldp = g.ldp;
+        e.bias_s = bias_s; e.relu = g.relu; e.bits_in = g.bits_in; e.bits_out = g.bits_out; e.bits_ld = g.bits_ld; e.mask = g.mask;
+        e.ld_mask = g.ld_mask; e.c_f32 = g.c_f32; e.ldc = g.ldc; e.planes = g.c_planes != nullptr; e.ldp = g.ldp;
         float amax = 0.f;
         float acc[128];
         uint32_t stage = 0, phase = 0;
@@ -423,6 +429,15 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
             }
 #undef MORL_UNIT
             const long long c1 = g.stats ? clock64() : 0;
+            if (wide) {
+                // this unit's biases (times the folded output scale), indexed by output column: every consumer warp has left the previous
+                // unit's epilogue (both warpgroups have finished the MMAs of this unit)
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+                const int col = n_begin + (int)threadIdx.x;
+                bias_s[threadIdx.x] = (g.bias && col < g.N) ? g.bias[col] * fold : 0.f;
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+                e.bias_s = bias_s - n_begin;
+            }
             const int rbase = tile * kGemmBM + wg * 64 + (warp & 3) * 16;
 #pragma unroll
             for (int c = 0; c < (SPLIT ? 4 : 8); ++c) {
@@ -595,7 +610,8 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
                     // x * s_act = acc * (s_act / (s_act * sB)) + s_act * bias  (powers of two: exact), as gemm_planes_kernel's folded epilogue
                     e.k_acc = s_act / (s_act * ld_scale(g.b_scale[job]));
                     e.c_mul = 1.0f;
-                    e.bias_s = bias_s; e.relu = g.relu; e.bits_in = g.bits_in[job]; e.bits_out = g.bits_out[job]; e.mask = nullptr; e.ld_mask = 0;
+                    e.bias_s = bias_s; e.relu = g.relu; e.bits_in = g.bits_in[job]; e.bits_out = g.bits_out[job]; e.bits_ld = relu_bits_words(BN);
+                    e.mask = nullptr; e.ld_mask = 0;
                     e.c_f32 = nullptr; e.ldc = 0; e.planes = 1; e.ldp = BN;
                     mma_unit<FMT, BN, 0>(acc, smA, smB, a_stage_bytes, b_stage_bytes, l == 0 ? n_kblk_first : n_kblk_full, full, empty, stage, phase, kStages,
                                          wg, lane, nullptr);
@@ -622,7 +638,8 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
 // MN-major split-K variant: weight gradients  dW[n, k] = sum_m G[m, n] * H[m, k]  (reduction over the 65,536 batch rows).
 // Both operands are the row-major plane tensors the forward/backward GEMMs already produced, read "MN-major" (the MMA's M / N
 // index is the contiguous one), 128-byte swizzle:  A = G^T (M_mma = n, 128 per CTA: 64 per warpgroup), B = H^T (N_mma = k <= 256), K_mma = m.
-// One CTA per (128-row block of n, split s of the m range); fp32 partial tiles are summed by reduce_partials_kernel
+// One CTA per (128-row block of n, unit of <= 256 columns of k, split s of the m range); H wider than 256 columns is two k units [0, 256) and
+// [256, NB), and only the CTAs of k unit 0 evaluate the fused column sums.  fp32 partial tiles are summed by reduce_partials_kernel
 // (deterministic, no atomics), which also removes the operand scales.
 // =================================================================================================================
 constexpr int kMnKT = 32;  // batch rows (K_mma direction) per pipeline stage
@@ -641,7 +658,7 @@ __device__ __forceinline__ uint64_t make_desc_mn_sw128(uint32_t smem_addr, uint3
 struct GemmMnArgs {
     int M;            // reduction length (batch rows)
     int n_tiles;      // ceil(A columns / 128)
-    int NB;           // N_mma = B columns covered (multiple of 64, <= 256)
+    int NB;           // B columns covered (multiple of 64, <= 512): N_mma of one k unit (<= 256), or of two ([0, 256) and [256, NB))
     int rows_per_split;
     float* partial;   // [S][n_tiles*128][NB]
     float* colsum_partial;  // [S][n_tiles*128] or nullptr: per-split column sums of G (bias gradient), fused as G^T . ones
@@ -652,7 +669,7 @@ struct GemmMnArgs {
 // branch between the wgmma of one commit group, or one 128-register accumulator array shared by the instantiations of all widths, makes
 // ptxas serialise the wgmma (its remarks C7519 / C7511).
 template <int FMT, int NB, bool COLSUM>
-__device__ __forceinline__ void mma_mn_unit(const GemmMnArgs& g, int split, int row, uint8_t* smA, uint8_t* smB, uint32_t a_stage, uint32_t b_stage,
+__device__ __forceinline__ void mma_mn_unit(const GemmMnArgs& g, int split, int row, int col0, uint8_t* smA, uint8_t* smB, uint32_t a_stage, uint32_t b_stage,
                                             uint32_t chunk_bytes, uint64_t ones_desc, int n_kblk, uint64_t* full, uint64_t* empty, int wg, int lane) {
     using F = PlaneFmt<FMT>;
     constexpr int P = F::P;
@@ -698,7 +715,7 @@ __device__ __forceinline__ void mma_mn_unit(const GemmMnArgs& g, int split, int 
     const int l4 = lane & 3;  // this thread holds output rows (n) row and row + 8
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        float* prow = g.partial + ((size_t)split * g.n_tiles * 128 + row + 8 * h) * NB + 2 * l4;
+        float* prow = g.partial + ((size_t)split * g.n_tiles * 128 + row + 8 * h) * g.NB + col0 + 2 * l4;
 #pragma unroll
         for (int j = 0; j < NB / 8; ++j) *reinterpret_cast<float2*>(prow + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
         if (COLSUM && l4 == 0) g.colsum_partial[(size_t)split * g.n_tiles * 128 + row + 8 * h] = cs[2 * h];
@@ -717,8 +734,11 @@ gemm_planes_mn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     uint8_t* gsmem = gsmem_raw + ((1024u - (g_smem_u32(gsmem_raw) & 1023u)) & 1023u);
     constexpr uint32_t chunk_bytes = (uint32_t)P * kMnKT * 128u;   // one 64-element MN chunk, P planes
     constexpr uint32_t a_stage = 2u * chunk_bytes;
-    constexpr uint32_t b_stage = 4u * chunk_bytes;                 // (allocated for NB = 256)
-    const int nb_chunks = g.NB / 64;
+    constexpr uint32_t b_stage = 4u * chunk_bytes;                 // (allocated for a k unit of 256 columns)
+    const int k_units = g.NB > 256 ? 2 : 1;
+    const int col0 = (int)(blockIdx.x / g.n_tiles % k_units) * 256;  // first column of H (k) of this CTA's unit
+    const int nb = g.NB - col0 < 256 ? g.NB - col0 : 256;
+    const int nb_chunks = nb / 64;
     uint8_t* smA = gsmem;
     uint8_t* smB = gsmem + kStages * a_stage;
     uint64_t* full = reinterpret_cast<uint64_t*>(smB + kStages * b_stage);
@@ -732,7 +752,7 @@ gemm_planes_mn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nt = blockIdx.x % g.n_tiles;
-    const int split = blockIdx.x / g.n_tiles;
+    const int split = blockIdx.x / (g.n_tiles * k_units);
     const int m_begin = split * g.rows_per_split;
     const int m_end = min(g.M, m_begin + g.rows_per_split);
     const int n_kblk = (m_end - m_begin + kMnKT - 1) / kMnKT;
@@ -756,7 +776,7 @@ gemm_planes_mn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                 g_mbar_expect_tx(&full[stage], (2u + (uint32_t)nb_chunks) * chunk_bytes);
                 const int m0 = m_begin + kb * kMnKT;
                 for (int c = 0; c < 2; ++c) tma_load_3d(smA + stage * a_stage + c * chunk_bytes, &tmA, &full[stage], nt * 128 + c * 64, m0, 0);
-                for (int c = 0; c < nb_chunks; ++c) tma_load_3d(smB + stage * b_stage + c * chunk_bytes, &tmB, &full[stage], c * 64, m0, 0);
+                for (int c = 0; c < nb_chunks; ++c) tma_load_3d(smB + stage * b_stage + c * chunk_bytes, &tmB, &full[stage], col0 + c * 64, m0, 0);
                 if (++stage == kStages) {
                     stage = 0;
                     phase ^= 1u;
@@ -767,14 +787,14 @@ gemm_planes_mn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         warpgroup_reg_inc<kGemmConsumerRegs>();
         const int wg = warp >> 2;
         const uint64_t ones_desc = make_desc_mn_sw128(g_smem_u32(ones), chunk_bytes);
-        const bool colsum = g.colsum_partial != nullptr;
+        const bool colsum = g.colsum_partial != nullptr && col0 == 0;
         const int row = nt * 128 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #define MORL_UNIT(N_)                                                                                                                               \
     case N_:                                                                                                                                        \
-        if (colsum) mma_mn_unit<FMT, N_, true>(g, split, row, smA, smB, a_stage, b_stage, chunk_bytes, ones_desc, n_kblk, full, empty, wg, lane);  \
-        else mma_mn_unit<FMT, N_, false>(g, split, row, smA, smB, a_stage, b_stage, chunk_bytes, ones_desc, n_kblk, full, empty, wg, lane);        \
+        if (colsum) mma_mn_unit<FMT, N_, true>(g, split, row, col0, smA, smB, a_stage, b_stage, chunk_bytes, ones_desc, n_kblk, full, empty, wg, lane); \
+        else mma_mn_unit<FMT, N_, false>(g, split, row, col0, smA, smB, a_stage, b_stage, chunk_bytes, ones_desc, n_kblk, full, empty, wg, lane);       \
         break;
-        switch (g.NB) {
+        switch (nb) {
             MORL_UNIT(64) MORL_UNIT(128) MORL_UNIT(192) MORL_UNIT(256)
             default: __trap();
         }
@@ -1275,8 +1295,7 @@ __global__ void __launch_bounds__(256) pairs_relu_split_kernel(const float* __re
             wbits |= __shfl_xor_sync(0xffffffffu, wbits, 1);
             wbits |= __shfl_xor_sync(0xffffffffu, wbits, 2);
             if (ok && (lane & 3) == 0) {
-                const int chunk = h8 >> 2;
-                bits_out[(size_t)row * 8 + (chunk & 1) * 4 + (chunk >> 1)] = wbits;
+                bits_out[(size_t)row * relu_bits_words(H) + relu_bits_word(32 * (h8 >> 2))] = wbits;
             }
         }
     }
@@ -1335,8 +1354,7 @@ __global__ void __launch_bounds__(256) pairs_relu_split_h256_kernel(const float*
                 uint32_t wbits = pos << (8 * (lane & 3));
                 wbits |= __shfl_xor_sync(0xffffffffu, wbits, 1);
                 wbits |= __shfl_xor_sync(0xffffffffu, wbits, 2);
-                const int chunk = lane >> 2;
-                if ((lane & 3) == 0) bits_out[(size_t)row * 8 + (chunk & 1) * 4 + (chunk >> 1)] = wbits;
+                if ((lane & 3) == 0) bits_out[(size_t)row * relu_bits_words(H) + relu_bits_word(8 * lane)] = wbits;
             }
         }
     }
@@ -1398,11 +1416,11 @@ extern "C" int morl_amax_scale_f32(const float* src, long long n, int target_exp
 extern "C" size_t morl_gemm_mn_workspace_bytes(int M, int a_cols, int b_cols) {
     if (M <= 0 || a_cols <= 0 || b_cols <= 0) return 0;
     const int n_tiles = (a_cols + 127) / 128;
-    int S = morl::mn_sm_count() / n_tiles;
+    const int NB = (b_cols + 63) / 64 * 64;
+    int S = morl::mn_sm_count() / (n_tiles * (NB > 256 ? 2 : 1));
     if (S < 1) S = 1;
     int rps = ((M + S - 1) / S + 31) / 32 * 32;
     S = (M + rps - 1) / rps;
-    const int NB = (b_cols + 63) / 64 * 64;
     return (size_t)S * n_tiles * 128 * NB * sizeof(float) + (size_t)256 * 256 * sizeof(float);  // tail: [S][n_tiles*128] column-sum partials
 }
 
@@ -1413,15 +1431,16 @@ extern "C" int morl_gemm_planes_mn_f32(int fmt, const void* g_planes, long long 
     MORL_REQUIRE(fmt_ok(fmt), MORL_ERR_UNSUPPORTED, "morl_gemm_planes_mn_f32: unknown plane format %d", fmt);
     MORL_REQUIRE(g_planes && h_planes && out && workspace, MORL_ERR_NULL, "morl_gemm_planes_mn_f32: NULL pointer argument");
     MORL_REQUIRE(M > 0 && g_cols > 0 && h_cols > 0, MORL_ERR_SHAPE, "morl_gemm_planes_mn_f32: bad shape M=%d g_cols=%d h_cols=%d", M, g_cols, h_cols);
-    MORL_REQUIRE(ldg % 64 == 0 && ldh % 64 == 0 && ldh <= 256 && g_cols <= ldg && h_cols <= ldh, MORL_ERR_UNSUPPORTED,
-                 "morl_gemm_planes_mn_f32: plane row lengths must be multiples of 64 (ldg=%d ldh=%d), ldh <= 256", ldg, ldh);
+    MORL_REQUIRE(ldg % 64 == 0 && ldh % 64 == 0 && ldh <= 512 && g_cols <= ldg && h_cols <= ldh, MORL_ERR_UNSUPPORTED,
+                 "morl_gemm_planes_mn_f32: plane row lengths must be multiples of 64 (ldg=%d ldh=%d), ldh <= 512", ldg, ldh);
     const int n_tiles = (g_cols + 127) / 128;
+    const int NB = (h_cols + 63) / 64 * 64;
+    const int k_units = NB > 256 ? 2 : 1;  // (morl_gemm_mn_workspace_bytes derives the same S)
     MORL_REQUIRE(n_tiles * 128 <= ldg || ldg % 128 == 0 || n_tiles * 128 - ldg <= 64, MORL_ERR_UNSUPPORTED, "morl_gemm_planes_mn_f32: ldg=%d", ldg);
-    int S = morl::mn_sm_count() / n_tiles;
+    int S = morl::mn_sm_count() / (n_tiles * k_units);
     if (S < 1) S = 1;
     const int rps = ((M + S - 1) / S + 31) / 32 * 32;
     S = (M + rps - 1) / rps;
-    const int NB = (h_cols + 63) / 64 * 64;
     CUtensorMap tmA, tmB;
     int rc = make_plane_map_mn(&tmA, fmt, g_planes, M, ldg, g_plane_stride);
     MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "morl_gemm_planes_mn_f32: cuTensorMapEncodeTiled(G) failed (%d)", rc);
@@ -1439,7 +1458,7 @@ extern "C" int morl_gemm_planes_mn_f32(int fmt, const void* g_planes, long long 
             cudaFuncSetAttribute(gemm_planes_mn_kernel<kFmt>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             attr_set = true;
         }
-        launch_k(gemm_planes_mn_kernel<kFmt>, dim3(n_tiles * S), dim3(kGemmThreads), smem, st, tmA, tmB, g);
+        launch_k(gemm_planes_mn_kernel<kFmt>, dim3(n_tiles * k_units * S), dim3(kGemmThreads), smem, st, tmA, tmB, g);
     });
     rc = check_launch("morl_gemm_planes_mn_f32");
     if (rc) return rc;
@@ -1594,8 +1613,8 @@ extern "C" int morl_pairs_relu_split_planes(int fmt, const float* u, const float
     long long blocks = (total + 255) / 256;
     if (blocks > 132 * 16) blocks = 132 * 16;
     if (relu_bits_out)
-        MORL_REQUIRE(H % 32 == 0 && H <= 256 && aligned16(relu_bits_out), MORL_ERR_SHAPE,
-                     "morl_pairs_relu_split_planes: ReLU bit masks need H %% 32 == 0, H <= 256 (H=%d)", H);
+        MORL_REQUIRE(H % 32 == 0 && H <= 512 && aligned16(relu_bits_out), MORL_ERR_SHAPE,
+                     "morl_pairs_relu_split_planes: ReLU bit masks need H %% 32 == 0, H <= 512 (H=%d)", H);
     if (H == 256) {
         const int jsplit = W >= 16 ? 4 : 1;
         const long long tasks = (long long)B * jsplit;
@@ -1631,7 +1650,8 @@ static int launch_gemm_planes(const CUtensorMap& tmA, const CUtensorMap& tmB, co
         cudaFuncSetAttribute(gemm_planes_kernel<FMT, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         attr_set = true;
     }
-    const int n_work = (g.M + kGemmBM - 1) / kGemmBM * ((SPLIT && g.N_pad > 128) ? 2 : 1);
+    constexpr int kUnitN = SPLIT ? 128 : 256;  // column units per tile: as gemm_planes_kernel
+    const int n_work = (g.M + kGemmBM - 1) / kGemmBM * ((g.N_pad + kUnitN - 1) / kUnitN);
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(n_work < sms ? n_work : sms);
@@ -1658,8 +1678,8 @@ extern "C" int morl_gemm_planes_f32(int fmt, const void* a_planes, long long a_p
     MORL_REQUIRE(a_planes && b_planes && (c_f32 || c_planes), MORL_ERR_NULL, "morl_gemm_planes_f32: NULL pointer argument");
     MORL_REQUIRE(M > 0 && N > 0 && K > 0 && N_pad >= N, MORL_ERR_SHAPE, "morl_gemm_planes_f32: bad shape M=%d N=%d N_pad=%d K=%d", M, N, N_pad, K);
     const int BK = fmt == MORL_FMT_F16X2 ? PlaneFmt<MORL_FMT_F16X2>::BK : PlaneFmt<MORL_FMT_BF16X3>::BK;
-    MORL_REQUIRE(K % BK == 0 && N_pad % 32 == 0 && N_pad <= 256, MORL_ERR_UNSUPPORTED,
-                 "morl_gemm_planes_f32: need K %% %d == 0, N_pad %% 32 == 0, N_pad <= 256 (K=%d N_pad=%d)", BK, K, N_pad);
+    MORL_REQUIRE(K % BK == 0 && N_pad % 32 == 0 && N_pad <= 512, MORL_ERR_UNSUPPORTED,
+                 "morl_gemm_planes_f32: need K %% %d == 0, N_pad %% 32 == 0, N_pad <= 512 (K=%d N_pad=%d)", BK, K, N_pad);
     MORL_REQUIRE(aligned16(a_planes) && aligned16(b_planes), MORL_ERR_ALIGN, "morl_gemm_planes_f32: operand planes must be 16-byte aligned");
     MORL_REQUIRE(aligned16(relu_bits_in) && aligned16(relu_bits_out), MORL_ERR_ALIGN, "morl_gemm_planes_f32: ReLU bit masks must be 16-byte aligned");
     if (c_planes)
@@ -1684,12 +1704,14 @@ extern "C" int morl_gemm_planes_f32(int fmt, const void* a_planes, long long a_p
     g.c_planes = c_planes; g.ldp = ldp; g.plane_stride = c_plane_stride;
     g.mask = static_cast<const uint16_t*>(relu_mask_plane0); g.ld_mask = ld_mask; g.relu = relu;
     g.bits_in = static_cast<const uint32_t*>(relu_bits_in); g.bits_out = static_cast<uint32_t*>(relu_bits_out);
+    g.bits_ld = relu_bits_words(N_pad);  // every 32-column chunk below N_pad has its word, padding chunks included
     {
         // TMA ring: A box + B rows per stage; a narrow B (the output layer: N_pad = 32) leaves room for a deeper ring, which is what
         // keeps enough bytes in flight per SM when a tile is four A boxes and almost no tensor work
         const uint32_t rowb = (uint32_t)BK * 2u, P = (uint32_t)fmt_planes(fmt);
         const uint32_t a_box = P * (uint32_t)kGemmBM * rowb;
-        const uint32_t b_box = (P * (uint32_t)N_pad * rowb + 1023u) & ~1023u;
+        const uint32_t n_unit = N_pad > 256 ? 256u : (uint32_t)N_pad;  // B rows of one column unit (outputs wider than 256: two units)
+        const uint32_t b_box = (P * n_unit * rowb + 1023u) & ~1023u;
         const uint32_t room = fmt == MORL_FMT_F16X2 ? KPlan<MORL_FMT_F16X2>::kOffC : KPlan<MORL_FMT_BF16X3>::kOffC;
         int n_st = (int)(room / (a_box + b_box));
         if (n_st > 8) n_st = 8;

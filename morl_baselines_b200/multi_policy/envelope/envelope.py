@@ -231,7 +231,7 @@ class Envelope(MOPolicy, MOAgent):
                                  or not TCPairMlp.trainable_supported(self.q_net.net, num_sample_w, self._tc_fmt)):
             raise ops._lib.MorlB200Error(
                 "morl_baselines_b200.Envelope: the tensor-core update path needs a flat observation, equal hidden widths that are multiples "
-                f"of 64 and <= 256, and num_sample_w <= 64 (got obs {self.observation_shape}, net_arch {net_arch}, num_sample_w {num_sample_w}); "
+                f"of 64 and <= 512, and num_sample_w <= 256 (got obs {self.observation_shape}, net_arch {net_arch}, num_sample_w {num_sample_w}); "
                 "pass use_tensor_cores=False to run the (slow) library-GEMM validation path explicitly")
         self.use_tensor_cores = bool(use_tensor_cores)
         self._tc_on = self._tc_tg = self._tc_train = None

@@ -411,7 +411,8 @@ def gemm_planes(a_planes: th.Tensor, b_planes: th.Tensor, n_out: int, bias: Opti
     smaller systematic error, ~20 % slower per launch); False (default): one double-buffered accumulator.
     ``relu_bits_out`` / ``relu_bits_in`` (:func:`empty_relu_bits`): the forward call records [C > 0] as one bit per column, the backward
     call zeroes the outputs whose bit is clear (ReLU backward from 32 bytes per row instead of the activation planes; ``relu_mask`` is the
-    plane-based form of the same mask).
+    plane-based form of the same mask).  Their width is the padded output width N_pad = b_planes.shape[1]
+    (``empty_relu_bits(M, device, N_pad)``): 8 words per row up to 256, 16 above.
     returns (c_f32 [M, n_out] or None, c_planes [P, M, ldp] holding c_scale * C, or None)."""
     fmt = fmt_of(a_planes)
     if fmt_of(b_planes) != fmt or not a_planes.is_cuda:
@@ -426,9 +427,10 @@ def gemm_planes(a_planes: th.Tensor, b_planes: th.Tensor, n_out: int, bias: Opti
     if out_planes and c_planes is None:
         c_planes = empty_planes(fmt, M, _pad(n_out, 32), dev)
     mask0 = None if relu_mask is None else relu_mask[0]
+    words = relu_bits_words(n_pad)  # one word per 32-column chunk of the padded output (the kernel visits them all)
     for bits in (relu_bits_in, relu_bits_out):
-        if bits is not None and (bits.dtype != th.int32 or tuple(bits.shape) != (M, 8) or not bits.is_contiguous() or bits.device != dev):
-            raise _lib.MorlB200Error(f"gemm_planes: ReLU bit masks must be contiguous int32 [{M}, 8] on {dev}")
+        if bits is not None and (bits.dtype != th.int32 or tuple(bits.shape) != (M, words) or not bits.is_contiguous() or bits.device != dev):
+            raise _lib.MorlB200Error(f"gemm_planes: ReLU bit masks must be contiguous int32 [{M}, {words}] on {dev}")
     rc = _lib.load().morl_gemm_planes_f32(fmt, _ptr(a_planes), a_planes.stride(0), _ptr(a_scale), _ptr(b_planes), b_planes.stride(0), _ptr(b_scale), M,
                                           n_out, n_pad, K, _ptr(bias), int(relu), _ptr(mask0), 0 if mask0 is None else mask0.stride(0), _ptr(c_f32),
                                           0 if c_f32 is None else c_f32.stride(0), _ptr(c_planes), 0 if c_planes is None else c_planes.shape[2],
@@ -524,7 +526,8 @@ class GemmChain:
         self.n_chains, self.n_layers = len(acts), len(weights[0])
         a0 = acts[0][1]  # (the first OUTPUT: the chain's input may be narrower, see k_first)
         self.fmt = fmt_of(a0)
-        _, self.M, self.K = a0.shape
+        _, self.M, self.K = a0.shape  # (square layers: the output width of every layer is also the reduction length)
+        self.N = a0.shape[2]  # output width of every layer: the width of its ReLU bit masks
         self.k_first = int(k_first) if k_first else self.K
         flat_a = [t for ch in acts for t in ch]
         flat_w = [t for ch in weights for t in ch]
@@ -543,8 +546,8 @@ class GemmChain:
             if fmt_of(t) != self.fmt or tuple(t.shape[1:]) != (256, kk) or not t.is_contiguous():
                 raise _lib.MorlB200Error(f"GemmChain: weight planes must be contiguous [P, 256, {kk}]")
         for t in flat_m + flat_i:
-            if t is not None and (t.dtype != th.int32 or tuple(t.shape) != (self.M, 8) or not t.is_contiguous()):
-                raise _lib.MorlB200Error(f"GemmChain: ReLU bit masks must be contiguous int32 [{self.M}, 8]")
+            if t is not None and (t.dtype != th.int32 or tuple(t.shape) != (self.M, relu_bits_words(self.N)) or not t.is_contiguous()):
+                raise _lib.MorlB200Error(f"GemmChain: ReLU bit masks must be contiguous int32 [{self.M}, {relu_bits_words(self.N)}]")
         self._keep = (flat_a, flat_w, flat_b, flat_s, flat_m, flat_i, act_scale)
         self.relu = bool(relu)
         arr = lambda ts: (C.c_void_p * len(ts))(*[None if t is None else t.data_ptr() for t in ts])  # noqa: E731
@@ -579,23 +582,34 @@ def qhead_gemm(a_planes: th.Tensor, w_planes: th.Tensor, n_out: int, bias: th.Te
     return out
 
 
-def empty_relu_bits(rows: int, device) -> th.Tensor:
-    """ReLU bit-mask tensor [rows, 8] int32 (layout: include/morl_b200.h, morl_gemm_planes_f32)."""
-    return th.empty((rows, 8), device=device, dtype=th.int32)
+def relu_bits_words(width: int) -> int:
+    """int32 words per row of the ReLU bit mask of an activation ``width`` columns wide: 8 up to 256 columns, 16 up to 512."""
+    return 16 if width > 256 else 8
+
+
+def relu_bits_word(chunk):
+    """Word of a bit-mask row holding columns [32 chunk, 32 chunk + 32) (int or integer tensor): within each 256-column half
+    (chunk & 1) * 4 + ((chunk >> 1) & 3), the second half's eight words after the first's (include/morl_b200.h)."""
+    return 8 * (chunk >> 3) + (chunk & 1) * 4 + ((chunk >> 1) & 3)
+
+
+def empty_relu_bits(rows: int, device, width: int = 256) -> th.Tensor:
+    """ReLU bit-mask tensor [rows, relu_bits_words(width)] int32 (layout: include/morl_b200.h, morl_gemm_planes_f32)."""
+    return th.empty((rows, relu_bits_words(width)), device=device, dtype=th.int32)
 
 
 def unpack_relu_bits(bits: th.Tensor, n_cols: int) -> th.Tensor:
     """[rows, n_cols] bool from a ReLU bit-mask tensor (tests / diagnostics)."""
     c = th.arange((n_cols + 31) // 32, device=bits.device)
-    words = bits[:, (c & 1) * 4 + (c >> 1)].to(th.int64) & 0xFFFFFFFF  # [rows, chunks]
+    words = bits[:, relu_bits_word(c)].to(th.int64) & 0xFFFFFFFF  # [rows, chunks]
     j = th.arange(32, device=bits.device)
     return (((words[:, :, None] >> j) & 1) != 0).reshape(bits.shape[0], -1)[:, :n_cols]
 
 
 def pairs_relu_split(u: th.Tensor, v: th.Tensor, out: Optional[th.Tensor] = None, fmt: int = FMT_F16X2, scale: Optional[th.Tensor] = None,
                      relu_bits_out: Optional[th.Tensor] = None) -> th.Tensor:
-    """relu(u[b] + v[j]) for every pair, written as planes [P, B*W, H] of scale * h (row b*W + j); ``relu_bits_out`` [B*W, 8] int32
-    additionally receives [h > 0] as bits (the ReLU-backward mask of :func:`gemm_planes`)."""
+    """relu(u[b] + v[j]) for every pair, written as planes [P, B*W, H] of scale * h (row b*W + j); ``relu_bits_out``
+    ([B*W, relu_bits_words(H)] int32) additionally receives [h > 0] as bits (the ReLU-backward mask of :func:`gemm_planes`)."""
     u, v = _dev(u, "u"), _dev(v, "v")
     B, H = u.shape
     W = v.shape[0]
@@ -603,6 +617,9 @@ def pairs_relu_split(u: th.Tensor, v: th.Tensor, out: Optional[th.Tensor] = None
         out = empty_planes(fmt, B * W, H, u.device)
     else:
         fmt = fmt_of(out)
+    if relu_bits_out is not None and (relu_bits_out.dtype != th.int32 or tuple(relu_bits_out.shape) != (B * W, relu_bits_words(H))
+                                      or not relu_bits_out.is_contiguous()):
+        raise _lib.MorlB200Error(f"pairs_relu_split: ReLU bit masks must be contiguous int32 [{B * W}, {relu_bits_words(H)}]")
     rc = _lib.load().morl_pairs_relu_split_planes(fmt, _ptr(u), _ptr(v), B, W, H, _ptr(out), out.stride(0), _ptr(scale), _ptr(relu_bits_out), _stream())
     _lib.check(rc, "morl_pairs_relu_split_planes")
     _count()
@@ -649,8 +666,12 @@ def pair_layer1_grad(dU: th.Tensor, dV: th.Tensor, feats: th.Tensor, wset: th.Te
     return dW1, db1
 
 
+def gemm_mn_workspace_bytes(M: int, g_cols: int, h_cols: int) -> int:
+    return int(_lib.load().morl_gemm_mn_workspace_bytes(int(M), int(g_cols), int(h_cols)))
+
+
 def gemm_mn_workspace(M: int, g_cols: int, h_cols: int, device) -> th.Tensor:
-    nbytes = _lib.load().morl_gemm_mn_workspace_bytes(int(M), int(g_cols), int(h_cols))
+    nbytes = gemm_mn_workspace_bytes(M, g_cols, h_cols)
     return th.empty((nbytes + 3) // 4, device=device, dtype=th.float32)
 
 

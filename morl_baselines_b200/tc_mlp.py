@@ -50,6 +50,8 @@ _CHAIN_BWD = os.environ.get("MORL_GEMM_CHAIN_BWD", "1") == "1"  # ... and the 25
 _NARROW_HEAD = os.environ.get("MORL_NARROW_HEAD", "1") == "1"  # output layer through morl_qhead_gemm_f32 (19.7 us against 26 us in the update; =0: general kernel)
 _DEFAULT_FMT = ops.FMT_BF16X3 if os.environ.get("MORL_TC_FMT", "f16x2") == "bf16x3" else ops.FMT_F16X2
 
+MAX_HIDDEN = 512      # widest hidden layer (outputs wider than 256 columns run as two column units of the K-major GEMM)
+MAX_TRAIN_W = 256     # most weight vectors per minibatch of the hand-written backward
 ACT_SCALE = 2.0        # f16x2 activations: |h| < 32,752 representable
 W_TARGET_EXP = 14      # f16x2 weights: amax * scale in [2^13, 2^14) (the matrix is known when it is split: it cannot overflow)
 G_TARGET_EXP = 2       # f16x2 gradients: amax(dL/dQ) * scale in [2, 4): 2^13 of growth head-room through the backward chain
@@ -72,15 +74,15 @@ class TCPairMlp:
             return False
         hidden = [l.out_features for l in lin[:-1]]
         kmul = 64 if fmt == ops.FMT_F16X2 else 32  # K extent of one pipeline stage
-        return all(h % kmul == 0 and h <= 256 for h in hidden) and lin[-1].out_features <= 256
+        return all(h % kmul == 0 and h <= MAX_HIDDEN for h in hidden) and lin[-1].out_features <= 256
 
     @staticmethod
     def trainable_supported(net: nn.Sequential, n_w: int, fmt: int = _DEFAULT_FMT) -> bool:
-        """The hand-written backward additionally needs equal hidden widths (multiples of 64) and at most 64 weight vectors."""
+        """The hand-written backward additionally needs equal hidden widths (multiples of 64) and at most MAX_TRAIN_W weight vectors."""
         if not TCPairMlp.supported(net, fmt):
             return False
         hidden = {m.out_features for m in list(net)[:-1] if isinstance(m, nn.Linear)}
-        return len(hidden) == 1 and next(iter(hidden)) % 64 == 0 and n_w <= 64
+        return len(hidden) == 1 and next(iter(hidden)) % 64 == 0 and n_w <= MAX_TRAIN_W
 
     def __init__(self, net: nn.Sequential, feat_dim: int, n_obs: int, n_w: int, share_weights_with: Optional["TCPairMlp"] = None,
                  trainable: bool = False, fmt: Optional[int] = None, split_acc: bool = False):
@@ -94,7 +96,7 @@ class TCPairMlp:
         self.fmt = fmt = (share_weights_with.fmt if share_weights_with is not None else _DEFAULT_FMT) if fmt is None else fmt
         if not TCPairMlp.supported(net, fmt):
             raise ops._lib.MorlB200Error("TCPairMlp: unsupported network (Linear/ReLU stack with hidden widths that are multiples of 64 (f16x2) or "
-                                         "32 (bf16x3) and <= 256)")
+                                         f"32 (bf16x3) and <= {MAX_HIDDEN}, output layer <= 256 wide)")
         dev = self.lin[0].weight.device
         M = n_obs * n_w
         scaled = fmt == ops.FMT_F16X2
@@ -111,15 +113,16 @@ class TCPairMlp:
         self._chain = self._gchain = self._gbufs = None
         self.trainable = trainable
         if trainable:
-            if n_w > 64:
-                raise ops._lib.MorlB200Error("TCPairMlp backward supports at most 64 weight vectors per minibatch")
+            if n_w > MAX_TRAIN_W:
+                raise ops._lib.MorlB200Error(f"TCPairMlp backward supports at most {MAX_TRAIN_W} weight vectors per minibatch")
             out = self.lin[-1].out_features
             self.ld_last = _pad(out, 64)
             hid = max(l.out_features for l in self.lin[:-1])
             self.g_last = ops.empty_planes(fmt, M, self.ld_last, dev)
             self.g = [ops.empty_planes(fmt, M, hid, dev) for _ in range(2)]
-            # relu'(H_k) as bits (32 B per row), written by the forward pass, read by the dX GEMMs instead of the 512-B activation rows
-            self.hbits = [ops.empty_relu_bits(M, dev) for _ in self.lin[:-1]]
+            # relu'(H_k) as bits (32 B per row up to 256 columns, 64 B up to 512), written by the forward pass, read by the dX GEMMs instead
+            # of the activation rows
+            self.hbits = [ops.empty_relu_bits(M, dev, l.out_features) for l in self.lin[:-1]]
             self.s_g = ops.scale_tensor(1.0, dev) if scaled else None
             self.ws_amax = th.zeros(2, device=dev, dtype=th.int32)
             # transposed weight planes W_l^T [P, in_l, K = padded out_l] for the dX products
@@ -127,8 +130,11 @@ class TCPairMlp:
             for k, l in enumerate(self.lin[1:], start=1):
                 kdim = self.ld_last if k == len(self.lin) - 1 else l.out_features
                 self.wtp.append(ops.empty_planes(fmt, _pad(l.in_features, 32), kdim, dev))
-            self.ws_mn = ops.gemm_mn_workspace(M, 256, 256, dev)
-            self.ws_red = th.empty(296 * max(n_w * hid, 256), device=dev, dtype=th.float32)
+            # the largest split-K workspace of the weight-gradient products dW_l = G_l^T H_{l-1} of layers 2..
+            self.ws_mn = th.empty(max(ops.gemm_mn_workspace_bytes(M, l.out_features, l.in_features) for l in self.lin[1:]) // 4 + 1,
+                                  device=dev, dtype=th.float32)
+            # pairs_grad_reduce: per-chunk dV partials, <= 296 chunks in the one-pass form (|W| <= 64), <= 74 in the two-pass form
+            self.ws_red = th.empty((296 if n_w <= 64 else 74) * max(n_w * hid, 256), device=dev, dtype=th.float32)
             first = self.lin[0]
             self.ws_l1 = ops.pair_layer1_grad_workspace(feat_dim, first.in_features - feat_dim, first.out_features, dev)
             self.dU = th.empty((n_obs, first.out_features), device=dev, dtype=th.float32)
