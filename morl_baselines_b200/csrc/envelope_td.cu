@@ -15,7 +15,8 @@
 #include <limits.h>
 #include <stdlib.h>
 
-#include "common.cuh"
+#include "envelope_wp.cuh"
+#include "gemm_tc.cuh"
 
 namespace morl {
 
@@ -127,96 +128,13 @@ __global__ void __launch_bounds__(512) envelope_td_kernel(const float* __restric
 
 
 // =================================================================================================================
-// v2 fast path: pairwise scalarisation (two weights per register pair), max tree, persistent CTAs with a
-// register-prefetched double buffer.  Bit-identical to the scalar arithmetic above:
-//   * mul.rn.f32x2 is two IEEE multiplies; the unfused add is issued as fma.rn.f32x2(acc, ONE, p) with ONE = 1.0f passed
-//     as a RUNTIME kernel argument -- ptxas may contract a multiply and a dependent add into an FMA even with -fmad=false
-//     (observed with CUDA 12.9), but it cannot fold a multiplier it does not know; fl(acc * 1 + p) == fl(acc + p);
-//   * the Q_on[b] block is transposed once into shared memory as SoA planes Qs[r][c] (c = j*A + a), so one LDS.128 yields
-//     the r-th objective of four consecutive candidates already sitting in aligned register pairs;
-//   * candidates are scanned in groups of 8: four packed dot products, max of 8, and only the GROUP index of
-//     the running maximum is tracked (strict '>' keeps the first group); the exact (first) position inside the winning
-//     group is recovered afterwards by re-evaluating its 8 scores with the scalar path and testing equality.
-// =================================================================================================================
-typedef unsigned long long u64;
-__device__ __forceinline__ u64 pk2(float lo, float hi) {
-    u64 r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void upk2(u64 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-// Hopper has no packed-fp32 arithmetic and no 3-input max: the pair forms below are two scalar IEEE operations on the halves of the
-// register pair (the same values a packed instruction would give), the 3-input max two FMNMX
-__device__ __forceinline__ u64 mul2(u64 a, u64 b) {
-    float a0, a1, b0, b1;
-    upk2(a, a0, a1);
-    upk2(b, b0, b1);
-    return pk2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
-}
-__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
-    float a0, a1, b0, b1, c0, c1;
-    upk2(a, a0, a1);
-    upk2(b, b0, b1);
-    upk2(c, c0, c1);
-    return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
-}
-__device__ __forceinline__ float max3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
-
-// packed w . q for two candidates; `one2` = (1.0f, 1.0f) built from the runtime kernel argument
-template <int D, int MODE>
-__device__ __forceinline__ u64 dotw2(const u64 (&w2)[D], const u64 (&q2)[D], u64 one2) {
-    if constexpr (MODE == MORL_DOT_UNFUSED) {
-        u64 acc = mul2(w2[0], q2[0]);
-#pragma unroll
-        for (int r = 1; r < D; ++r) acc = fma2(acc, one2, mul2(w2[r], q2[r]));
-        return acc;
-    } else if constexpr (MODE == MORL_DOT_FMA) {
-        u64 acc = mul2(w2[0], q2[0]);
-#pragma unroll
-        for (int r = 1; r < D; ++r) acc = fma2(w2[r], q2[r], acc);
-        return acc;
-    } else {
-        u64 acc = 0;
-#pragma unroll
-        for (int r = 0; r + 1 < D; r += 2) {
-            const u64 p = fma2(w2[r + 1], q2[r + 1], mul2(w2[r], q2[r]));
-            acc = (r == 0) ? p : fma2(acc, one2, p);
-        }
-        if constexpr (D % 2 == 1) {
-            const u64 t = mul2(w2[D - 1], q2[D - 1]);
-            acc = (D == 1) ? t : fma2(acc, one2, t);
-        }
-        return acc;
-    }
-}
-
-// ---- 1-D bulk async copy (TMA, UBLKCP) + mbarrier helpers -----------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)), "l"(src),
-                 "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "WAIT_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra DONE_%=;\n\t"
-        "bra WAIT_%=;\n\t"
-        "DONE_%=:\n\t}" ::"r"(smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
-
-// v3 kernel.  On top of the packed arithmetic described above:
+// v3 kernel: CUDA-core fast path for the shapes the weight-pair kernel below does not take (|W| <= 32, W*A not a multiple of 16).
+//   * Q_on[b] arrives by a 1-D bulk async copy (AoS staging) and is transposed once, smem -> smem, into SoA planes Qs[r][c]
+//     (c = j*A + a), so one LDS.128 yields the r-th objective of four consecutive candidates.  The transposing pass walks
+//     candidates (no div/mod) and is bank-conflict free for odd D;
+//   * candidates are scanned in groups of 8: eight FMA-chain scores, max of 8, and only the GROUP index of the running maximum is
+//     tracked (strict '>' keeps the first group); the exact (first) position inside the winning group is recovered afterwards by
+//     re-evaluating its 8 scores in the contract arithmetic and taking the first strict maximum;
 //   * FILTER (MODE != FMA): the scan uses the 3-op FMA chain t = fma(w2,q2, fma(w1,q1, w0*q0)) as an approximation of the
 //     contract arithmetic e (5 roundings).  |t - e| <= 6u * sum_r |w_r q_r| < eps := 2^-21 * (sum_r |w_r|) * max|Q_on[b]|.
 //     Per weight the scan keeps the best group maximum, its (first) group, and the runner-up group maximum.  If
@@ -224,15 +142,14 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 //     smaller than the best group's maximum, so the exact first argmax lies in that group and is found by evaluating its 8
 //     candidates in the contract arithmetic.  Otherwise (near tie, ~1e-4 of the rows on continuous data; always for constant
 //     or non-finite Q) the row is re-scanned exactly by its whole warp.  The result is bit-identical to the exact scan.
-//   * Q_tg[b] is staged with one 1-D bulk async copy (TMA) that overlaps the scan; reward/done are pre-loaded;
-//   * the transposing Q_on load walks candidates (no div/mod), bank-conflict free.
+//   * Q_tg[b] is staged with one 1-D bulk async copy that overlaps the scan; reward/done are pre-loaded.
+// =================================================================================================================
 template <int D, int MODE>
 __global__ void __launch_bounds__(256) envelope_td_v3_kernel(const float* __restrict__ q_on, const float* __restrict__ q_tg,
                                                              const float* __restrict__ wset, const float* __restrict__ reward,
-                                                             const float* __restrict__ done, float gamma, float one, int B, int W,
-                                                             int A, int Cp, int CS, int gps, int row_order,
-                                                             float* __restrict__ target_out, int32_t* __restrict__ pref_out,
-                                                             int32_t* __restrict__ act_out) {
+                                                             const float* __restrict__ done, float gamma, int B, int W, int A,
+                                                             int Cp, int CS, int gps, int row_order, float* __restrict__ target_out,
+                                                             int32_t* __restrict__ pref_out, int32_t* __restrict__ act_out) {
     constexpr bool FILTER = (MODE != MORL_DOT_FMA);
     constexpr int SCAN_MODE = MORL_DOT_FMA;  // arithmetic of the scan: the FMA chain (exact when MODE == FMA)
     extern __shared__ __align__(16) float smem[];
@@ -255,15 +172,12 @@ __global__ void __launch_bounds__(256) envelope_td_v3_kernel(const float* __rest
     const bool active = i < W;
     const int lane = threadIdx.x & 31;
     const int nwarps = blockDim.x >> 5;
-    const u64 one2 = pk2(one, one);
 
     float w[D];
-    u64 w2[D];
     float wsum = 0.f;
 #pragma unroll
     for (int r = 0; r < D; ++r) {
         w[r] = active ? __ldg(wset + (size_t)i * D + r) : 0.f;
-        w2[r] = pk2(w[r], w[r]);
         wsum += fabsf(w[r]);
     }
     const int ngroups = (C + 7) / 8;
@@ -273,8 +187,9 @@ __global__ void __launch_bounds__(256) envelope_td_v3_kernel(const float* __rest
     const uint32_t qt_bytes = (uint32_t)(C * D) * 4u;  // multiple of 16 (launcher)
 
     if (threadIdx.x == 0) {
-        mbar_init(bar, 1);
-        mbar_init(bar_on, 1);
+        g_mbar_init(bar, 1);
+        g_mbar_init(bar_on, 1);
+        g_mbar_init_fence();
     }
     for (int t = threadIdx.x; t < (Cp - C) * D; t += blockDim.x) Qs[(t / (Cp - C)) * plane + C + t % (Cp - C)] = 0.f;
     __syncthreads();
@@ -282,9 +197,9 @@ __global__ void __launch_bounds__(256) envelope_td_v3_kernel(const float* __rest
     uint32_t parity = 0;
     for (int b = blockIdx.x; b < B; b += gridDim.x, parity ^= 1u) {
         if (threadIdx.x == 0) {
-            mbar_expect_tx(bar_on, qt_bytes);
+            g_mbar_expect_tx(bar_on, qt_bytes);
             bulk_g2s(Qa, q_on + (size_t)b * C * D, qt_bytes, bar_on);
-            mbar_expect_tx(bar, qt_bytes);
+            g_mbar_expect_tx(bar, qt_bytes);
             bulk_g2s(Qt, q_tg + (size_t)b * C * D, qt_bytes, bar);
         }
         // pre-load the per-transition scalars of the epilogue
@@ -299,7 +214,7 @@ __global__ void __launch_bounds__(256) envelope_td_v3_kernel(const float* __rest
         // (reads at stride D words are bank-conflict free for odd D; the running max |q| feeds the filter threshold)
         float amax = 0.f;
         {
-            mbar_wait(bar_on, parity);
+            g_mbar_wait(bar_on, parity);
             for (int c = threadIdx.x; c < C; c += blockDim.x) {
                 float x[D];
 #pragma unroll
@@ -322,30 +237,34 @@ __global__ void __launch_bounds__(256) envelope_td_v3_kernel(const float* __rest
         if (FILTER)
             for (int k = 0; k < nwarps; ++k) qmax = fmaxf(qmax, red_amax[k]);
 
-        // ---- scan: groups of 8 candidates, packed FMA-chain scores, best / runner-up group maxima ----
+        // ---- scan: groups of 8 candidates, FMA-chain scores, best / runner-up group maxima ----
         float best = -INFINITY, second = -INFINITY;
         int bg = INT_MAX;
         auto scan_group = [&](int g, bool tail) {
             const int c0 = 8 * g;
-            u64 q2[4][D];
+            float q[8][D];
 #pragma unroll
             for (int r = 0; r < D; ++r) {
                 const float4 lo = *reinterpret_cast<const float4*>(Qs + r * plane + c0);
                 const float4 hi = *reinterpret_cast<const float4*>(Qs + r * plane + c0 + 4);
-                q2[0][r] = pk2(lo.x, lo.y);
-                q2[1][r] = pk2(lo.z, lo.w);
-                q2[2][r] = pk2(hi.x, hi.y);
-                q2[3][r] = pk2(hi.z, hi.w);
+                q[0][r] = lo.x;
+                q[1][r] = lo.y;
+                q[2][r] = lo.z;
+                q[3][r] = lo.w;
+                q[4][r] = hi.x;
+                q[5][r] = hi.y;
+                q[6][r] = hi.z;
+                q[7][r] = hi.w;
             }
             float x[8];
 #pragma unroll
-            for (int p = 0; p < 4; ++p) upk2(dotw2<D, SCAN_MODE>(w2, q2[p], one2), x[2 * p], x[2 * p + 1]);
+            for (int k = 0; k < 8; ++k) x[k] = dotw<D, SCAN_MODE>(w, q[k]);
             if (tail) {
 #pragma unroll
                 for (int k = 0; k < 8; ++k)
                     if (c0 + k >= C) x[k] = -INFINITY;
             }
-            const float m = fmaxf(max3(x[0], x[1], x[2]), max3(max3(x[3], x[4], x[5]), x[6], x[7]));
+            const float m = fmaxf(wp::max3(x[0], x[1], x[2]), wp::max3(wp::max3(x[3], x[4], x[5]), x[6], x[7]));
             if (FILTER) second = fmaxf(second, fminf(best, m));
             if (m > best) {
                 best = m;
@@ -418,7 +337,7 @@ __global__ void __launch_bounds__(256) envelope_td_v3_kernel(const float* __rest
                     if (lane == L) cstar = (bc == INT_MAX) ? 0 : bc;
                 }
             }
-            mbar_wait(bar, parity);  // Q_tg[b] has landed in shared memory
+            g_mbar_wait(bar, parity);  // Q_tg[b] has landed in shared memory
             if (active) {
                 const int jstar = cstar / A;
                 const int astar = cstar - jstar * A;
@@ -435,216 +354,57 @@ __global__ void __launch_bounds__(256) envelope_td_v3_kernel(const float* __rest
 }
 
 // =================================================================================================================
-// v5 kernel ("weight pairs"): the same FMA-chain filter + exact re-check as v3, re-blocked so that
-//   * a thread owns TWO scalarising weights packed in f32x2 registers and the candidate value is the scalar operand of the packed
-//     a multiply / FMA pair per candidate: one LDS.128 of the AoS block feeds two weights, so the
-//     shared-memory traffic per score halves and Q_on[b] is consumed exactly as the bulk copy (TMA) delivered it -- the
-//     AoS -> SoA transposition pass of v3 (and its barrier) disappears;
-//   * a warp covers all 64 weights of a weight block (lane = weight pair) and one quarter of the candidates, so every
-//     shared-memory read is a warp-wide broadcast;
-//   * groups of 16 candidates (book-keeping amortised over twice as many scores); the winner group is re-evaluated in the
-//     contract arithmetic by two threads per weight.
-// 2.9 instructions per score instead of 3.8.  Shapes: W*A a multiple of 16, 16-byte multiple Q blocks, |W| > 32 (below that half of
-// the lanes would idle and v3 is used).  Bit-identical to v1 / v3 / the oracle (tests/test_kernels_gpu.py).
+// Weight-pair kernel, the default whenever the shape fits: one 128-thread CTA per block of 64 scalarising weights (blockIdx.y),
+// persistent over the transitions b.  Q_on[b] and Q_tg[b] arrive by 1-D bulk async copies and are consumed as delivered (AoS, no
+// transposition); the scan of a transition is wp::scan_transition (envelope_wp.cuh), the same code as in the fused head of
+// qhead_envelope.cu.  Shapes: W*A a multiple of 16, 16-byte multiple Q blocks, |W| > 32 (below that half of the lanes would idle and
+// v3 is used).
 // =================================================================================================================
 template <int D, int MODE>
 __global__ void __launch_bounds__(128) envelope_td_wp_kernel(const float* __restrict__ q_on, const float* __restrict__ q_tg,
                                                              const float* __restrict__ wset, const float* __restrict__ reward,
                                                              const float* __restrict__ done, float gamma, int B, int W, int A,
                                                              int row_order, float* __restrict__ target_out,
-                                                             int32_t* __restrict__ pref_out, int32_t* __restrict__ act_out, int pdl) {
-    constexpr bool FILTER = (MODE != MORL_DOT_FMA);
+                                                             int32_t* __restrict__ pref_out, int32_t* __restrict__ act_out) {
     extern __shared__ __align__(16) float smem[];
     const int C = W * A;
     const int CDp = (C * D + 3) & ~3;
-    if (pdl) {
-        // programmatic dependent launch: this grid was allowed to become resident while its predecessor in the stream was still
-        // draining; let OUR successor do the same, then wait until the predecessor's results are visible before any global read
-        asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        asm volatile("griddepcontrol.wait;" ::: "memory");
-    }
-    float* Qa = smem;                                         // [C*D] AoS Q_on[b]  (bulk async copy)
-    float* Qt = Qa + CDp;                                     // [C*D] AoS Q_tg[b]  (bulk async copy)
-    float* red_v = Qt + CDp;                                  // [4][64] best group maximum per (candidate quarter, weight)
-    float* red_s = red_v + 256;                               // [4][64] runner-up
-    int* red_g = reinterpret_cast<int*>(red_s + 256);         // [4][64] group of best
-    unsigned* red_amax = reinterpret_cast<unsigned*>(red_g + 256);  // [4]
-    uint64_t* bar_on = reinterpret_cast<uint64_t*>(red_amax + 4);
+    float* Qa = smem;                                              // [C*D] AoS Q_on[b]  (bulk async copy)
+    float* Qt = Qa + CDp;                                          // [C*D] AoS Q_tg[b]  (bulk async copy)
+    wp::Scratch* sc = reinterpret_cast<wp::Scratch*>(Qt + CDp);
+    uint64_t* bar_on = reinterpret_cast<uint64_t*>(sc + 1);
     uint64_t* bar_tg = bar_on + 1;
 
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x, part = tid & 1;
     const int wbase = blockIdx.y * 64;
-    // scan role: lane = weight pair, warp = candidate quarter
-    const int i0 = wbase + 2 * lane, i1 = i0 + 1;
-    u64 wp2[D];
-#pragma unroll
-    for (int r = 0; r < D; ++r) wp2[r] = pk2(i0 < W ? __ldg(wset + (size_t)i0 * D + r) : 0.f, i1 < W ? __ldg(wset + (size_t)i1 * D + r) : 0.f);
-    // finish role: thread pair (2 k, 2 k + 1) finishes weight wbase + k
-    const int fi = wbase + (tid >> 1), part = tid & 1;
-    const bool f_active = fi < W;
-    float fw[D];
-    float wsum = 0.f;
-#pragma unroll
-    for (int r = 0; r < D; ++r) {
-        fw[r] = f_active ? __ldg(wset + (size_t)fi * D + r) : 0.f;
-        wsum += fabsf(fw[r]);
-    }
-    const int ngroups = C >> 4;
-    const int gpw = (ngroups + 3) >> 2;
-    const int g_begin = warp * gpw, g_end = min(g_begin + gpw, ngroups);
+    wp::Role<D> role;
+    wp::load_role<D>(role, wset + (size_t)wbase * D, W - wbase, tid);
+    const int fi = wbase + role.fi;
     const uint32_t q_bytes = (uint32_t)(C * D) * 4u;  // multiple of 16 (launcher)
 
     if (tid == 0) {
-        mbar_init(bar_on, 1);
-        mbar_init(bar_tg, 1);
+        g_mbar_init(bar_on, 1);
+        g_mbar_init(bar_tg, 1);
+        g_mbar_init_fence();
     }
     __syncthreads();
 
     uint32_t parity = 0;
     for (int b = blockIdx.x; b < B; b += gridDim.x, parity ^= 1u) {
         if (tid == 0) {
-            mbar_expect_tx(bar_on, q_bytes);
+            g_mbar_expect_tx(bar_on, q_bytes);
             bulk_g2s(Qa, q_on + (size_t)b * C * D, q_bytes, bar_on);
-            mbar_expect_tx(bar_tg, q_bytes);
+            g_mbar_expect_tx(bar_tg, q_bytes);
             bulk_g2s(Qt, q_tg + (size_t)b * C * D, q_bytes, bar_tg);
         }
         float rw[D];
         const float dn = __ldg(done + b);
 #pragma unroll
         for (int r = 0; r < D; ++r) rw[r] = __ldg(reward + (size_t)b * D + r);
-        mbar_wait(bar_on, parity);
-
-        // ---- max |Q_on[b]| for the filter threshold (integer max of the magnitude bits: NaN / inf sort above every finite value) ----
-        if (FILTER) {
-            unsigned am = 0u;
-            for (int t = tid; t < (C * D) >> 2; t += 128) {
-                const uint4 x = *reinterpret_cast<const uint4*>(Qa + 4 * t);
-                am = max(max(am, x.x & 0x7FFFFFFFu), max(x.y & 0x7FFFFFFFu, max(x.z & 0x7FFFFFFFu, x.w & 0x7FFFFFFFu)));
-            }
-#pragma unroll
-            for (int off = 16; off > 0; off >>= 1) am = max(am, __shfl_xor_sync(0xffffffffu, am, off));
-            if (lane == 0) red_amax[warp] = am;
-        }
-
-        // ---- scan: groups of 16 candidates, two weights per thread, FMA-chain scores ----
-        float best0 = -INFINITY, second0 = -INFINITY, best1 = -INFINITY, second1 = -INFINITY;
-        int bg0 = INT_MAX, bg1 = INT_MAX;
-#pragma unroll 1
-        for (int g = g_begin; g < g_end; ++g) {
-            const float4* src = reinterpret_cast<const float4*>(Qa + (size_t)g * 16 * D);
-            float m0 = -INFINITY, m1 = -INFINITY;
-#pragma unroll
-            for (int sub = 0; sub < 4; ++sub) {
-                float f[4 * D];
-#pragma unroll
-                for (int v = 0; v < D; ++v) {
-                    const float4 x = src[sub * D + v];
-                    f[4 * v + 0] = x.x;
-                    f[4 * v + 1] = x.y;
-                    f[4 * v + 2] = x.z;
-                    f[4 * v + 3] = x.w;
-                }
-                float lo[4], hi[4];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    u64 acc = mul2(wp2[0], pk2(f[k * D], f[k * D]));
-#pragma unroll
-                    for (int r = 1; r < D; ++r) acc = fma2(wp2[r], pk2(f[k * D + r], f[k * D + r]), acc);
-                    upk2(acc, lo[k], hi[k]);
-                }
-                m0 = max3(max3(m0, lo[0], lo[1]), lo[2], lo[3]);
-                m1 = max3(max3(m1, hi[0], hi[1]), hi[2], hi[3]);
-            }
-            if (FILTER) {
-                second0 = fmaxf(second0, fminf(best0, m0));
-                second1 = fmaxf(second1, fminf(best1, m1));
-            }
-            if (m0 > best0) {
-                best0 = m0;
-                bg0 = g;
-            }
-            if (m1 > best1) {
-                best1 = m1;
-                bg1 = g;
-            }
-        }
-        {
-            const int k0 = warp * 64 + 2 * lane;
-            *reinterpret_cast<float2*>(red_v + k0) = make_float2(best0, best1);
-            *reinterpret_cast<int2*>(red_g + k0) = make_int2(bg0, bg1);
-            if (FILTER) *reinterpret_cast<float2*>(red_s + k0) = make_float2(second0, second1);
-        }
-        __syncthreads();
-
-        // ---- finish weight fi: merge the four quarters (candidate order), exact re-check of the winning group ----
-        const int fl = tid >> 1;
-        float bb = -INFINITY, ss = -INFINITY;
-        int g = INT_MAX;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const float pb = red_v[k * 64 + fl];
-            if (FILTER) ss = fmaxf(fmaxf(ss, red_s[k * 64 + fl]), fminf(bb, pb));
-            if (pb > bb) {
-                bb = pb;
-                g = red_g[k * 64 + fl];
-            }
-        }
-        bool amb = false;
-        if (FILTER) {
-            const unsigned am = max(max(red_amax[0], red_amax[1]), max(red_amax[2], red_amax[3]));
-            const float qmax = am >= 0x7F800000u ? INFINITY : __uint_as_float(am);
-            const float thr = 1.9073486328125e-06f * wsum * qmax;  // 2^-19 * sum|w| * max|Q|
-            amb = f_active && !(ss < bb - thr);                    // also true for NaN / inf
-        }
-        int cstar = 0;
-        {
-            const int gg = (g == INT_MAX) ? 0 : g;  // every candidate was -inf / NaN: th.argmax returns 0 (found by the re-check below)
-            const int c0 = 16 * gg + 8 * part;
-            float ev = -INFINITY;
-            int ei = INT_MAX;
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                float q[D];
-#pragma unroll
-                for (int r = 0; r < D; ++r) q[r] = Qa[(c0 + k) * D + r];
-                const float s = dotw<D, MODE>(fw, q);
-                if (s > ev) {
-                    ev = s;
-                    ei = c0 + k;
-                }
-            }
-            const float ev2 = __shfl_xor_sync(0xffffffffu, ev, 1);
-            const int ei2 = __shfl_xor_sync(0xffffffffu, ei, 1);
-            argmax_merge(ev, ei, ev2, ei2);
-            cstar = (ei == INT_MAX) ? 0 : ei;
-        }
-        if (FILTER) {
-            // near ties: the whole warp re-scans the row exactly (rare)
-            unsigned ambmask = __ballot_sync(0xffffffffu, amb && part == 0);
-            while (ambmask) {
-                const int L = __ffs(ambmask) - 1;
-                ambmask &= ambmask - 1;
-                float wl[D];
-#pragma unroll
-                for (int r = 0; r < D; ++r) wl[r] = __shfl_sync(0xffffffffu, fw[r], L);
-                float bv = -INFINITY;
-                int bc = INT_MAX;
-                for (int c = lane; c < C; c += 32) {
-                    float q[D];
-#pragma unroll
-                    for (int r = 0; r < D; ++r) q[r] = Qa[c * D + r];
-                    const float s = dotw<D, MODE>(wl, q);
-                    if (s > bv) {
-                        bv = s;
-                        bc = c;
-                    }
-                }
-                warp_argmax(bv, bc);
-                if ((lane & ~1) == L) cstar = (bc == INT_MAX) ? 0 : bc;
-            }
-        }
-        mbar_wait(bar_tg, parity);  // Q_tg[b] has landed in shared memory
-        if (f_active) {
+        g_mbar_wait(bar_on, parity);
+        const int cstar = wp::scan_transition<D, MODE>(Qa, *sc, role, tid, C, [] { __syncthreads(); });
+        g_mbar_wait(bar_tg, parity);  // Q_tg[b] has landed in shared memory
+        if (role.f_active) {
             const size_t k = (row_order == MORL_ROWS_REFERENCE) ? ((size_t)fi * B + b) : ((size_t)b * W + fi);
             if (part == 0) {
                 const float* qt = Qt + (size_t)cstar * D;
@@ -656,27 +416,25 @@ __global__ void __launch_bounds__(128) envelope_td_wp_kernel(const float* __rest
                 if (act_out) act_out[k] = cstar - jstar * A;
             }
         }
-        __syncthreads();  // Qa / Qt / red_* are rewritten by the next transition
+        __syncthreads();  // Qa / Qt / the scratch are rewritten by the next transition
     }
 }
 
-struct EnvelopeV2Plan {
+struct EnvelopeV3Plan {
     bool ok;
-    int Cp, CS, gps, WI;
+    int Cp, CS, gps;
     dim3 grid, block;
     size_t smem;
 };
 
-static EnvelopeV2Plan plan_envelope_v2(int B, int W, int A, int D, int sm_count) {
-    EnvelopeV2Plan p{};
-    (void)B;
-    (void)sm_count;
+static EnvelopeV3Plan plan_envelope_v3(int W, int A, int D) {
+    EnvelopeV3Plan p{};
     const long long C = (long long)W * A;
     p.ok = false;
     if ((C * D) % 4 != 0) return p;  // Q_tg[b] must be a 16-byte multiple for the bulk copy
     const int Wp = (W + 31) / 32 * 32;
-    p.WI = Wp < 256 ? Wp : 256;
-    const int warps_i = p.WI / 32;
+    const int WI = Wp < 256 ? Wp : 256;
+    const int warps_i = WI / 32;
     int cs = 4 / warps_i;
     if (cs < 1) cs = 1;
     const int ngroups = (int)((C + 7) / 8);
@@ -684,12 +442,12 @@ static EnvelopeV2Plan plan_envelope_v2(int B, int W, int A, int D, int sm_count)
     p.CS = cs;
     p.gps = (ngroups + cs - 1) / cs;
     p.Cp = ngroups * 8;
-    p.block = dim3((unsigned)(p.WI * p.CS), 1, 1);
+    p.block = dim3((unsigned)(WI * p.CS), 1, 1);
     const size_t qs = (size_t)D * p.Cp * sizeof(float);
     const size_t qt = (((size_t)C * D + 3) & ~(size_t)3) * sizeof(float);
-    p.smem = qs + 2 * qt + 3 * (size_t)p.CS * p.WI * sizeof(float) + 32 * sizeof(float) + 16;
+    p.smem = qs + 2 * qt + 3 * (size_t)p.CS * WI * sizeof(float) + 32 * sizeof(float) + 16;
     if (p.smem > 96 * 1024) return p;
-    p.grid = dim3(1u, (unsigned)((W + p.WI - 1) / p.WI), 1);  // grid.x is set by the launcher from the measured occupancy
+    p.grid = dim3(1u, (unsigned)((W + WI - 1) / WI), 1);  // grid.x is set by the launcher from the measured occupancy
     p.ok = true;
     return p;
 }
@@ -721,17 +479,25 @@ static EnvelopePlan plan_envelope(int B, int W, int A, int D) {
     return p;
 }
 
-// Path selection, read on every call: MORL_ENVELOPE_PATH = "v1" (generic kernel), "v3" (CUDA-core fast path), "wp" (v5, weight-pair
-// re-blocking of v3; the default whenever the shape fits, then v3, then v1).  MORL_ENVELOPE_FORCE_V1 is the
-// older spelling of "v1".
-static int envelope_path_override() {
-    if (getenv("MORL_ENVELOPE_FORCE_V1") != nullptr) return 1;
+// grid.x of the persistent kernels: every transition co-resident in one wave when they fit, else CTAs striding over b
+static unsigned persistent_grid_x(int sms, int occ, unsigned gy, int B) {
+    long long gx = (long long)sms * (occ < 1 ? 1 : occ) / gy;
+    if (gx < 1) gx = 1;
+    if (gx > B) gx = B;
+    return (unsigned)gx;
+}
+
+// Path selection, read on every call: MORL_ENVELOPE_PATH = "v1" (generic kernel), "v3" (CUDA-core fast path), "wp" (weight-pair
+// kernel).  Unset: "wp" whenever the shape fits, then "v3", then "v1".
+enum EnvelopePath { kPathAuto, kPathV1, kPathV3, kPathWp };
+
+static EnvelopePath envelope_path_override() {
     const char* e = getenv("MORL_ENVELOPE_PATH");
-    if (!e) return 0;
-    if (e[0] == 'v' && e[1] == '1') return 1;
-    if (e[0] == 'v' && e[1] == '3') return 3;
-    if (e[0] == 'w' && e[1] == 'p') return 5;
-    return 0;
+    if (!e) return kPathAuto;
+    if (e[0] == 'v' && e[1] == '1') return kPathV1;
+    if (e[0] == 'v' && e[1] == '3') return kPathV3;
+    if (e[0] == 'w' && e[1] == 'p') return kPathWp;
+    return kPathAuto;
 }
 
 }  // namespace morl
@@ -753,80 +519,42 @@ extern "C" int morl_envelope_td_f32(const float* q_online, const float* q_target
     MORL_REQUIRE(aligned16(q_online) && aligned16(q_target) && aligned16(target_out), MORL_ERR_ALIGN,
                  "morl_envelope_td_f32: q_online/q_target/target_out must be 16-byte aligned");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    static int sm_count_cached = 0;
-    if (sm_count_cached == 0) {
-        int dev = 0, n = 0;
-        if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
-            sm_count_cached = n;
-        else {
-            (void)cudaGetLastError();
-            sm_count_cached = 132;
-        }
-    }
-    const int path = envelope_path_override();
-    // v5 (weight pairs): the default fast path when the shape fits; "wp" forces it, "v3" / "v1" skip it
+    int sms = morl_device_sm_count();
+    if (sms <= 0) sms = 132;
+    const EnvelopePath path = envelope_path_override();
     const long long Cw = (long long)W * A;
-    const bool wp_ok = W > 32 && (Cw % 16) == 0 && ((Cw * D) % 4) == 0 && (2 * ((Cw * D + 3) & ~3LL) + 3 * 256 + 16) * 4 <= 96 * 1024;
-    MORL_REQUIRE(path != 5 || wp_ok, MORL_ERR_UNSUPPORTED, "morl_envelope_td_f32: MORL_ENVELOPE_PATH=wp but the shape W=%d A=%d D=%d is outside the weight-pair path", W, A, D);
-    if (wp_ok && (path == 0 || path == 5)) {
-        bool launched5 = false;
-        const size_t smem5 = (size_t)(2 * ((Cw * D + 3) & ~3LL) + 3 * 256 + 16) * 4;
+    const size_t wp_smem = (size_t)(2 * ((Cw * D + 3) & ~3LL) + 3 * 256 + 16) * 4;  // Q_on[b], Q_tg[b], wp::Scratch, barriers
+    const bool wp_ok = W > 32 && (Cw % 16) == 0 && ((Cw * D) % 4) == 0 && wp_smem <= 96 * 1024;
+    MORL_REQUIRE(path != kPathWp || wp_ok, MORL_ERR_UNSUPPORTED, "morl_envelope_td_f32: MORL_ENVELOPE_PATH=wp but the shape W=%d A=%d D=%d is outside the weight-pair path", W, A, D);
+    if (wp_ok && (path == kPathAuto || path == kPathWp)) {
+        bool launched = false;
         MORL_DISPATCH_D(D, MORL_DISPATCH_MODE(dot_mode, {
                             auto kern = envelope_td_wp_kernel<kD, kMode>;
-                            if (smem5 > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem5);
+                            if (wp_smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wp_smem);
                             int occ = 0;
-                            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 128, smem5);
-                            if (occ < 1) occ = 1;
+                            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 128, wp_smem);
                             const unsigned gy = (unsigned)((W + 63) / 64);
-                            long long gx = (long long)sm_count_cached * occ / gy;
-                            if (gx < 1) gx = 1;
-                            if (gx > B) gx = B;
-                            // opt-in only: it can help when one CTA per SM is resident and in launch-bound python loops, but at the north-star
-                            // shape the next grid's early CTAs compete with the resident CTAs of the running grid (not measured on H100)
-                            static const bool want_pdl = [] { const char* e = getenv("MORL_ENVELOPE_PDL"); return e && e[0] == '1'; }();
-                            if (want_pdl) {
-                                // programmatic stream serialisation: the grid may start (barrier init, CTA residency) while the previous
-                                // kernel of the stream drains; the kernel's griddepcontrol.wait restores the data dependency
-                                cudaLaunchConfig_t cfg = {};
-                                cfg.gridDim = dim3((unsigned)gx, gy, 1);
-                                cfg.blockDim = dim3(128, 1, 1);
-                                cfg.dynamicSmemBytes = smem5;
-                                cfg.stream = st;
-                                cudaLaunchAttribute attr[1];
-                                attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-                                attr[0].val.programmaticStreamSerializationAllowed = 1;
-                                cfg.attrs = attr;
-                                cfg.numAttrs = 1;
-                                cudaLaunchKernelEx(&cfg, kern, q_online, q_target, wset, reward, done, gamma, B, W, A, row_order, target_out, pref_out,
-                                                   act_out, 1);
-                            } else {
-                                kern<<<dim3((unsigned)gx, gy, 1), 128, smem5, st>>>(q_online, q_target, wset, reward, done, gamma, B, W, A, row_order,
-                                                                                  target_out, pref_out, act_out, 0);
-                            }
-                            launched5 = true;
+                            kern<<<dim3(persistent_grid_x(sms, occ, gy, B), gy, 1), 128, wp_smem, st>>>(
+                                q_online, q_target, wset, reward, done, gamma, B, W, A, row_order, target_out, pref_out, act_out);
+                            launched = true;
                         }));
-        MORL_REQUIRE(launched5, MORL_ERR_UNSUPPORTED, "morl_envelope_td_f32: no weight-pair kernel for D=%d mode=%d", D, dot_mode);
+        MORL_REQUIRE(launched, MORL_ERR_UNSUPPORTED, "morl_envelope_td_f32: no weight-pair kernel for D=%d mode=%d", D, dot_mode);
         return check_launch("morl_envelope_td_f32(wp)");
     }
-    EnvelopeV2Plan p2 = plan_envelope_v2(B, W, A, D, sm_count_cached);
-    if (p2.ok && path != 1) {
-        bool launched2 = false;
+    EnvelopeV3Plan p3 = plan_envelope_v3(W, A, D);
+    if (p3.ok && path != kPathV1) {
+        bool launched = false;
         MORL_DISPATCH_D(D, MORL_DISPATCH_MODE(dot_mode, {
                             auto kern = envelope_td_v3_kernel<kD, kMode>;
-                            if (p2.smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p2.smem);
+                            if (p3.smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p3.smem);
                             int occ = 0;
-                            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, (int)p2.block.x, p2.smem);
-                            if (occ < 1) occ = 1;
-                            // all transitions co-resident in one wave when they fit, else persistent CTAs striding over b
-                            long long gx = (long long)sm_count_cached * occ / (long long)p2.grid.y;
-                            if (gx < 1) gx = 1;
-                            if (gx > B) gx = B;
-                            p2.grid.x = (unsigned)gx;
-                            kern<<<p2.grid, p2.block, p2.smem, st>>>(q_online, q_target, wset, reward, done, gamma, 1.0f, B, W, A, p2.Cp,
-                                                                      p2.CS, p2.gps, row_order, target_out, pref_out, act_out);
-                            launched2 = true;
+                            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, (int)p3.block.x, p3.smem);
+                            p3.grid.x = persistent_grid_x(sms, occ, p3.grid.y, B);
+                            kern<<<p3.grid, p3.block, p3.smem, st>>>(q_online, q_target, wset, reward, done, gamma, B, W, A, p3.Cp, p3.CS, p3.gps,
+                                                                      row_order, target_out, pref_out, act_out);
+                            launched = true;
                         }));
-        MORL_REQUIRE(launched2, MORL_ERR_UNSUPPORTED, "morl_envelope_td_f32: no fast-path kernel for D=%d mode=%d", D, dot_mode);
+        MORL_REQUIRE(launched, MORL_ERR_UNSUPPORTED, "morl_envelope_td_f32: no fast-path kernel for D=%d mode=%d", D, dot_mode);
         return check_launch("morl_envelope_td_f32(v3)");
     }
     const EnvelopePlan p = plan_envelope(B, W, A, D);

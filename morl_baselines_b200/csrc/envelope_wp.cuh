@@ -1,12 +1,12 @@
-// envelope_wp.cuh -- the "weight pair" envelope scan of ONE transition by a group of 128 threads, as a device function, so that the
-// operator can run inside another kernel's epilogue (qhead_envelope.cu: the Q tiles are produced in shared memory by the output layer's
-// tensor-core GEMMs and never exist in HBM).  Same algorithm, arithmetic and tie rules as envelope_td_wp_kernel (envelope_td.cu):
-//   scan   : lane = weight pair (two scalarising weights packed in f32x2 registers), warp = candidate quarter, groups of 16 candidates,
-//            FMA-chain scores (the FILTER), best / runner-up group maxima per weight;
+// envelope_wp.cuh -- the "weight pair" envelope scan of ONE transition by a group of 128 threads, as a device function.  It is the body of
+// the standalone operator (envelope_td_wp_kernel, envelope_td.cu: Q tiles bulk-copied from HBM) and of the fused head (qhead_envelope.cu:
+// the Q tiles are produced in shared memory by the output layer's tensor-core GEMMs and never exist in HBM), so the two are one algorithm:
+//   scan   : lane = weight pair (a thread scores every candidate against two scalarising weights), warp = candidate quarter, groups of 16
+//            candidates, FMA-chain scores (the FILTER), best / runner-up group maxima per weight;
 //   finish : thread pair (2k, 2k+1) re-evaluates weight k's winning group in the CONTRACT arithmetic (first occurrence), near ties
 //            (runner-up within 2^-19 * sum|w| * max|Q| of the best) are re-scanned exactly by the whole warp;
-//   output : r + ((1 - done) gamma) Q_tg[b, j*, a*, :]  (reference multi_policy/envelope/envelope.py:422-440, 298).
-// Bit-identical to the standalone operator on identical Q tiles (tests/test_qhead_envelope_gpu.py).
+//   output : r + ((1 - done) gamma) Q_tg[b, j*, a*, :]  (reference multi_policy/envelope/envelope.py:422-440, 298), written by the caller.
+// Bit-identical to the v1 / v3 kernels and the oracle (tests/test_kernels_gpu.py, tests/test_qhead_envelope_gpu.py).
 #pragma once
 #include <limits.h>
 
@@ -15,28 +15,7 @@
 namespace morl {
 namespace wp {
 
-typedef unsigned long long u64;
-__device__ __forceinline__ u64 pk2(float lo, float hi) {
-    u64 r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void upk2(u64 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-// Hopper has no packed-fp32 arithmetic and no 3-input max: the pair forms below are two scalar IEEE operations on the halves of the
-// register pair (the same values a packed instruction would give), the 3-input max two FMNMX
-__device__ __forceinline__ u64 mul2(u64 a, u64 b) {
-    float a0, a1, b0, b1;
-    upk2(a, a0, a1);
-    upk2(b, b0, b1);
-    return pk2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
-}
-__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
-    float a0, a1, b0, b1, c0, c1;
-    upk2(a, a0, a1);
-    upk2(b, b0, b1);
-    upk2(c, c0, c1);
-    return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
-}
+// Hopper has no 3-input max: two FMNMX
 __device__ __forceinline__ float max3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 
 // per-group scratch in shared memory: [4][64] best group maximum, runner-up, group of best; [4] max |Q| bits per warp
@@ -50,19 +29,23 @@ struct Scratch {
 // per-thread constants of a group member (the weight set does not change between transitions)
 template <int D>
 struct Role {
-    u64 wp2[D];    // scan role: weights 2*lane, 2*lane + 1
-    float fw[D];   // finish role: weight tid >> 1
+    float w0[D], w1[D];  // scan role: weights 2*lane, 2*lane + 1
+    float fw[D];         // finish role: weight tid >> 1
     float wsum;
-    int fi;        // finish weight index
+    int fi;              // finish weight index
     bool f_active;
 };
 
+// `wset` / `W`: the group's weights (a block of at most 64 of them); weights at or past W are zero and their outputs inactive
 template <int D>
 __device__ __forceinline__ void load_role(Role<D>& ro, const float* __restrict__ wset, int W, int tid) {
     const int lane = tid & 31;
     const int i0 = 2 * lane, i1 = i0 + 1;
 #pragma unroll
-    for (int r = 0; r < D; ++r) ro.wp2[r] = pk2(i0 < W ? __ldg(wset + (size_t)i0 * D + r) : 0.f, i1 < W ? __ldg(wset + (size_t)i1 * D + r) : 0.f);
+    for (int r = 0; r < D; ++r) {
+        ro.w0[r] = i0 < W ? __ldg(wset + (size_t)i0 * D + r) : 0.f;
+        ro.w1[r] = i1 < W ? __ldg(wset + (size_t)i1 * D + r) : 0.f;
+    }
     ro.fi = tid >> 1;
     ro.f_active = ro.fi < W;
     ro.wsum = 0.f;
@@ -73,10 +56,10 @@ __device__ __forceinline__ void load_role(Role<D>& ro, const float* __restrict__
     }
 }
 
-// One transition.  Qa / Qt: AoS [C][D] tiles of Q_on[b] / Q_tg[b] in shared memory (C = W*A candidates, c = j*A + a, C % 16 == 0,
-// C*D % 4 == 0, 16-byte aligned).  `tid` in [0, 128) is the thread's index in its group, `sync()` a barrier over exactly the group.
+// One transition.  Qa: AoS [C][D] tile of Q_on[b] in shared memory (C = W*A candidates, c = j*A + a, C % 16 == 0, C*D % 4 == 0, 16-byte
+// aligned).  `tid` in [0, 128) is the thread's index in its group, `sync()` a barrier over exactly the group.
 // Returns the winning candidate c* (valid when ro.f_active); the caller writes the outputs.  Ends with the group in step (one barrier
-// inside); the caller must barrier once more before Qa / Qt / the scratch are rewritten.
+// inside); the caller must barrier once more before Qa / the scratch are rewritten.
 template <int D, int MODE, typename SyncF>
 __device__ __forceinline__ int scan_transition(const float* __restrict__ Qa, Scratch& sc, const Role<D>& ro, int tid, int C, SyncF sync) {
     constexpr bool FILTER = (MODE != MORL_DOT_FMA);
@@ -115,16 +98,17 @@ __device__ __forceinline__ int scan_transition(const float* __restrict__ Qa, Scr
                 f[4 * v + 2] = x.z;
                 f[4 * v + 3] = x.w;
             }
-            float lo[4], hi[4];
+            float s0[4], s1[4];
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
-                u64 acc = mul2(ro.wp2[0], pk2(f[k * D], f[k * D]));
+                float q[D];
 #pragma unroll
-                for (int r = 1; r < D; ++r) acc = fma2(ro.wp2[r], pk2(f[k * D + r], f[k * D + r]), acc);
-                upk2(acc, lo[k], hi[k]);
+                for (int r = 0; r < D; ++r) q[r] = f[k * D + r];
+                s0[k] = dotw<D, MORL_DOT_FMA>(ro.w0, q);
+                s1[k] = dotw<D, MORL_DOT_FMA>(ro.w1, q);
             }
-            m0 = max3(max3(m0, lo[0], lo[1]), lo[2], lo[3]);
-            m1 = max3(max3(m1, hi[0], hi[1]), hi[2], hi[3]);
+            m0 = max3(max3(m0, s0[0], s0[1]), s0[2], s0[3]);
+            m1 = max3(max3(m1, s1[0], s1[1]), s1[2], s1[3]);
         }
         if (FILTER) {
             second0 = fmaxf(second0, fminf(best0, m0));

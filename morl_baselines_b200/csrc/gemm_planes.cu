@@ -336,7 +336,7 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
             g_mbar_init(&full[s], 1);
             g_mbar_init(&empty[s], 8);  // one arrival per consumer warp
         }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        g_mbar_init_fence();
     }
     if (g.pdl) {
         // programmatic dependent launch: this grid may have become resident (barrier init above) while the previous kernel
@@ -542,7 +542,7 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
             g_mbar_init(&empty[s], 8);
         }
         for (int s = 0; s < kChainLanes; ++s) g_mbar_init(&stored[s], 8);  // the 8 consumer warps
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        g_mbar_init_fence();
     }
     if (g.pdl) {
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -762,7 +762,7 @@ gemm_planes_mn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
             g_mbar_init(&full[s], 1);
             g_mbar_init(&empty[s], 8);  // one arrival per consumer warp
         }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        g_mbar_init_fence();
     }
     __syncthreads();
     pdl_enter();  // (nothing above reads or writes global memory: barriers and the tile of ones overlap the predecessor)

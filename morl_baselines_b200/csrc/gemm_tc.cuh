@@ -1,5 +1,6 @@
 // gemm_tc.cuh -- wgmma / TMA / mbarrier PTX wrappers, the split-operand plane formats and the tensor-map helpers shared by
-// the tensor-core kernels of libmorl_b200.so (gemm_planes.cu, qhead_envelope.cu).  sm_90a only.
+// the tensor-core kernels of libmorl_b200.so (gemm_planes.cu, qhead_envelope.cu); envelope_td.cu uses the mbarrier and bulk-copy
+// wrappers.  sm_90a only.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -15,6 +16,8 @@ __device__ __forceinline__ uint32_t g_smem_u32(const void* p) { return (uint32_t
 __device__ __forceinline__ void g_mbar_init(uint64_t* bar, int count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(g_smem_u32(bar)), "r"(count));
 }
+// once after the last g_mbar_init, before any thread or bulk copy uses the barriers
+__device__ __forceinline__ void g_mbar_init_fence() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void g_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(g_smem_u32(bar)), "r"(bytes) : "memory");
 }
@@ -41,6 +44,12 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
         "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(g_smem_u32(dst)),
         "l"(map), "r"(g_smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
         : "memory");
+}
+// 1-D bulk copy of `bytes` (a multiple of 16; both addresses 16-byte aligned) from global to shared memory, completing on `bar`
+__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(g_smem_u32(dst)), "l"(src),
+                 "r"(bytes), "r"(g_smem_u32(bar))
+                 : "memory");
 }
 __device__ __forceinline__ uint64_t l2_policy_evict_first() {
     uint64_t p;

@@ -101,7 +101,7 @@ qhead_envelope_kernel(const __grid_constant__ CUtensorMap tmA_on, const __grid_c
             g_mbar_init(&empty[s], 8);  // one arrival per consumer warp (both groups walk every stage)
         }
         g_mbar_init(bfull, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        g_mbar_init_fence();
     }
     if (g.pdl) {  // nothing above reads global memory; everything below may (see gemm_planes_kernel)
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");

@@ -4,7 +4,9 @@
 
 Runs bench.py's envelope workload in fresh subprocesses, alternating A, B, A, B, ... with morl_baselines_b200._lib.LIB_PATH pointed at
 the given library, and prints per run `value`, `e2e.value`, the chained launch (`roofline.us_per_launch`), the per-layer launch
-(`roofline_gemm_layer.us_per_launch`) and the clocks / throttle reasons bench.py samples; then median and min-max per side, next to the
+(`roofline_gemm_layer.us_per_launch`), the envelope operator as the update runs it (`roofline_envelope.us_per_launch`: the fused head at
+the north-star shape) and standalone on Q tensors in HBM (`roofline_envelope_operator.us_per_launch`), and the clocks / throttle reasons
+bench.py samples; then median and min-max per side, next to the
 card's name and power limit.  With --dump-dir the first run of each side writes its outputs (bench.py --dump-outputs) and the script
 reports whether every array is bit-identical between the sides.  Needs a GPU: there is nothing to fall back to.  Changes no device
 setting; every child has exited when it returns."""
@@ -42,7 +44,7 @@ def run_once(lib, steps, warmup, dump):
         raise SystemExit(f"bench.py failed with {lib} (exit {r.returncode}):\n{r.stdout[-2000:]}\n{r.stderr[-4000:]}")
     d = json.loads(lines[-1])
     return {"value": d["value"], "e2e": d["e2e"]["value"], "chain_us": d["roofline"]["us_per_launch"], "layer_us": d["roofline_gemm_layer"]["us_per_launch"],
-            "clocks": d.get("clocks")}
+            "env_us": d["roofline_envelope"]["us_per_launch"], "env_op_us": d["roofline_envelope_operator"]["us_per_launch"], "clocks": d.get("clocks")}
 
 
 def same_dumps(dir_a, dir_b):
@@ -79,12 +81,12 @@ def main():
             res = run_once(lib, args.steps, args.warmup, dump)
             runs.append(res)
             print(f"{name} round {rnd}: value {res['value']:.1f} updates/s  e2e {res['e2e']:.1f}  chain {res['chain_us']:.1f} us  layer {res['layer_us']:.1f} us  "
-                  f"clocks {res['clocks']}", flush=True)
+                  f"envelope {res['env_us']:.2f} us  envelope operator {res['env_op_us']:.2f} us  clocks {res['clocks']}", flush=True)
     for name, (lib, runs) in sides.items():
         print(f"# {name} = {lib}")
-        for key in ("value", "e2e", "chain_us", "layer_us"):
+        for key in ("value", "e2e", "chain_us", "layer_us", "env_us", "env_op_us"):
             v = [r[key] for r in runs]
-            print(f"#   {key:9s} median {statistics.median(v):.1f}  min {min(v):.1f}  max {max(v):.1f}")
+            print(f"#   {key:9s} median {statistics.median(v):.2f}  min {min(v):.2f}  max {max(v):.2f}")
     va, vb = ([r["value"] for r in sides[s][1]] for s in "AB")
     ca, cb = (statistics.median(r["chain_us"] for r in sides[s][1]) for s in "AB")
     print(f"# B / A: value median x{statistics.median(vb) / statistics.median(va):.3f}, min(B) {'>' if min(vb) > max(va) else '<='} max(A); "

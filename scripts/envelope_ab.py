@@ -1,13 +1,23 @@
-"""A/B of the three envelope-TD paths (MORL_ENVELOPE_PATH = v1 | v3 | tc): bit-exact agreement on a sweep of shapes and value
-patterns, then CUDA-event timing at the north-star shape on 16 rotating input sets (> L2).  Development aid, not the bench."""
+"""A/B of the envelope-TD kernel families (MORL_ENVELOPE_PATH = v1 | v3 | wp): bit-exact agreement of v3 and wp with v1 on a sweep of
+shapes and value patterns, then CUDA-event timing on 16 rotating input sets (> L2): v3 at |W| = 16, wp at |W| = 64 (north star), 128
+and 256 (several blocks of 64 weights).  Development aid, not the bench.
+
+    python scripts/envelope_ab.py [LIB]
+
+LIB: the libmorl_b200.so to load (default: the in-tree build), so that two builds can be timed one after the other in one call."""
 import os
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import numpy as np
 import torch as th
 
+from morl_baselines_b200 import _lib
+
+if len(sys.argv) > 1:
+    _lib.LIB_PATH = os.path.abspath(sys.argv[1])
 from morl_baselines_b200 import ops
+
+print(f"# library: {_lib.LIB_PATH}", flush=True)
 
 dev = th.device("cuda:0")
 
@@ -62,7 +72,7 @@ def same(a, b):
 
 bad = 0
 shapes = [(1024, 64, 8, 3), (256, 32, 6, 3), (64, 8, 8, 3), (96, 16, 4, 2), (128, 16, 8, 3), (33, 50, 8, 3), (7, 64, 8, 1), (300, 2, 8, 3),
-          (17, 64, 4, 2), (5, 16, 1, 3), (1, 64, 8, 3), (600, 62, 8, 3)]
+          (17, 64, 4, 2), (5, 16, 1, 3), (1, 64, 8, 3), (600, 62, 8, 3), (64, 128, 8, 3), (16, 256, 8, 3), (9, 96, 4, 4)]
 for shape in shapes:
     for kind in ["plain", "ties", "neartie", "signed", "special"]:
         for mode in (ops.DOT_UNFUSED, ops.DOT_FMA, ops.DOT_PAIRFMA):
@@ -71,7 +81,7 @@ for shape in shapes:
                     continue
                 inp = make(*shape, kind, seed=sum(shape) + len(kind))
                 ref = run("v1", *inp, 0.99, mode, order)
-                for path in (["tc", "wp"] if shape[1] > 32 else ["tc"]):
+                for path in (["v3", "wp"] if shape[1] > 32 else ["v3"]):
                     got = run(path, *inp, 0.99, mode, order)
                     th.cuda.synchronize()
                     ok = all(same(r, g) for r, g in zip(ref, got))
@@ -83,7 +93,7 @@ for shape in shapes:
                         print(f"MISMATCH path={path} shape={shape} kind={kind} mode={mode} order={order}: target rows {nt}, pref {np_}, act {na} of {ref[1].numel()}", flush=True)
 print("agreement sweep:", "OK" if bad == 0 else f"{bad} FAILED", flush=True)
 
-# ---- timing at the north-star shape ----
+# ---- timing ----
 # 16 rotating input sets (> L2).  Two clocks: a python launch loop (includes the host's per-call cost: ctypes + checks, which can
 # exceed the kernel) and a CUDA-graph replay of the same 16 launches (back-to-back GPU time, what the update's graph sees).
 def timed(path, B, W, A, D, sets, out):
@@ -121,11 +131,12 @@ def timed(path, B, W, A, D, sets, out):
     return t_loop, e0.elapsed_time(e1) * 1e-3 / 400
 
 
-for (B, W, A, D) in [(1024, 64, 8, 3), (132, 64, 8, 3), (2048, 64, 8, 3)]:
+for (B, W, A, D), paths in [((1024, 16, 8, 3), ["v3", "v3"]), ((1024, 64, 8, 3), ["v3", "wp", "v3", "wp"]), ((132, 64, 8, 3), ["wp", "wp"]),
+                            ((2048, 64, 8, 3), ["wp", "wp"]), ((512, 128, 8, 3), ["wp", "wp"]), ((256, 256, 8, 3), ["wp", "wp"])]:
     sets = [make(B, W, A, D, "plain", 100 + i) for i in range(16)]
     out = th.empty(W * B, D, device=dev)
     alg = 2 * B * W * A * D * 4 + W * D * 4 + B * D * 4 + B * 4 + W * B * D * 4
-    for path in ["v3", "wp", "tc", "v3", "wp"]:
+    for path in paths:
         t_loop, t_graph = timed(path, B, W, A, D, sets, out)
-        print(f"B={B} path {path}: python loop {t_loop * 1e6:.2f} us/launch, graph replay {t_graph * 1e6:.2f} us/launch = {alg / t_graph / 1e9:.0f} GB/s algorithmic",
-              flush=True)
+        print(f"B={B} W={W} path {path}: python loop {t_loop * 1e6:.2f} us/launch, graph replay {t_graph * 1e6:.2f} us/launch = "
+              f"{alg / t_graph / 1e9:.0f} GB/s algorithmic", flush=True)

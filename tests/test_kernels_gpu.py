@@ -143,11 +143,13 @@ def _env_path(path, *a, **k):
         os.environ.pop("MORL_ENVELOPE_PATH", None)
 
 
-@pytest.mark.parametrize("shape", [(1024, 64, 8, 3), (256, 32, 6, 3), (96, 16, 4, 2), (33, 50, 8, 3), (7, 64, 8, 1), (300, 2, 8, 3), (600, 62, 8, 3)])
+@pytest.mark.parametrize("shape", [(1024, 64, 8, 3), (256, 32, 6, 3), (96, 16, 4, 2), (33, 50, 8, 3), (7, 64, 8, 1), (300, 2, 8, 3), (600, 62, 8, 3),
+                                   (64, 128, 8, 3), (16, 256, 8, 3), (9, 96, 4, 4)])
 @pytest.mark.parametrize("kind", ["plain", "ties", "neartie", "signed", "special"])
 def test_envelope_td_kernel_families_agree_bitwise(cuda, shape, kind):
     """The kernel families of morl_envelope_td_f32 -- generic (v1), CUDA-core fast paths (v3: FMA-chain filter + exact re-check; wp: its
-    weight-pair re-blocking, the default at |W| > 32) -- return bit-identical targets and indices, in every
+    weight-pair re-blocking, the default at |W| > 32; |W| 96, 128 and 256 run it with several blocks of 64 weights) -- return
+    bit-identical targets and indices, in every
     arithmetic mode and row order, on continuous data, exact ties, candidates a few ulps apart, mixed-sign weights / large values,
     and NaN / +-inf / all-zero / huge / tiny blocks.  v1 is pinned to the oracle and the reference's golden vectors above."""
     from morl_baselines_b200 import ops
