@@ -330,6 +330,24 @@ MORL_API int morl_gemm_planes_f32(int fmt, const void* a_planes, long long a_pla
                                   int relu, const void* relu_mask_plane0, int ld_mask, float* c_f32, int ldc, void* c_planes, int ldp,
                                   long long c_plane_stride, const float* c_scale, int reverse_tiles, int split_accumulators,
                                   const void* relu_bits_in, void* relu_bits_out, void* stream);
+/* Hidden layer Linear -> Dropout(p) -> LayerNorm -> ReLU of GPI-PD's Q-network (reference gpi_pd.py:41-76, networks.py:10-48) as ONE
+ * K-major GEMM whose epilogue computes, per output row,  y = relu(LN(dropout(A . B^T / (a_scale b_scale) + bias)))  (csrc/gemm_planes.cu,
+ * gemm_planes_kernel<FMT, 0, kEpiLn>).  Operands, scales, reverse_tiles, c_f32 / c_planes as in morl_gemm_planes_f32 with N_pad = N; the
+ * re-split planes hold c_scale * y (c_scale applied after the ReLU: LayerNorm is not scale-invariant through eps).  N % 32 == 0, N <= 256.
+ *   layer_norm != 0: two-pass fp32 mean and biased variance over the N columns of the row, (x - mean) rsqrt(var + ln_eps) gamma + beta;
+ *                    ln_gamma / ln_beta [N] device vectors (NULL = 1 / 0).
+ *   dropout (drop_seed != NULL): keep element (row, col) iff its Philox4x32-10 draw is >= round(drop_p 2^32), kept values times
+ *                    float(1 / (1 - drop_p)); key = *drop_seed, counter = (*drop_offset, drop_salt, row, column group).  Seed and offset are
+ *                    device-resident: advance the offset with morl_philox_advance inside the same stream (or captured graph) for fresh masks.
+ *   drop_bits_out (nullable, 16-byte aligned): the keep mask as bits in the ReLU-bit layout ([M][8] uint32; bit set = kept).
+ * With layer_norm = 0 and no dropout the outputs equal morl_gemm_planes_f32(relu = 1, split_accumulators = 0) bit for bit. */
+MORL_API int morl_gemm_planes_ln_f32(int fmt, const void* a_planes, long long a_plane_stride, const float* a_scale, const void* b_planes,
+                                     long long b_plane_stride, const float* b_scale, int M, int N, int K, const float* bias, int layer_norm,
+                                     const float* ln_gamma, const float* ln_beta, float ln_eps, float drop_p, const unsigned long long* drop_seed,
+                                     const unsigned int* drop_offset, unsigned int drop_salt, float* c_f32, int ldc, void* c_planes, int ldp,
+                                     long long c_plane_stride, const float* c_scale, int reverse_tiles, void* drop_bits_out, void* stream);
+/* *offset += inc as one stream-ordered launch (the dropout pass counter of morl_gemm_planes_ln_f32; capture-safe). */
+MORL_API int morl_philox_advance(unsigned int* offset, unsigned int inc, void* stream);
 /* Several 256-wide hidden layers (Linear + ReLU) of one or two networks in ONE persistent launch (csrc/gemm_planes.cu: gemm_chain_kernel):
  * job (c, l):  act[c][l+1] = f(act[c][l] . W[c][l]^T + bias[c][l]),  planes in / planes out at the scale `act_scale`; f = ReLU (relu != 0:
  * forward chains, optionally recording the ReLU bit masks) or the ReLU-backward mask relu_bits_in[job] (dX chains of the backward pass:
@@ -395,6 +413,10 @@ MORL_API int morl_qhead_envelope_td_f32(int fmt, const void* a_on_planes, const 
 MORL_API int morl_pairs_relu_split_planes(int fmt, const float* u, const float* v, int B, int W, int H, void* dst_planes,
                                           long long plane_stride, const float* scale, void* relu_bits_out, void* stream);
 
+/* Product-conditioned first layer of GPI-PD's Q-network (reference gpi_pd.py:62-65, sf * wf):  h[b*P + p, :] = u[b, :] * v[p, :] (one fp32
+ * multiply) written directly as planes [P_fmt][B*P][H] of scale * h.  u, v, dst 16-byte aligned, H % 8 == 0. */
+MORL_API int morl_pairs_product_split_planes(int fmt, const float* u, const float* v, int B, int P, int H, void* dst_planes,
+                                             long long plane_stride, const float* scale, void* stream);
 
 /* Weight-gradient GEMM (reduction over the batch rows), split-K, deterministic:
  *   out[n, k] = sum_m G[m, n] * H[m, k]      G planes [P][M][ldg] (n < g_cols, scaled by *g_scale), H planes [P][M][ldh] (k < h_cols,
@@ -420,6 +442,11 @@ MORL_API int morl_pairs_grad_reduce_planes(int fmt, const void* planes, long lon
  * sgemms and their epilogue kernels).  W1 is the row-major nn.Linear weight [H, F + D]; u [B, H], v [W, H]. */
 MORL_API int morl_pair_layer1_uv_f32(const float* feats, const float* wset, const float* W1, const float* b1, int B, int W, int F, int D, int H,
                                      float* u, float* v, void* stream);
+
+/* The two feature maps of GPI-PD's Q-network in ONE launch:  u = relu(s . Ls^T + bs) [B, H] (state_features on the B observations s [B, F])
+ * and v = relu(m . Lw^T + bw) [P, H] (weights_features on the P weight vectors m [P, D]); Ls [H, F], Lw [H, D] row-major nn.Linear weights. */
+MORL_API int morl_product_layer1_uv_f32(const float* s, const float* Ls, const float* bs, int B, int F, const float* m, const float* Lw, const float* bw,
+                                        int P, int D, int H, float* u, float* v, void* stream);
 
 /* Parameter gradients of the separable first layer (backward of morl_pair_layer1_uv_f32; autograd of nn.Linear at envelope.py:316 on the
  * effective batch, restricted to layer 1):  dW1 [H, F + D] = [dU^T feats | dV^T wset],  db1 [H] = colsum(dV), with dU [B, H] / dV [W, H]

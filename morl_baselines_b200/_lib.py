@@ -57,6 +57,9 @@ SIGNATURES = {
     "morl_split_planes": (_i, [_i, _vp, _i, _i, _i, _i, _vp, _i, _i, C.c_longlong, _vp, _vp]),
     "morl_gemm_planes_f32": (_i, [_i, _vp, C.c_longlong, _vp, _vp, C.c_longlong, _vp, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _i, C.c_longlong,
                                   _vp, _i, _i, _vp, _vp, _vp]),
+    "morl_gemm_planes_ln_f32": (_i, [_i, _vp, C.c_longlong, _vp, _vp, C.c_longlong, _vp, _i, _i, _i, _vp, _i, _vp, _vp, _f, _f, _vp, _vp, C.c_uint,
+                                     _vp, _i, _vp, _i, C.c_longlong, _vp, _i, _vp, _vp]),
+    "morl_philox_advance": (_i, [_vp, C.c_uint, _vp]),
     "morl_gemm_chain_supported": (_i, [_i, _i, _i]),
     "morl_gemm_chain_f32": (_i, [_i, _i, _i, _vp, C.c_longlong, _vp, _vp, C.c_longlong, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp]),
     "morl_debug_gemm_stats": (_i, [_vp, _i]),
@@ -67,11 +70,13 @@ SIGNATURES = {
     "morl_qhead_envelope_td_f32": (_i, [_i, _vp, _vp, C.c_longlong, _vp, _vp, _vp, _vp, C.c_longlong, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _f, _i, _i,
                                         _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "morl_pairs_relu_split_planes": (_i, [_i, _vp, _vp, _i, _i, _i, _vp, C.c_longlong, _vp, _vp, _vp]),
+    "morl_pairs_product_split_planes": (_i, [_i, _vp, _vp, _i, _i, _i, _vp, C.c_longlong, _vp, _vp]),
     "morl_gemm_mn_workspace_bytes": (_sz, [_i, _i, _i]),
     "morl_gemm_planes_mn_f32": (_i, [_i, _vp, C.c_longlong, _i, _i, _vp, _vp, C.c_longlong, _i, _i, _vp, _i, _i, _vp, _i, _vp, _vp, _vp]),
     "morl_colsum_planes": (_i, [_i, _vp, C.c_longlong, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "morl_pairs_grad_reduce_planes": (_i, [_i, _vp, C.c_longlong, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "morl_pair_layer1_uv_f32": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "morl_product_layer1_uv_f32": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "morl_pair_layer1_grad_workspace_bytes": (_sz, [_i, _i, _i]),
     "morl_pair_layer1_grad_f32": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "morl_adam_workspace_bytes": (_sz, [_i, _i64]),

@@ -85,7 +85,37 @@ struct GemmArgs {
     int reverse;                 // walk the row tiles from the last to the first (see morl_gemm_planes_f32: L2 reuse between chained layers)
     unsigned long long* stats;   // diagnostics (MORL_GEMM_STATS=1), else nullptr: [0] consumer wait-on-TMA cycles, [1] consumer loop total,
                                  // [2] producer wait-on-free-stage, [3] epilogue busy
+    // LayerNorm / dropout epilogue (EPI == kEpiLn only; appended so that the fields above keep their parameter offsets)
+    int ln;                      // LayerNorm over the N output columns of a row
+    float ln_eps;
+    const float* ln_gamma;       // [N] or nullptr = 1
+    const float* ln_beta;        // [N] or nullptr = 0
+    const unsigned long long* drop_seed;  // device Philox key, or nullptr = no dropout
+    const unsigned int* drop_offset;      // device pass counter (Philox counter word 0)
+    unsigned int drop_salt;      // layer salt (counter word 1)
+    unsigned int drop_thr;       // keep iff draw >= drop_thr = round(p 2^32)
+    float drop_scale;            // float(1 / (1 - p))
+    uint32_t* drop_bits;         // keep mask [M][relu_bits_words(N)] in the ReLU-bit layout, or nullptr
 };
+
+constexpr int kEpiPlain = 0;     // x k_acc + bias [, ReLU / ReLU mask]
+constexpr int kEpiLn = 1;        // relu(LN(dropout(x k_acc + bias))) c_scale
+
+// Philox4x32-10 (Salmon et al., SC'11): four 32-bit draws per (counter, key)
+__device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1, uint32_t (&r)[4]) {
+#pragma unroll
+    for (int i = 0; i < 10; ++i) {
+        const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
+        const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
+        c0 = hi1 ^ c1 ^ k0;
+        c1 = lo1;
+        c2 = hi0 ^ c3 ^ k1;
+        c3 = lo0;
+        k0 += 0x9E3779B9u;
+        k1 += 0xBB67AE85u;
+    }
+    r[0] = c0; r[1] = c1; r[2] = c2; r[3] = c3;
+}
 
 __device__ unsigned long long g_gemm_stats[8];
 
@@ -177,7 +207,8 @@ struct EpiArgs {
 // Epilogue of one 32-column chunk of a consumer warp's 16 accumulator rows [rbase, rbase + 16): thread l holds a[4 q + 2 h + e] = column
 // col0 + 8 q + 2 (l % 4) + e of row rbase + l / 4 + 8 h (the wgmma fragment).  The re-split planes leave through the warp's two staging tiles in
 // turn (n_stored counts the warp's bulk stores): a chunk is staged while the TMA store of the previous one is still reading the other tile.
-template <int FMT>
+// PRE: a[] already holds the pre-activation (the LayerNorm epilogue has applied scale, bias, dropout and LayerNorm).
+template <int FMT, bool PRE = false>
 __device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, int rbase, int lane, const EpiArgs& e, const CUtensorMap* tmC,
                                                uint8_t* my_stage, uint32_t& n_stored, float& amax) {
     using F = PlaneFmt<FMT>;
@@ -192,7 +223,9 @@ __device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, i
         for (int q = 0; q < 4; ++q)
 #pragma unroll
             for (int c = 0; c < 2; ++c) {
-                float f = __fmaf_rn(a[4 * q + 2 * h + c], e.k_acc, e.bias_s[col0 + 8 * q + 2 * l4 + c]);
+                float f;
+                if constexpr (PRE) f = a[4 * q + 2 * h + c];
+                else f = __fmaf_rn(a[4 * q + 2 * h + c], e.k_acc, e.bias_s[col0 + 8 * q + 2 * l4 + c]);
                 if (e.relu) f = (f < 0.f) ? 0.f : f;  // (NaN stays NaN, like torch.relu: an overflow upstream must reach the loss)
                 x[h][2 * q + c] = f;
             }
@@ -286,10 +319,90 @@ __device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, i
     }
 }
 
+// LayerNorm / dropout epilogue, in place on a consumer warp's accumulators (one column unit holds all N <= 256 columns of its 64 rows;
+// thread l holds rows rbase + l / 4 and rbase + l / 4 + 8, acc[16 c + 4 q + 2 h + e] = column 32 c + 8 q + 2 (l % 4) + e of row h):
+//   x = acc k_acc + bias;  dropout: x = keep ? x drop_scale : 0 with keep = draw >= drop_thr;  LayerNorm: (x - mean) rstd gamma + beta
+// with the two-pass fp32 mean and biased variance of the row (per-thread partial sums + two quad shuffles), rstd = rsqrt(var + eps).
+// Draws: Philox4x32-10, key = seed, counter = (*drop_offset, drop_salt, row, g) with column group g = 8 c + 2 (l % 4) + k; draw i of group
+// g is column 32 c + 8 (2 k + i / 2) + 2 (l % 4) + i % 2.  Each draw is made once and applied in place, before the statistics.
+__device__ __forceinline__ void ln_dropout_unit(float (&acc)[128], int N, int rbase, int lane, const float* bias_s, float k_acc, const GemmArgs& g,
+                                                uint32_t k0, uint32_t k1, uint32_t ctr0) {
+    const int l4 = lane & 3, lr = lane >> 2;
+    const bool drop = g.drop_seed != nullptr;
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+        if (32 * c < N) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = rbase + lr + 8 * h;
+                uint32_t kept = 0;
+#pragma unroll
+                for (int k = 0; k < 2; ++k) {
+                    uint32_t r[4] = {0u, 0u, 0u, 0u};
+                    if (drop) philox4x32_10(ctr0, g.drop_salt, (uint32_t)row, (uint32_t)(8 * c + 2 * l4 + k), k0, k1, r);
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        const int q = 2 * k + (i >> 1), e = i & 1;
+                        const int j = 16 * c + 4 * q + 2 * h + e;
+                        float x = __fmaf_rn(acc[j], k_acc, bias_s[32 * c + 8 * q + 2 * l4 + e]);
+                        if (drop) {
+                            const bool keep = r[i] >= g.drop_thr;
+                            x = keep ? __fmul_rn(x, g.drop_scale) : 0.f;
+                            kept |= (keep ? 1u : 0u) << (8 * q + 2 * l4 + e);
+                        }
+                        acc[j] = x;
+                    }
+                }
+                if (g.drop_bits) {
+                    kept |= __shfl_xor_sync(0xffffffffu, kept, 1);
+                    kept |= __shfl_xor_sync(0xffffffffu, kept, 2);
+                    if (l4 == 0 && row < g.M) g.drop_bits[(size_t)row * relu_bits_words(N) + relu_bits_word(32 * c)] = kept;
+                }
+            }
+        }
+    }
+    if (!g.ln) return;
+    const float inv_n = 1.0f / (float)N;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        float s = 0.f;
+#pragma unroll
+        for (int c = 0; c < 8; ++c)
+            if (32 * c < N)
+#pragma unroll
+                for (int t = 0; t < 8; ++t) s = __fadd_rn(s, acc[16 * c + 4 * (t >> 1) + 2 * h + (t & 1)]);
+        s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, 1));
+        s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, 2));
+        const float mean = __fmul_rn(s, inv_n);
+        float v = 0.f;
+#pragma unroll
+        for (int c = 0; c < 8; ++c)
+            if (32 * c < N)
+#pragma unroll
+                for (int t = 0; t < 8; ++t) {
+                    const float d = __fsub_rn(acc[16 * c + 4 * (t >> 1) + 2 * h + (t & 1)], mean);
+                    v = __fmaf_rn(d, d, v);
+                }
+        v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 1));
+        v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 2));
+        const float rstd = rsqrtf(__fadd_rn(__fmul_rn(v, inv_n), g.ln_eps));
+#pragma unroll
+        for (int c = 0; c < 8; ++c)
+            if (32 * c < N)
+#pragma unroll
+                for (int t = 0; t < 8; ++t) {
+                    const int col = 32 * c + 8 * (t >> 1) + 2 * l4 + (t & 1);
+                    const int j = 16 * c + 4 * (t >> 1) + 2 * h + (t & 1);
+                    const float gm = g.ln_gamma ? __ldg(g.ln_gamma + col) : 1.0f, bt = g.ln_beta ? __ldg(g.ln_beta + col) : 0.0f;
+                    acc[j] = __fmaf_rn(__fmul_rn(__fsub_rn(acc[j], mean), rstd), gm, bt);
+                }
+    }
+}
+
 // One CTA per 128-row tile.  SPLIT = 1: see mma_unit; a tile wider than 128 columns is then computed as column units of 128 (the A boxes of
 // the tile are staged once per unit).  SPLIT = 0 and N_pad > 256: two column units [0, 256) and [256, N_pad), each with the stage plan of
-// N_pad = 256 and this unit's 256 biases in shared memory.
-template <int FMT, int SPLIT>
+// N_pad = 256 and this unit's 256 biases in shared memory.  EPI = kEpiLn (SPLIT = 0, N = N_pad <= 256): ln_dropout_unit before the chunks.
+template <int FMT, int SPLIT, int EPI = kEpiPlain>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC,
                    const GemmArgs g) {
@@ -393,7 +506,8 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         // x = acc / (sA sB) + bias; when only planes are written (the hidden layers) the output scale is FOLDED into the two constants:
         // fold * x = acc * (fold / (sA sB)) + fold * bias (exact, powers of two), and max / mask commute with a positive factor
         const float c_mul = ld_scale(g.c_scale);
-        const bool folded = g.c_f32 == nullptr;
+        // (LayerNorm is not scale-invariant through eps: its output scale is applied after the ReLU instead)
+        const bool folded = EPI == kEpiPlain && g.c_f32 == nullptr;
         const float fold = folded ? c_mul : 1.0f;
         if (warp == 0 && folded)  // (bias_s was filled before the CTA barrier; one warp rescales it)
             for (int t = lane; t < 256; t += 32) bias_s[t] *= fold;
@@ -404,6 +518,15 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         e.c_mul = folded ? 1.0f : c_mul;
         e.bias_s = bias_s; e.relu = g.relu; e.bits_in = g.bits_in; e.bits_out = g.bits_out; e.bits_ld = g.bits_ld; e.mask = g.mask;
         e.ld_mask = g.ld_mask; e.c_f32 = g.c_f32; e.ldc = g.ldc; e.planes = g.c_planes != nullptr; e.ldp = g.ldp;
+        uint32_t key0 = 0, key1 = 0, ctr0 = 0;
+        if constexpr (EPI == kEpiLn) {
+            if (g.drop_seed) {
+                const unsigned long long seed = *g.drop_seed;
+                key0 = (uint32_t)seed;
+                key1 = (uint32_t)(seed >> 32);
+                ctr0 = *g.drop_offset;
+            }
+        }
         float amax = 0.f;
         float acc[128];
         uint32_t stage = 0, phase = 0;
@@ -439,13 +562,14 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
                 e.bias_s = bias_s - n_begin;
             }
             const int rbase = tile * kGemmBM + wg * 64 + (warp & 3) * 16;
+            if constexpr (EPI == kEpiLn) ln_dropout_unit(acc, n_cnt, rbase, lane, bias_s, e.k_acc, g, key0, key1, ctr0);
 #pragma unroll
             for (int c = 0; c < (SPLIT ? 4 : 8); ++c) {
                 if (32 * c < n_cnt) {
                     float a[16];
 #pragma unroll
                     for (int j = 0; j < 16; ++j) a[j] = SPLIT ? __fadd_rn(acc[16 * c + j], acc[64 + 16 * c + j]) : acc[16 * c + j];
-                    epilogue_chunk<FMT>(a, n_begin + 32 * c, rbase, lane, e, &tmC, my_stage, n_stored, amax);
+                    epilogue_chunk<FMT, EPI == kEpiLn>(a, n_begin + 32 * c, rbase, lane, e, &tmC, my_stage, n_stored, amax);
                 }
             }
             if (g.stats) busy += clock64() - c1;
@@ -1250,7 +1374,8 @@ __global__ void __launch_bounds__(256) split_planes_multi_kernel(const __grid_co
 }
 
 // ---- separable first layer: h[b*W + j] = relu(u[b] + v[j]) straight into planes ------------------------------------------------
-template <int FMT>
+// PRODUCT: the product-conditioned first layer h[b*W + j] = u[b] * v[j] (one fp32 multiply, no activation: u and v are ReLU outputs)
+template <int FMT, bool PRODUCT = false>
 __global__ void __launch_bounds__(256) pairs_relu_split_kernel(const float* __restrict__ u, const float* __restrict__ v, int B, int W, int H,
                                                                uint16_t* __restrict__ dst, long long plane_stride, const float* __restrict__ scale,
                                                                uint32_t* __restrict__ bits_out) {
@@ -1272,13 +1397,24 @@ __global__ void __launch_bounds__(256) pairs_relu_split_kernel(const float* __re
         const float4* up = reinterpret_cast<const float4*>(u + (size_t)b * H + 8 * h8);
         const float4* vp = reinterpret_cast<const float4*>(v + (size_t)j * H + 8 * h8);
         const float4 u0 = __ldg(up), u1 = __ldg(up + 1), v0 = __ldg(vp), v1 = __ldg(vp + 1);
-        const float x[8] = {u0.x + v0.x, u0.y + v0.y, u0.z + v0.z, u0.w + v0.w, u1.x + v1.x, u1.y + v1.y, u1.z + v1.z, u1.w + v1.w};
+        float x[8];
+        if constexpr (PRODUCT) {
+            x[0] = __fmul_rn(u0.x, v0.x); x[1] = __fmul_rn(u0.y, v0.y); x[2] = __fmul_rn(u0.z, v0.z); x[3] = __fmul_rn(u0.w, v0.w);
+            x[4] = __fmul_rn(u1.x, v1.x); x[5] = __fmul_rn(u1.y, v1.y); x[6] = __fmul_rn(u1.z, v1.z); x[7] = __fmul_rn(u1.w, v1.w);
+        } else {
+            x[0] = u0.x + v0.x; x[1] = u0.y + v0.y; x[2] = u0.z + v0.z; x[3] = u0.w + v0.w;
+            x[4] = u1.x + v1.x; x[5] = u1.y + v1.y; x[6] = u1.z + v1.z; x[7] = u1.w + v1.w;
+        }
         uint32_t o[F::P][4];
         uint32_t pos = 0;  // bit t = (column 8 h8 + t is positive)
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
             uint32_t w[F::P];
-            const float r0 = x[2 * q] < 0.f ? 0.f : x[2 * q], r1 = x[2 * q + 1] < 0.f ? 0.f : x[2 * q + 1];  // NaN-propagating ReLU
+            float r0 = x[2 * q], r1 = x[2 * q + 1];
+            if constexpr (!PRODUCT) {
+                r0 = r0 < 0.f ? 0.f : r0;  // NaN-propagating ReLU
+                r1 = r1 < 0.f ? 0.f : r1;
+            }
             pos |= (r0 > 0.f ? 1u : 0u) << (2 * q) | (r1 > 0.f ? 1u : 0u) << (2 * q + 1);
             F::split2(r0 * s, r1 * s, w, amax);
 #pragma unroll
@@ -1627,6 +1763,22 @@ extern "C" int morl_pairs_relu_split_planes(int fmt, const float* u, const float
     return check_launch("morl_pairs_relu_split_planes");
 }
 
+extern "C" int morl_pairs_product_split_planes(int fmt, const float* u, const float* v, int B, int P, int H, void* dst_planes, long long plane_stride,
+                                               const float* scale, void* stream) {
+    using namespace morl;
+    MORL_REQUIRE(fmt_ok(fmt), MORL_ERR_UNSUPPORTED, "morl_pairs_product_split_planes: unknown plane format %d", fmt);
+    MORL_REQUIRE(u && v && dst_planes, MORL_ERR_NULL, "morl_pairs_product_split_planes: NULL pointer argument");
+    MORL_REQUIRE(B > 0 && P > 0 && H > 0 && H % 8 == 0 && plane_stride % 8 == 0 && plane_stride >= (long long)B * P * H, MORL_ERR_SHAPE,
+                 "morl_pairs_product_split_planes: bad shape B=%d P=%d H=%d", B, P, H);
+    MORL_REQUIRE(aligned16(u) && aligned16(v) && aligned16(dst_planes), MORL_ERR_ALIGN, "morl_pairs_product_split_planes: operands must be 16-byte aligned");
+    const long long total = (long long)B * P * (H / 8);
+    long long blocks = (total + 255) / 256;
+    if (blocks > 132 * 16) blocks = 132 * 16;
+    MORL_DISPATCH_FMT(fmt, (launch_k(pairs_relu_split_kernel<kFmt, true>, dim3((int)blocks), dim3(256), 0, static_cast<cudaStream_t>(stream),
+                                     u, v, B, P, H, static_cast<uint16_t*>(dst_planes), plane_stride, scale, static_cast<uint32_t*>(nullptr))));
+    return check_launch("morl_pairs_product_split_planes");
+}
+
 // Diagnostics: cycle counters of the K-major GEMM roles, accumulated over all CTAs and launches since the last reset
 // (only when MORL_GEMM_STATS=1 was set before the first GEMM call).
 extern "C" int morl_debug_gemm_stats(unsigned long long* out8, int reset) {
@@ -1642,12 +1794,12 @@ extern "C" int morl_debug_gemm_stats(unsigned long long* out8, int reset) {
 }
 
 namespace morl {
-template <int FMT, int SPLIT>
+template <int FMT, int SPLIT, int EPI = kEpiPlain>
 static int launch_gemm_planes(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmArgs& g, int sms, cudaStream_t st) {
     constexpr size_t smem = KPlan<FMT>::kBytes;
     static bool attr_set = false;
     if (!attr_set) {
-        cudaFuncSetAttribute(gemm_planes_kernel<FMT, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaFuncSetAttribute(gemm_planes_kernel<FMT, SPLIT, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         attr_set = true;
     }
     constexpr int kUnitN = SPLIT ? 128 : 256;  // column units per tile: as gemm_planes_kernel
@@ -1663,42 +1815,53 @@ static int launch_gemm_planes(const CUtensorMap& tmA, const CUtensorMap& tmB, co
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = g.pdl ? 1 : 0;
-    cudaLaunchKernelEx(&cfg, gemm_planes_kernel<FMT, SPLIT>, tmA, tmB, tmC, g);
-    return check_launch("morl_gemm_planes_f32");
+    cudaLaunchKernelEx(&cfg, gemm_planes_kernel<FMT, SPLIT, EPI>, tmA, tmB, tmC, g);
+    return check_launch(EPI == kEpiLn ? "morl_gemm_planes_ln_f32" : "morl_gemm_planes_f32");
 }
-}  // namespace morl
 
-extern "C" int morl_gemm_planes_f32(int fmt, const void* a_planes, long long a_plane_stride, const float* a_scale, const void* b_planes,
-                                    long long b_plane_stride, const float* b_scale, int M, int N, int N_pad, int K, const float* bias, int relu,
-                                    const void* relu_mask_plane0, int ld_mask, float* c_f32, int ldc, void* c_planes, int ldp, long long c_plane_stride,
-                                    const float* c_scale, int reverse_tiles, int split_accumulators, const void* relu_bits_in, void* relu_bits_out,
-                                    void* stream) {
-    using namespace morl;
-    MORL_REQUIRE(fmt_ok(fmt), MORL_ERR_UNSUPPORTED, "morl_gemm_planes_f32: unknown plane format %d", fmt);
-    MORL_REQUIRE(a_planes && b_planes && (c_f32 || c_planes), MORL_ERR_NULL, "morl_gemm_planes_f32: NULL pointer argument");
-    MORL_REQUIRE(M > 0 && N > 0 && K > 0 && N_pad >= N, MORL_ERR_SHAPE, "morl_gemm_planes_f32: bad shape M=%d N=%d N_pad=%d K=%d", M, N, N_pad, K);
+// the LayerNorm / dropout part of a morl_gemm_planes_ln_f32 call (nullptr: morl_gemm_planes_f32)
+struct LnDropArgs {
+    int ln;
+    float eps;
+    const float *gamma, *beta;
+    const unsigned long long* seed;
+    const unsigned int* offset;
+    unsigned int salt, thr;
+    float scale;
+    void* bits;
+};
+
+static int gemm_planes_impl(int fmt, const void* a_planes, long long a_plane_stride, const float* a_scale, const void* b_planes,
+                            long long b_plane_stride, const float* b_scale, int M, int N, int N_pad, int K, const float* bias, int relu,
+                            const void* relu_mask_plane0, int ld_mask, float* c_f32, int ldc, void* c_planes, int ldp, long long c_plane_stride,
+                            const float* c_scale, int reverse_tiles, int split_accumulators, const void* relu_bits_in, void* relu_bits_out,
+                            const LnDropArgs* lnd, const char* name, void* stream) {
+    MORL_REQUIRE(fmt_ok(fmt), MORL_ERR_UNSUPPORTED, "%s: unknown plane format %d", name, fmt);
+    MORL_REQUIRE(a_planes && b_planes && (c_f32 || c_planes), MORL_ERR_NULL, "%s: NULL pointer argument", name);
+    MORL_REQUIRE(M > 0 && N > 0 && K > 0 && N_pad >= N, MORL_ERR_SHAPE, "%s: bad shape M=%d N=%d N_pad=%d K=%d", name, M, N, N_pad, K);
     const int BK = fmt == MORL_FMT_F16X2 ? PlaneFmt<MORL_FMT_F16X2>::BK : PlaneFmt<MORL_FMT_BF16X3>::BK;
     MORL_REQUIRE(K % BK == 0 && N_pad % 32 == 0 && N_pad <= 512, MORL_ERR_UNSUPPORTED,
-                 "morl_gemm_planes_f32: need K %% %d == 0, N_pad %% 32 == 0, N_pad <= 512 (K=%d N_pad=%d)", BK, K, N_pad);
-    MORL_REQUIRE(aligned16(a_planes) && aligned16(b_planes), MORL_ERR_ALIGN, "morl_gemm_planes_f32: operand planes must be 16-byte aligned");
-    MORL_REQUIRE(aligned16(relu_bits_in) && aligned16(relu_bits_out), MORL_ERR_ALIGN, "morl_gemm_planes_f32: ReLU bit masks must be 16-byte aligned");
+                 "%s: need K %% %d == 0, N_pad %% 32 == 0, N_pad <= 512 (K=%d N_pad=%d)", name, BK, K, N_pad);
+    MORL_REQUIRE(aligned16(a_planes) && aligned16(b_planes), MORL_ERR_ALIGN, "%s: operand planes must be 16-byte aligned", name);
+    MORL_REQUIRE(aligned16(relu_bits_in) && aligned16(relu_bits_out), MORL_ERR_ALIGN, "%s: ReLU bit masks must be 16-byte aligned", name);
     if (c_planes)
         MORL_REQUIRE(ldp % 32 == 0 && ldp >= N && ldp <= N_pad && aligned16(c_planes) && c_plane_stride % 8 == 0, MORL_ERR_SHAPE,
-                     "morl_gemm_planes_f32: ldp=%d must be a multiple of 32 with N <= ldp <= N_pad", ldp);
+                     "%s: ldp=%d must be a multiple of 32 with N <= ldp <= N_pad", name, ldp);
     int sms = morl_device_sm_count();
     if (sms <= 0) sms = 132;
     CUtensorMap tmA, tmB;
     int rc = make_plane_map(&tmA, fmt, a_planes, M, K, a_plane_stride, kGemmBM, BK);
-    MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "morl_gemm_planes_f32: cuTensorMapEncodeTiled(A) failed (%d)", rc);
+    MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "%s: cuTensorMapEncodeTiled(A) failed (%d)", name, rc);
     rc = make_plane_map(&tmB, fmt, b_planes, N_pad, K, b_plane_stride, kGemmBoxN, BK, true);
-    MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "morl_gemm_planes_f32: cuTensorMapEncodeTiled(B) failed (%d)", rc);
+    MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "%s: cuTensorMapEncodeTiled(B) failed (%d)", name, rc);
     CUtensorMap tmC;
     memset(&tmC, 0, sizeof(tmC));
     if (c_planes) {  // store map of the re-split output: [P][M][ldp], box 32 cols x 16 rows x P planes (64-byte swizzle)
         rc = make_plane_map(&tmC, fmt, c_planes, M, ldp, c_plane_stride, 16, 32);
-        MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "morl_gemm_planes_f32: cuTensorMapEncodeTiled(C) failed (%d)", rc);
+        MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "%s: cuTensorMapEncodeTiled(C) failed (%d)", name, rc);
     }
     GemmArgs g;
+    memset(&g, 0, sizeof(g));
     g.M = M; g.N = N; g.N_pad = N_pad; g.K = K;
     g.bias = bias; g.c_f32 = c_f32; g.ldc = ldc;
     g.c_planes = c_planes; g.ldp = ldp; g.plane_stride = c_plane_stride;
@@ -1738,10 +1901,64 @@ extern "C" int morl_gemm_planes_f32(int fmt, const void* a_planes, long long a_p
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     // accumulator mode (see gemm_planes_kernel): per call; MORL_GEMM_SPLIT_ACC=0 / 1 overrides every call (A/B measurements)
     static const int split_env = [] { const char* e = getenv("MORL_GEMM_SPLIT_ACC"); return e ? (e[0] == '0' ? 0 : 1) : -1; }();
+    if (lnd) {
+        g.ln = lnd->ln; g.ln_eps = lnd->eps; g.ln_gamma = lnd->gamma; g.ln_beta = lnd->beta;
+        g.drop_seed = lnd->seed; g.drop_offset = lnd->offset; g.drop_salt = lnd->salt; g.drop_thr = lnd->thr; g.drop_scale = lnd->scale;
+        g.drop_bits = static_cast<uint32_t*>(lnd->bits);
+        return fmt == MORL_FMT_F16X2 ? launch_gemm_planes<MORL_FMT_F16X2, 0, kEpiLn>(tmA, tmB, tmC, g, sms, st)
+                                     : launch_gemm_planes<MORL_FMT_BF16X3, 0, kEpiLn>(tmA, tmB, tmC, g, sms, st);
+    }
     const bool split_acc = split_env >= 0 ? split_env != 0 : split_accumulators != 0;
     if (fmt == MORL_FMT_F16X2)
         return split_acc ? launch_gemm_planes<MORL_FMT_F16X2, 1>(tmA, tmB, tmC, g, sms, st) : launch_gemm_planes<MORL_FMT_F16X2, 0>(tmA, tmB, tmC, g, sms, st);
     return split_acc ? launch_gemm_planes<MORL_FMT_BF16X3, 1>(tmA, tmB, tmC, g, sms, st) : launch_gemm_planes<MORL_FMT_BF16X3, 0>(tmA, tmB, tmC, g, sms, st);
+}
+
+__global__ void philox_advance_kernel(unsigned int* offset, unsigned int inc) {
+    pdl_enter();
+    *offset += inc;
+}
+}  // namespace morl
+
+extern "C" int morl_gemm_planes_f32(int fmt, const void* a_planes, long long a_plane_stride, const float* a_scale, const void* b_planes,
+                                    long long b_plane_stride, const float* b_scale, int M, int N, int N_pad, int K, const float* bias, int relu,
+                                    const void* relu_mask_plane0, int ld_mask, float* c_f32, int ldc, void* c_planes, int ldp, long long c_plane_stride,
+                                    const float* c_scale, int reverse_tiles, int split_accumulators, const void* relu_bits_in, void* relu_bits_out,
+                                    void* stream) {
+    return morl::gemm_planes_impl(fmt, a_planes, a_plane_stride, a_scale, b_planes, b_plane_stride, b_scale, M, N, N_pad, K, bias, relu, relu_mask_plane0,
+                                  ld_mask, c_f32, ldc, c_planes, ldp, c_plane_stride, c_scale, reverse_tiles, split_accumulators, relu_bits_in,
+                                  relu_bits_out, nullptr, "morl_gemm_planes_f32", stream);
+}
+
+extern "C" int morl_gemm_planes_ln_f32(int fmt, const void* a_planes, long long a_plane_stride, const float* a_scale, const void* b_planes,
+                                       long long b_plane_stride, const float* b_scale, int M, int N, int K, const float* bias, int layer_norm,
+                                       const float* ln_gamma, const float* ln_beta, float ln_eps, float drop_p, const unsigned long long* drop_seed,
+                                       const unsigned int* drop_offset, unsigned int drop_salt, float* c_f32, int ldc, void* c_planes, int ldp,
+                                       long long c_plane_stride, const float* c_scale, int reverse_tiles, void* drop_bits_out, void* stream) {
+    using namespace morl;
+    MORL_REQUIRE(fmt_ok(fmt), MORL_ERR_UNSUPPORTED, "morl_gemm_planes_ln_f32: unknown plane format %d", fmt);
+    MORL_REQUIRE(N > 0 && N <= 256 && N % 32 == 0, MORL_ERR_UNSUPPORTED, "morl_gemm_planes_ln_f32: need N %% 32 == 0 and N <= 256 (N=%d)", N);
+    MORL_REQUIRE(!(drop_p < 0.f) && drop_p < 1.f, MORL_ERR_SHAPE, "morl_gemm_planes_ln_f32: dropout probability %g outside [0, 1)", (double)drop_p);
+    MORL_REQUIRE(!layer_norm || ln_eps > 0.f, MORL_ERR_SHAPE, "morl_gemm_planes_ln_f32: LayerNorm eps must be positive (got %g)", (double)ln_eps);
+    MORL_REQUIRE((drop_seed == nullptr) == (drop_offset == nullptr), MORL_ERR_NULL, "morl_gemm_planes_ln_f32: dropout needs both the seed and the offset");
+    MORL_REQUIRE(drop_seed || !drop_bits_out, MORL_ERR_NULL, "morl_gemm_planes_ln_f32: a keep mask needs dropout (seed and offset)");
+    MORL_REQUIRE(aligned16(drop_bits_out), MORL_ERR_ALIGN, "morl_gemm_planes_ln_f32: the keep mask must be 16-byte aligned");
+    LnDropArgs a;
+    a.ln = layer_norm ? 1 : 0; a.eps = ln_eps; a.gamma = ln_gamma; a.beta = ln_beta;
+    a.seed = drop_seed; a.offset = drop_offset; a.salt = drop_salt;
+    const double t = rint((double)drop_p * 4294967296.0);  // keep iff draw >= round(p 2^32); p < 1 keeps it below 2^32
+    a.thr = t >= 4294967295.0 ? 4294967295u : (unsigned int)t;
+    a.scale = (float)(1.0 / (1.0 - (double)drop_p));
+    a.bits = drop_bits_out;
+    return gemm_planes_impl(fmt, a_planes, a_plane_stride, a_scale, b_planes, b_plane_stride, b_scale, M, N, N, K, bias, 1, nullptr, 0, c_f32, ldc,
+                            c_planes, ldp, c_plane_stride, c_scale, reverse_tiles, 0, nullptr, nullptr, &a, "morl_gemm_planes_ln_f32", stream);
+}
+
+extern "C" int morl_philox_advance(unsigned int* offset, unsigned int inc, void* stream) {
+    using namespace morl;
+    MORL_REQUIRE(offset, MORL_ERR_NULL, "morl_philox_advance: NULL pointer argument");
+    launch_k(philox_advance_kernel, dim3(1), dim3(1), 0, static_cast<cudaStream_t>(stream), offset, inc);
+    return check_launch("morl_philox_advance");
 }
 
 

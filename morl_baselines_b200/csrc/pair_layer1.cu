@@ -75,6 +75,60 @@ __global__ void __launch_bounds__(256) pair_layer1_uv_kernel(const float* __rest
     }
 }
 
+// ---- product-conditioned first layer (GPI-PD's QNet): u = relu(s Ls^T + bs) on the B observations, v = relu(m Lw^T + bw) on the P weight
+// vectors, in one launch; grid.x = ceil((B + P) / kL1Rows), rows < B are observations.  Ls [H, F], Lw [H, D] row-major (nn.Linear).
+__global__ void __launch_bounds__(256) product_layer1_uv_kernel(const float* __restrict__ s, const float* __restrict__ Ls, const float* __restrict__ bs,
+                                                                const float* __restrict__ m, const float* __restrict__ Lw, const float* __restrict__ bw,
+                                                                int B, int P, int F, int D, int H, float* __restrict__ u, float* __restrict__ v) {
+    pdl_enter();
+    extern __shared__ float xs[];  // [kL1Rows][max(F, D)]
+    const int r0 = blockIdx.x * kL1Rows;
+    const int kmax = F > D ? F : D;
+    for (int t = threadIdx.x; t < kL1Rows * kmax; t += blockDim.x) {
+        const int rr = t / kmax, k = t - rr * kmax;
+        const int r = r0 + rr;
+        float x = 0.f;
+        if (r < B) {
+            if (k < F) x = __ldg(s + (size_t)r * F + k);
+        } else if (r < B + P) {
+            if (k < D) x = __ldg(m + (size_t)(r - B) * D + k);
+        }
+        xs[t] = x;
+    }
+    __syncthreads();
+    for (int h = threadIdx.x; h < H; h += blockDim.x) {
+        float accu[kL1Rows];
+        const float b_s = __ldg(bs + h), b_w = __ldg(bw + h);
+#pragma unroll
+        for (int rr = 0; rr < kL1Rows; ++rr) accu[rr] = r0 + rr < B ? b_s : b_w;
+        if (r0 < B) {
+            for (int k = 0; k < F; ++k) {
+                const float wk = __ldg(Ls + (size_t)h * F + k);
+#pragma unroll
+                for (int rr = 0; rr < kL1Rows; ++rr)
+                    if (r0 + rr < B) accu[rr] = __fmaf_rn(xs[rr * kmax + k], wk, accu[rr]);
+            }
+        }
+        if (r0 + kL1Rows > B) {
+            for (int k = 0; k < D; ++k) {
+                const float wk = __ldg(Lw + (size_t)h * D + k);
+#pragma unroll
+                for (int rr = 0; rr < kL1Rows; ++rr)
+                    if (r0 + rr >= B) accu[rr] = __fmaf_rn(xs[rr * kmax + k], wk, accu[rr]);
+            }
+        }
+#pragma unroll
+        for (int rr = 0; rr < kL1Rows; ++rr) {
+            const int r = r0 + rr;
+            const float y = accu[rr] <= 0.f ? 0.f : accu[rr];  // ReLU (-0 -> +0, NaN propagates)
+            if (r < B)
+                u[(size_t)r * H + h] = y;
+            else if (r < B + P)
+                v[(size_t)(r - B) * H + h] = y;
+        }
+    }
+}
+
 // ---- backward: dW1 [H, F + D] = [dU^T feats | dV^T wset], db1 [H] = colsum(dV) -------------------------------------------------------------
 // grid = (ceil(H / 32), kL1Splits); block 256 = 32 output rows h (lane) x 8 column groups (warp).  Split s reduces transitions
 // [s*bs, (s+1)*bs) into the F "u" columns and weight vectors [s*js, (s+1)*js) into the D "v" columns + the bias column.  A chunk of
@@ -217,4 +271,17 @@ extern "C" int morl_pair_layer1_grad_f32(const float* dU, const float* dV, const
     dim3 grid((H + 31) / 32, kL1Splits);
     launch_k(pair_layer1_grad_kernel, dim3(grid), dim3(256), 0, static_cast<cudaStream_t>(stream), dU, dV, feats, wset, B, W, F, D, H, dW1, db1, partial, counters);
     return check_launch("morl_pair_layer1_grad_f32");
+}
+
+extern "C" int morl_product_layer1_uv_f32(const float* s, const float* Ls, const float* bs, int B, int F, const float* m, const float* Lw, const float* bw,
+                                          int P, int D, int H, float* u, float* v, void* stream) {
+    using namespace morl;
+    MORL_REQUIRE(s && Ls && bs && m && Lw && bw && u && v, MORL_ERR_NULL, "morl_product_layer1_uv_f32: NULL pointer argument");
+    MORL_REQUIRE(B > 0 && P > 0 && F > 0 && D > 0 && H > 0, MORL_ERR_SHAPE, "morl_product_layer1_uv_f32: bad shape B=%d P=%d F=%d D=%d H=%d", B, P, F, D, H);
+    const int kmax = F > D ? F : D;
+    const size_t smem = (size_t)kL1Rows * kmax * sizeof(float);
+    MORL_REQUIRE(smem <= 48 * 1024, MORL_ERR_UNSUPPORTED, "morl_product_layer1_uv_f32: input dimension %d too large", kmax);
+    const int blocks = (B + P + kL1Rows - 1) / kL1Rows;
+    launch_k(product_layer1_uv_kernel, dim3(blocks), dim3(256), smem, static_cast<cudaStream_t>(stream), s, Ls, bs, m, Lw, bw, B, P, F, D, H, u, v);
+    return check_launch("morl_product_layer1_uv_f32");
 }

@@ -40,6 +40,7 @@ from ...common.networks import NatureCNN, layer_init, mlp, polyak_update
 from ...common.prioritized_buffer import PrioritizedReplayBuffer
 from ...common.utils import linearly_decaying_value, unique_tol
 from ...common.weights import equally_spaced_weights
+from ...tc_mlp import TCProductMlp
 
 
 class QNet(nn.Module):
@@ -138,6 +139,8 @@ class GPIPD(MOPolicy, MOAgent):
         seed: Optional[int] = None,
         device: Union[th.device, str] = "auto",
         use_cuda_graph: bool = True,
+        use_tensor_cores: bool = False,
+        tensor_core_format: Optional[str] = None,
     ):
         MOAgent.__init__(self, env, device=device, seed=seed)
         MOPolicy.__init__(self, device=device)
@@ -173,6 +176,28 @@ class GPIPD(MOPolicy, MOAgent):
         # a torch.optim.Adam subclass with the reference's arithmetic and state_dict layout, two launches per step, capture-safe
         self.q_optim = FusedClipAdam(chain(*[net.parameters() for net in self.q_nets]), lr=self.learning_rate)
         self.use_cuda_graph = use_cuda_graph
+        # no-grad policy-set evaluations (_envelope_target, _reset_priorities, _rollout_dynamics) on the tensor cores (tc_mlp.TCProductMlp:
+        # LayerNorm and dropout in the GEMM epilogue); the row-paired training pass and gpi_action stay on autograd.  Dropout masks then come
+        # from the engine's Philox stream, not torch's generator: statistically equivalent, not bit-equal.
+        fmt_name = tensor_core_format or os.environ.get("MORL_TC_FMT", "f16x2")
+        if fmt_name not in ("f16x2", "bf16x3"):
+            raise ValueError(f"tensor_core_format must be 'f16x2' or 'bf16x3', got {fmt_name!r}")
+        self.tensor_core_format = fmt_name
+        self._tc_fmt = ops.FMT_F16X2 if fmt_name == "f16x2" else ops.FMT_BF16X3
+        if use_tensor_cores and not TCProductMlp.supported(self.q_nets[0], self._tc_fmt):
+            raise ops._lib.MorlB200Error(
+                "morl_baselines_b200.GPIPD: the tensor-core policy-set evaluation needs a flat observation and equal widths that are multiples "
+                f"of 64 (f16x2) or 32 (bf16x3) and <= 256 (got obs {self.observation_shape}, net_arch {net_arch}, format {fmt_name}); "
+                "pass use_tensor_cores=False to evaluate with library GEMMs")
+        self.use_tensor_cores = bool(use_tensor_cores)
+        self._tc_plans = None  # (plan of q_nets[0], plans of the target nets), activation buffers shared, sized for self._tc_rows pair rows
+        self._tc_rows = 0
+        if self.use_tensor_cores:
+            # made once here, so their dropout seeds are drawn from torch's CPU generator at a fixed point (th.manual_seed reproduces them)
+            tg = [TCProductMlp(self.target_q_nets[0], 128, self._tc_fmt)]
+            tg += [TCProductMlp(n, 128, self._tc_fmt, share_buffers_with=tg[0]) for n in self.target_q_nets[1:]]
+            self._tc_plans = (TCProductMlp(self.q_nets[0], 128, self._tc_fmt, share_buffers_with=tg[0]), tg)
+            self._tc_rows = 128
         self._graphs = {}
         self._support_cache = None
         self.per = per
@@ -288,7 +313,11 @@ class GPIPD(MOPolicy, MOAgent):
             model_env = ModelEnv(self.dynamics, self.env.unwrapped.spec.id, rew_dim=len(w))
             for _h in range(self.dynamics_rollout_len):
                 M = self._support_matrix()
-                q = self.q_nets[0].forward_pairs(obs, M)  # [N, P, A, D] (module mode as the caller left it: dropout as in the reference)
+                if self.use_tensor_cores:
+                    q0, _ = self._tc(obs.shape[0] * M.shape[0])
+                    q = q0.forward_pairs(obs, M).view(obs.shape[0], M.shape[0], self.action_dim, self.reward_dim)
+                else:
+                    q = self.q_nets[0].forward_pairs(obs, M)  # [N, P, A, D] (module mode as the caller left it: dropout as in the reference)
                 _, _, actions = ops.gpi_envelope(q.unsqueeze(0), w.reshape(1, -1), dot_mode=self.dot_mode)  # argmax_i max_a w . Q(s, a, M_i)
                 actions_one_hot = F.one_hot(actions.long(), num_classes=self.action_dim)
                 next_obs_pred, r_pred, dones, info = model_env.step_device(obs, actions_one_hot, deterministic=False)
@@ -320,6 +349,24 @@ class GPIPD(MOPolicy, MOAgent):
         X = np.hstack((m_obs, one_hot))
         Y = np.hstack((m_rewards, m_next_obs - m_obs))
         return self.dynamics.fit(X, Y)
+
+    def _tc_reserve(self, rows: int):
+        """Give the tensor-core plans room for ``rows`` pair rows.  Growing the shared activation buffers drops the captured update graphs,
+        which hold the old ones; ``update`` reserves its rows before it looks a graph up, so no growth happens inside a capture."""
+        if rows <= self._tc_rows:
+            return
+        q0, tg = self._tc_plans
+        cap = max(rows, 2 * self._tc_rows)
+        tg[0].reserve(cap)
+        for p in tg[1:] + [q0]:
+            p.reserve(cap, share_buffers_with=tg[0])
+        self._tc_rows = cap
+        self._graphs = {}
+
+    def _tc(self, rows: int):
+        """(plan of q_nets[0], plans of the target nets) with room for ``rows`` pair rows."""
+        self._tc_reserve(rows)
+        return self._tc_plans
 
     def _support_matrix(self) -> th.Tensor:
         """[P, D] matrix of the support set, cached per support list (captured graphs read it)."""
@@ -381,6 +428,9 @@ class GPIPD(MOPolicy, MOAgent):
         for _ in range(self.gradient_updates if self.global_step >= self.dynamics_rollout_starts else 1):
             P = len(self.weight_support)
             want_prio = self.per or self.gpi_pd
+            if self.use_tensor_cores and self.gpi_pd:
+                # pair rows of this step's envelope target (_device_update): doubled batch x sampled support weights
+                self._tc_reserve((2 * B0 if P > 1 else B0) * (5 if P > 5 else max(P, 1)))
             if not graphable:
                 s_obs, s_actions, s_rewards, s_next_obs, s_dones, idxes = self._sample_batch_experiences()
                 s_actions = s_actions.to(th.int32).reshape(-1)
@@ -447,7 +497,14 @@ class GPIPD(MOPolicy, MOAgent):
     def _envelope_target(self, obs: th.Tensor, w: th.Tensor, sampled_w: th.Tensor, rewards=None, dones=None):
         """GPI envelope target over ``sampled_w`` with the critic-min over the target nets (reference gpi_pd.py:662-690).
         Returns (max_next_q [B, D], None); with rewards/dones the Bellman line is fused in (TILE map for a doubled batch)."""
-        q = th.stack([tn.forward_pairs(obs, sampled_w) for tn in self.target_q_nets])  # [n, B, P, A, D]
+        if self.use_tensor_cores:
+            B, P = obs.shape[0], sampled_w.shape[0]
+            _, plans = self._tc(B * P)
+            q = th.empty((len(plans), B, P, self.action_dim, self.reward_dim), device=obs.device, dtype=th.float32)
+            for i, plan in enumerate(plans):
+                plan.forward_pairs(obs, sampled_w, out=q[i].view(B * P, -1))
+        else:
+            q = th.stack([tn.forward_pairs(obs, sampled_w) for tn in self.target_q_nets])  # [n, B, P, A, D]
         out, _, _ = ops.gpi_envelope(q, w, rewards, dones, self.gamma if rewards is not None else 0.0, self.dot_mode, ops.MAP_BLOCK, ops.MAP_TILE)
         return out, None
 
@@ -499,12 +556,18 @@ class GPIPD(MOPolicy, MOAgent):
         obs_s, nobs_s, act_s, rew_s, done_s = rb.device_stores()
         D = self.reward_dim
         M = self._support_matrix()
+        if self.use_tensor_cores:
+            self._tc_reserve(min(n, chunk) * max(M.shape[0], 1))
         for b in range(0, n, chunk):
             e = min(b + chunk, n)
             obs, nobs, rew, done = obs_s[b:e], nobs_s[b:e], rew_s[b:e], done_s[b:e]
             act = act_s[b:e].long().reshape(-1, 1, 1).expand(-1, 1, D)
             wrow = w.reshape(1, D)
-            q_a = self.q_nets[0](obs, wrow.expand(e - b, D)).gather(1, act).squeeze(1)
+            if self.use_tensor_cores:  # the chunk against the single weight: a P = 1 pair batch
+                q0, _ = self._tc(e - b)
+                q_a = q0.forward_pairs(obs, wrow).view(e - b, self.action_dim, D).gather(1, act).squeeze(1)
+            else:
+                q_a = self.q_nets[0](obs, wrow.expand(e - b, D)).gather(1, act).squeeze(1)
             if self.gpi_pd:
                 max_next_q, _ = self._envelope_target(nobs, wrow, M)
             else:

@@ -441,6 +441,68 @@ def gemm_planes(a_planes: th.Tensor, b_planes: th.Tensor, n_out: int, bias: Opti
     return c_f32, c_planes
 
 
+def gemm_planes_ln(a_planes: th.Tensor, b_planes: th.Tensor, n_out: int, bias: Optional[th.Tensor] = None, ln_weight: Optional[th.Tensor] = None,
+                   ln_bias: Optional[th.Tensor] = None, ln_eps: Optional[float] = None, drop_p: float = 0.0, drop_seed: Optional[th.Tensor] = None,
+                   drop_offset: Optional[th.Tensor] = None, drop_salt: int = 0, out_f32: bool = False, out_planes: bool = True,
+                   c_f32: Optional[th.Tensor] = None, c_planes: Optional[th.Tensor] = None, reverse_tiles: bool = False,
+                   a_scale: Optional[th.Tensor] = None, b_scale: Optional[th.Tensor] = None, c_scale: Optional[th.Tensor] = None,
+                   drop_bits_out: Optional[th.Tensor] = None):
+    """Hidden layer Linear -> Dropout -> LayerNorm -> ReLU in one tensor-core GEMM: C = relu(LN(dropout(A . B^T + bias))).
+    a_planes [P, M, K], b_planes [P, n_out, K] (n_out % 32 == 0, <= 256).  ``ln_eps`` None: no LayerNorm (``ln_weight`` / ``ln_bias``
+    [n_out] fp32, None = 1 / 0).  Dropout runs when ``drop_seed`` (int64 [1]) and ``drop_offset`` (int32 [1], the pass counter, see
+    :func:`philox_advance`) are given: element kept iff its Philox4x32-10 draw >= round(drop_p 2^32), kept values scaled by 1 / (1 - drop_p);
+    ``drop_salt`` separates the layers of one pass.  ``drop_bits_out`` ([M, 8] int32) receives the keep mask in the ReLU-bit layout.
+    Returns (c_f32 [M, n_out] or None, c_planes [P, M, n_out] holding c_scale * C, or None)."""
+    fmt = fmt_of(a_planes)
+    if fmt_of(b_planes) != fmt or not a_planes.is_cuda:
+        raise _lib.MorlB200Error("gemm_planes_ln: operands must be CUDA plane tensors of the same format")
+    _, M, K = a_planes.shape
+    _, n_pad, Kb = b_planes.shape
+    if Kb != K or a_planes.stride(1) != K or b_planes.stride(1) != K:
+        raise _lib.MorlB200Error("gemm_planes_ln: operand planes must be K-major with equal K")
+    if n_pad != n_out or n_out % 32 or n_out > 256:
+        raise _lib.MorlB200Error(f"gemm_planes_ln: need weight planes [P, n_out, K] with n_out % 32 == 0 and n_out <= 256 (got {tuple(b_planes.shape)}, n_out={n_out})")
+    if not 0.0 <= drop_p < 1.0:
+        raise _lib.MorlB200Error(f"gemm_planes_ln: dropout probability {drop_p} outside [0, 1)")
+    if (drop_seed is None) != (drop_offset is None):
+        raise _lib.MorlB200Error("gemm_planes_ln: dropout needs both drop_seed and drop_offset")
+    if drop_seed is not None and (drop_seed.dtype != th.int64 or drop_offset.dtype != th.int32 or not drop_seed.is_cuda or not drop_offset.is_cuda):
+        raise _lib.MorlB200Error("gemm_planes_ln: drop_seed must be a CUDA int64 [1] tensor and drop_offset a CUDA int32 [1] tensor")
+    for name, t in (("bias", bias), ("ln_weight", ln_weight), ("ln_bias", ln_bias)):
+        if t is not None and (t.dtype != th.float32 or t.numel() != n_out or not t.is_contiguous() or not t.is_cuda):
+            raise _lib.MorlB200Error(f"gemm_planes_ln: {name} must be a contiguous CUDA float32 vector of {n_out}")
+    dev = a_planes.device
+    if out_f32 and c_f32 is None:
+        c_f32 = th.empty((M, n_out), device=dev, dtype=th.float32)
+    if out_planes and c_planes is None:
+        c_planes = empty_planes(fmt, M, n_out, dev)
+    if c_f32 is None and c_planes is None:
+        raise _lib.MorlB200Error("gemm_planes_ln: no output requested")
+    if drop_bits_out is not None and (drop_bits_out.dtype != th.int32 or tuple(drop_bits_out.shape) != (M, relu_bits_words(n_out))
+                                      or not drop_bits_out.is_contiguous()):
+        raise _lib.MorlB200Error(f"gemm_planes_ln: the keep mask must be contiguous int32 [{M}, {relu_bits_words(n_out)}]")
+    rc = _lib.load().morl_gemm_planes_ln_f32(fmt, _ptr(a_planes), a_planes.stride(0), _ptr(a_scale), _ptr(b_planes), b_planes.stride(0), _ptr(b_scale), M,
+                                             n_out, K, _ptr(None if bias is None else bias.detach()), int(ln_eps is not None),
+                                             _ptr(None if ln_weight is None else ln_weight.detach()), _ptr(None if ln_bias is None else ln_bias.detach()),
+                                             float(ln_eps or 0.0), float(drop_p), _ptr(drop_seed), _ptr(drop_offset), int(drop_salt) & 0xFFFFFFFF,
+                                             _ptr(c_f32), 0 if c_f32 is None else c_f32.stride(0), _ptr(c_planes),
+                                             0 if c_planes is None else c_planes.shape[2], 0 if c_planes is None else c_planes.stride(0), _ptr(c_scale),
+                                             int(reverse_tiles), _ptr(drop_bits_out), _stream())
+    _lib.check(rc, "morl_gemm_planes_ln_f32")
+    _count()
+    return c_f32, c_planes
+
+
+def philox_advance(offset: th.Tensor, inc: int = 1) -> th.Tensor:
+    """offset[0] += inc (int32 [1] CUDA tensor, wrapping) as one stream-ordered launch: the dropout pass counter of :func:`gemm_planes_ln`."""
+    if not isinstance(offset, th.Tensor) or not offset.is_cuda or offset.dtype != th.int32 or offset.numel() != 1:
+        raise _lib.MorlB200Error("philox_advance: offset must be a CUDA int32 [1] tensor")
+    rc = _lib.load().morl_philox_advance(_ptr(offset), int(inc) & 0xFFFFFFFF, _stream())
+    _lib.check(rc, "morl_philox_advance")
+    _count()
+    return offset
+
+
 def ensemble_sample(out: th.Tensor, max_logvar: th.Tensor, min_logvar: th.Tensor, model_idx: th.Tensor, noise: Optional[th.Tensor] = None,
                     obs: Optional[th.Tensor] = None, rew_dim: int = 0):
     """Probabilistic-ensemble sampling + ensemble uncertainty in one pass (reference probabilistic_ensemble.py:115-154, utils.py:165).
@@ -624,6 +686,45 @@ def pairs_relu_split(u: th.Tensor, v: th.Tensor, out: Optional[th.Tensor] = None
     _lib.check(rc, "morl_pairs_relu_split_planes")
     _count()
     return out
+
+
+def pairs_product_split(u: th.Tensor, v: th.Tensor, out: Optional[th.Tensor] = None, fmt: int = FMT_F16X2, scale: Optional[th.Tensor] = None) -> th.Tensor:
+    """u[b] * v[p] for every pair (one fp32 multiply), written as planes [P_fmt, B*P, H] of scale * h (row b*P + p): the product-conditioned
+    first layer of GPI-PD's Q-network."""
+    u, v = _dev(u, "u"), _dev(v, "v")
+    B, H = u.shape
+    P = v.shape[0]
+    if v.shape[1] != H or H % 8:
+        raise _lib.MorlB200Error(f"pairs_product_split: u {tuple(u.shape)} and v {tuple(v.shape)} need equal widths, a multiple of 8")
+    if out is None:
+        out = empty_planes(fmt, B * P, H, u.device)
+    else:
+        fmt = fmt_of(out)
+        if out.shape[1] < B * P or out.shape[2] != H or out.stride(1) != H:
+            raise _lib.MorlB200Error(f"pairs_product_split: out must be planes [P, >= {B * P}, {H}] with rows of {H}")
+    rc = _lib.load().morl_pairs_product_split_planes(fmt, _ptr(u), _ptr(v), B, P, H, _ptr(out), out.stride(0), _ptr(scale), _stream())
+    _lib.check(rc, "morl_pairs_product_split_planes")
+    _count()
+    return out
+
+
+def product_layer1_uv(s: th.Tensor, s_weight: th.Tensor, s_bias: th.Tensor, m: th.Tensor, w_weight: th.Tensor, w_bias: th.Tensor,
+                      u: Optional[th.Tensor] = None, v: Optional[th.Tensor] = None):
+    """u = relu(s @ Ls^T + bs) [B, H] and v = relu(m @ Lw^T + bw) [P, H] in one launch (the two feature maps of GPI-PD's Q-network)."""
+    s, m = _dev(s, "s"), _dev(m, "m")
+    s_weight, s_bias, w_weight, w_bias = _dev(s_weight.detach(), "s_weight"), _dev(s_bias.detach(), "s_bias"), _dev(w_weight.detach(), "w_weight"), _dev(w_bias.detach(), "w_bias")
+    B, F = s.shape
+    P, D = m.shape
+    H = s_weight.shape[0]
+    if s_weight.shape[1] != F or tuple(w_weight.shape) != (H, D) or s_bias.numel() != H or w_bias.numel() != H:
+        raise _lib.MorlB200Error(f"product_layer1_uv: weights {tuple(s_weight.shape)} / {tuple(w_weight.shape)} do not match s {tuple(s.shape)}, m {tuple(m.shape)}")
+    u = th.empty((B, H), device=s.device, dtype=th.float32) if u is None else u
+    v = th.empty((P, H), device=s.device, dtype=th.float32) if v is None else v
+    rc = _lib.load().morl_product_layer1_uv_f32(_ptr(s), _ptr(s_weight), _ptr(s_bias), B, F, _ptr(m), _ptr(w_weight), _ptr(w_bias), P, D, H, _ptr(u),
+                                                _ptr(v), _stream())
+    _lib.check(rc, "morl_product_layer1_uv_f32")
+    _count()
+    return u, v
 
 
 def pair_layer1_uv(feats: th.Tensor, wset: th.Tensor, weight: th.Tensor, bias: th.Tensor, u: Optional[th.Tensor] = None,

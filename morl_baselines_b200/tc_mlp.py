@@ -340,3 +340,149 @@ class TCPairMlpFn(th.autograd.Function):
         feats, wset = ctx.saved_tensors
         grads = ctx.plan.backward(feats, wset, dq.contiguous())
         return (None, None, None, *grads)
+
+
+MAX_PRODUCT_WIDTH = 256   # LayerNorm epilogue: one column unit holds the whole row
+
+
+class TCProductMlp:
+    """Forward-only tensor-core plan for GPI-PD's product-conditioned Q-network (multi_policy/gpi_pd/gpi_pd.py ``QNet``):
+
+        layer 1 : u = relu(s Ls^T + bs) (B rows), v = relu(M Lw^T + bw) (P rows) -- one launch (morl_product_layer1_uv_f32) --
+                  h1[b*P + p] = u[b] * v[p] straight into operand planes (morl_pairs_product_split_planes);
+        hidden  : Linear [Dropout] [LayerNorm] ReLU, one morl_gemm_planes_ln_f32 launch each (dropout and LayerNorm in the epilogue);
+        output  : fp32 Q rows, morl_qhead_gemm_f32 when <= 32 wide, else morl_gemm_planes_f32.
+
+    Dropout runs iff the module is in train mode and p > 0, as torch applies it, but its masks come from the engine's Philox stream (key drawn
+    once from torch's CPU generator when the plan is made, counter advanced on the device once per pass), not from torch's generator: they
+    are statistically equivalent, not bit-equal.  The plan is sized for ``max_rows`` pair rows (two ping-pong activation buffers, shareable
+    between plans with ``share_buffers_with``) and runs any smaller call on views."""
+
+    @staticmethod
+    def supported(qnet: nn.Module, fmt: int = _DEFAULT_FMT) -> bool:
+        return TCProductMlp._layers(qnet, fmt) is not None
+
+    @staticmethod
+    def _layers(qnet: nn.Module, fmt: int):
+        """(state Linear, weight Linear, [(Linear, Dropout or None, LayerNorm or None)], output Linear), or None if unsupported."""
+        sf, wf, net = getattr(qnet, "state_features", None), getattr(qnet, "weights_features", None), getattr(qnet, "net", None)
+        if not all(isinstance(m, nn.Sequential) for m in (sf, wf, net)):
+            return None  # (NatureCNN image features among others)
+        if len(sf) != 2 or len(wf) != 2 or not all(isinstance(a, nn.Linear) and isinstance(b, nn.ReLU) for a, b in (sf, wf)):
+            return None
+        width = sf[0].out_features
+        if wf[0].out_features != width:
+            return None
+        mods, hidden, i = list(net), [], 0
+        while i < len(mods) - 1:
+            lin = mods[i]
+            if not isinstance(lin, nn.Linear):
+                return None
+            i += 1
+            drop = ln = None
+            if i < len(mods) and isinstance(mods[i], nn.Dropout):
+                drop, i = mods[i], i + 1
+            if i < len(mods) and isinstance(mods[i], nn.LayerNorm):
+                ln, i = mods[i], i + 1
+                if not ln.elementwise_affine or ln.weight is None or ln.bias is None or tuple(ln.normalized_shape) != (lin.out_features,):
+                    return None
+            if i >= len(mods) or not isinstance(mods[i], nn.ReLU):
+                return None
+            i += 1
+            hidden.append((lin, drop, ln))
+        if i != len(mods) - 1 or not isinstance(mods[-1], nn.Linear):
+            return None
+        out = mods[-1]
+        kmul = 64 if fmt == ops.FMT_F16X2 else 32
+        widths = {width} | {l.out_features for l, _, _ in hidden}
+        if len(widths) != 1 or width % kmul or width > MAX_PRODUCT_WIDTH or out.out_features > 256:
+            return None
+        if any(l.in_features != width for l, _, _ in hidden) or out.in_features != width:
+            return None
+        return sf[0], wf[0], hidden, out
+
+    def __init__(self, qnet: nn.Module, max_rows: int, fmt: Optional[int] = None, share_buffers_with: Optional["TCProductMlp"] = None):
+        fmt = _DEFAULT_FMT if fmt is None else fmt
+        layers = TCProductMlp._layers(qnet, fmt)
+        if layers is None:
+            raise ops._lib.MorlB200Error("TCProductMlp: unsupported network (vector observations; state / weight features Linear + ReLU; hidden layers "
+                                         "Linear [Dropout] [LayerNorm] ReLU of one width, a multiple of 64 (f16x2) or 32 (bf16x3) and <= "
+                                         f"{MAX_PRODUCT_WIDTH}; output layer <= 256 wide)")
+        self.qnet, self.fmt = qnet, fmt
+        self.l_s, self.l_w, self.hidden, self.last = layers
+        self.width = self.l_s.out_features
+        self.n_out = self.last.out_features
+        dev = self.l_s.weight.device
+        self.max_rows, self.act = 0, None
+        self.reserve(max_rows, share_buffers_with)
+        scaled = fmt == ops.FMT_F16X2
+        self.s_act = ops.scale_tensor(ACT_SCALE, dev) if scaled else None
+        lins = [l for l, _, _ in self.hidden] + [self.last]
+        self.wp = [ops.empty_planes(fmt, _pad(l.out_features, 32), l.in_features, dev) for l in lins]
+        self.s_w = [ops.scale_tensor(1.0, dev) if scaled else None for _ in lins]
+        self.seed = th.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=th.int64).to(dev)  # torch's CPU generator: th.manual_seed reproduces it
+        self.offset = th.zeros(1, dtype=th.int32, device=dev)
+        self.drop_bits = None  # list of [rows, 8] int32 keep masks, one per hidden layer (tests)
+
+    def reserve(self, max_rows: int, share_buffers_with: Optional["TCProductMlp"] = None):
+        """Size the two activation buffers for ``max_rows`` pair rows (new buffers, or those of ``share_buffers_with``).  Seeds, weight
+        planes and the dropout pass counter are kept.  Captured CUDA graphs that used the old buffers must be discarded by the caller."""
+        if share_buffers_with is not None:
+            o = share_buffers_with
+            if o.fmt != self.fmt or o.width != self.width or o.max_rows < max_rows:
+                raise ops._lib.MorlB200Error("TCProductMlp: plans sharing buffers need the same format, width and at least as many rows")
+            self.act, self.max_rows = o.act, o.max_rows
+        else:
+            self.max_rows = int(max_rows)
+            self.act = [ops.empty_planes(self.fmt, self.max_rows, self.width, self.l_s.weight.device) for _ in range(2)]
+
+    def refresh_weights(self):
+        lins = [l for l, _, _ in self.hidden] + [self.last]
+        jobs = [(l.weight.detach(), wp, False, s, W_TARGET_EXP if self.fmt == ops.FMT_F16X2 else None) for l, wp, s in zip(lins, self.wp, self.s_w)]
+        for i in range(0, len(jobs), 16):
+            ops.split_planes_multi(jobs[i:i + 16], self.fmt)
+
+    def dropout_active(self) -> bool:
+        return any(d is not None and d.training and d.p > 0 for _, d, _ in self.hidden)
+
+    @th.no_grad()
+    def forward_pairs(self, obs: th.Tensor, M: th.Tensor, out: Optional[th.Tensor] = None) -> th.Tensor:
+        """Q(s_b, M_p) for every pair: obs [B, F], M [P, D] -> out [B*P, A*D] fp32 (row b*P + p; ``out`` may be a contiguous slice of a
+        caller's [n_nets, B*P, A*D] tensor).  Weight planes are re-split first, so in-place optimiser / Polyak steps are always seen."""
+        obs = obs.reshape(obs.shape[0], -1)
+        B, P = obs.shape[0], M.shape[0]
+        rows = B * P
+        if rows > self.max_rows:
+            raise ops._lib.MorlB200Error(f"TCProductMlp: {rows} pair rows exceed the plan's {self.max_rows}")
+        if out is None:
+            out = th.empty((rows, self.n_out), device=obs.device, dtype=th.float32)
+        elif tuple(out.shape) != (rows, self.n_out) or not out.is_contiguous():
+            raise ops._lib.MorlB200Error(f"TCProductMlp: out must be a contiguous [{rows}, {self.n_out}] tensor")
+        self.refresh_weights()
+        drop = self.dropout_active()
+        if drop:
+            ops.philox_advance(self.offset)  # a fresh mask per pass, also under CUDA-graph replay
+        u, v = ops.product_layer1_uv(obs, self.l_s.weight, self.l_s.bias, M, self.l_w.weight, self.l_w.bias)
+        a = ops.pairs_product_split(u, v, out=self.act[0][:, :rows], scale=self.s_act)
+        for k, (lin, d, ln) in enumerate(self.hidden):
+            on = d is not None and d.training and d.p > 0
+            bits = None
+            if self.drop_bits is not None and on:
+                bits = self.drop_bits[k][:rows]
+            _, a = ops.gemm_planes_ln(a, self.wp[k], lin.out_features, bias=lin.bias, ln_weight=None if ln is None else ln.weight,
+                                      ln_bias=None if ln is None else ln.bias, ln_eps=None if ln is None else float(ln.eps),
+                                      drop_p=float(d.p) if on else 0.0, drop_seed=self.seed if on else None, drop_offset=self.offset if on else None,
+                                      drop_salt=k, c_planes=self.act[(k + 1) & 1][:, :rows], reverse_tiles=_SNAKE and bool(k & 1),
+                                      a_scale=self.s_act, b_scale=self.s_w[k], c_scale=self.s_act, drop_bits_out=bits)
+        n = len(self.hidden)
+        rev = _SNAKE and bool(n & 1)
+        if _NARROW_HEAD and self.wp[n].shape[1] == 32 and ops.qhead_gemm_supported(self.fmt, rows, self.n_out, self.width):
+            return ops.qhead_gemm(a, self.wp[n], self.n_out, self.last.bias.detach(), out=out, a_scale=self.s_act, w_scale=self.s_w[n], reverse_tiles=rev)
+        ops.gemm_planes(a, self.wp[n], self.n_out, bias=self.last.bias.detach(), relu=False, out_f32=True, c_f32=out, reverse_tiles=rev,
+                        a_scale=self.s_act, b_scale=self.s_w[n])
+        return out
+
+    def record_masks(self, on: bool = True):
+        """Keep the dropout keep masks of the following passes in ``drop_bits`` (one [max_rows, 8] int32 tensor per hidden layer; tests)."""
+        dev = self.l_s.weight.device
+        self.drop_bits = [ops.empty_relu_bits(self.max_rows, dev, self.width) for _ in self.hidden] if on else None
