@@ -34,6 +34,12 @@ bool pdl_enabled() {
     return on;
 }
 
+bool gemm_pdl_enabled() {
+    // programmatic dependent launch between the consecutive tensor-core GEMMs of the update (MORL_GEMM_PDL=0 disables it)
+    static const bool on = [] { const char* e = getenv("MORL_GEMM_PDL"); return !(e && e[0] == '0'); }();
+    return on;
+}
+
 }  // namespace morl
 
 extern "C" {

@@ -38,10 +38,12 @@ __device__ __forceinline__ void pdl_enter() {
     asm volatile("griddepcontrol.wait;" ::: "memory");
 }
 
-bool pdl_enabled();  // api.cu
+bool pdl_enabled();       // api.cu: MORL_PDL=1
+bool gemm_pdl_enabled();  // api.cu: MORL_GEMM_PDL, default on (the tensor-core GEMM and qhead launches)
 
+// Launch with the PDL attribute iff `pdl`.
 template <typename... KArgs, typename... Args>
-static inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
+static inline void launch_k_pdl(bool pdl, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = grid;
@@ -52,8 +54,26 @@ static inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = pdl ? 1 : 0;
     cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+
+template <typename... KArgs, typename... Args>
+static inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
+    launch_k_pdl(pdl_enabled(), kernel, grid, block, smem, stream, static_cast<Args&&>(args)...);
+}
+
+// Raises the dynamic-shared-memory limit of kernel K to `bytes` once per process (the first call of each instantiation).
+template <auto K>
+static inline void set_smem_limit_once(size_t bytes) {
+    static const bool done = (cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes), true);
+    (void)done;
+}
+
+// SMs of the current device, 132 (H100 SXM) when it cannot be queried
+static inline int sm_count() {
+    const int n = morl_device_sm_count();
+    return n > 0 ? n : 132;
 }
 
 // ---- scalarisation w . q in the three documented arithmetics (include/morl_b200.h) --------------

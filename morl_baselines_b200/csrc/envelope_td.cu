@@ -519,8 +519,7 @@ extern "C" int morl_envelope_td_f32(const float* q_online, const float* q_target
     MORL_REQUIRE(aligned16(q_online) && aligned16(q_target) && aligned16(target_out), MORL_ERR_ALIGN,
                  "morl_envelope_td_f32: q_online/q_target/target_out must be 16-byte aligned");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int sms = morl_device_sm_count();
-    if (sms <= 0) sms = 132;
+    const int sms = sm_count();
     const EnvelopePath path = envelope_path_override();
     const long long Cw = (long long)W * A;
     const size_t wp_smem = (size_t)(2 * ((Cw * D + 3) & ~3LL) + 3 * 256 + 16) * 4;  // Q_on[b], Q_tg[b], wp::Scratch, barriers

@@ -28,6 +28,8 @@
 //              64-byte swizzle, 2 x 72 KB), mbarrier ring; it keeps loading the next tile while the consumers are in their epilogue.
 // Operands: A [P][M][K] (K-major), B [P][N_pad][K] (K-major), K % BK == 0, N_pad % 32 == 0, N_pad <= 512.  An output wider than 256
 // columns runs as two column units [0, 256) and [256, N_pad) of the same tile, each with the shared-memory plan of N_pad = 256.
+// The chained hidden layers (gemm_chain_kernel) run the same pipeline -- carve_kplan, the producer's load_unit, the consumer's consume_unit and
+// reload_bias -- on their own schedule of units.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -80,8 +82,6 @@ struct GemmArgs {
     const float* a_scale;        // device scalars (powers of two) the A / B planes were scaled by; nullptr = 1
     const float* b_scale;
     const float* c_scale;        // scale applied to the output before it is re-split into c_planes; nullptr = 1
-    int l2_hint;                 // L2 eviction hints on the operand loads (MORL_GEMM_L2HINT=1, default off): A evict_first, B evict_last
-    int pdl;                     // launched with programmatic stream serialisation: overlap this grid's prologue with the predecessor's tail
     int reverse;                 // walk the row tiles from the last to the first (see morl_gemm_planes_f32: L2 reuse between chained layers)
     unsigned long long* stats;   // diagnostics (MORL_GEMM_STATS=1), else nullptr: [0] consumer wait-on-TMA cycles, [1] consumer loop total,
                                  // [2] producer wait-on-free-stage, [3] epilogue busy
@@ -137,6 +137,56 @@ struct KPlan {
     static_assert(kBytes <= 227 * 1024, "dynamic shared memory of one CTA on sm_90");
 };
 
+// The carve of KPlan in the dynamic shared memory of a K-major kernel (gemm_planes_kernel, gemm_chain_kernel)
+struct KSmem {
+    uint8_t* a;                  // ring stages of A boxes (KPlan::kAStage each)
+    uint8_t* b;                  // ring stages of B rows, b_stage bytes each
+    uint32_t b_stage;
+    uint8_t* c;                  // TMA-store staging tiles, two per consumer warp
+    uint64_t* full;              // ring barriers [kMaxStages]
+    uint64_t* empty;             // [kMaxStages], followed by the kernel's own barriers
+    float* bias;                 // [256]: the biases of the current unit, indexed by column within the unit
+};
+
+template <int FMT>
+__device__ __forceinline__ KSmem carve_kplan(uint8_t* smem_raw, uint32_t n_stages, uint32_t b_stage) {
+    using L = KPlan<FMT>;
+    uint8_t* sm = align_1k(smem_raw);
+    KSmem s;
+    s.a = sm;
+    s.b = sm + n_stages * L::kAStage;  // (n_stages * (A + B) <= kOffC, checked on the host)
+    s.b_stage = b_stage;
+    s.c = sm + L::kOffC;
+    s.full = reinterpret_cast<uint64_t*>(sm + L::kOffBar);
+    s.empty = s.full + L::kMaxStages;
+    s.bias = reinterpret_cast<float*>(sm + L::kOffBias);
+    return s;
+}
+
+// Producer of one work unit: per K block, wait for a free stage, then one A box (P planes x 128 rows x BK) and the P x n_cnt / 32 B boxes of
+// the unit's columns [n_begin, n_begin + n_cnt).  Returns the cycles spent waiting for free stages if `stats`, else 0.
+template <int FMT>
+__device__ __forceinline__ long long load_unit(const KSmem& s, Ring& ring, const CUtensorMap* tmA, const CUtensorMap* tmB, int row0, int n_begin, int n_cnt,
+                                               int n_kblk, bool stats) {
+    using F = PlaneFmt<FMT>;
+    using L = KPlan<FMT>;
+    const uint32_t b_plane = (uint32_t)n_cnt * L::kRowB;
+    long long wait_cycles = 0;
+    for (int kb = 0; kb < n_kblk; ++kb) {
+        const long long c0 = stats ? clock64() : 0;
+        g_mbar_wait(&s.empty[ring.stage], ring.phase ^ 1u);
+        if (stats) wait_cycles += clock64() - c0;
+        uint64_t* full = &s.full[ring.stage];
+        g_mbar_expect_tx(full, L::kAStage + (uint32_t)F::P * b_plane);
+        tma_load_3d(s.a + ring.stage * L::kAStage, tmA, full, kb * F::BK, row0, 0);
+        uint8_t* bs = s.b + ring.stage * s.b_stage;
+        for (int p = 0; p < F::P; ++p)
+            for (int r = 0; r < n_cnt; r += kGemmBoxN) tma_load_3d(bs + (uint32_t)p * b_plane + (uint32_t)r * L::kRowB, tmB, full, kb * F::BK, n_begin + r, p);
+        ring.advance();
+    }
+    return wait_cycles;
+}
+
 // One work unit of a consumer warpgroup: D[64 x N] = sum over the K blocks of the staged planes, NPROD products per K step in the order of
 // PlaneFmt (small terms first).  A stage goes back to the producer as soon as the MMAs reading it have completed: one group of
 // wgmma stays in flight while the next stage is awaited.
@@ -145,9 +195,7 @@ struct KPlan {
 // mode the LEADING products A0B0 go to acc[0, 64) and the correction products (2^-11 / 2^-8 of the magnitude) to acc[64, 128), so only
 // K/16 accumulations happen at full magnitude; the epilogue adds the two with one correctly rounded fp32 add.
 template <int FMT, int N, int SPLIT>
-__device__ __forceinline__ void mma_unit(float (&acc)[128], uint8_t* smA, uint8_t* smB, uint32_t a_stage_bytes, uint32_t b_stage_stride, int n_kblk,
-                                         uint64_t* full, uint64_t* empty, uint32_t& stage, uint32_t& phase, uint32_t n_stages, int wg, int lane,
-                                         long long* wait_cycles) {
+__device__ __forceinline__ void mma_unit(float (&acc)[128], const KSmem& s, Ring& ring, int n_kblk, int wg, int lane, long long* wait_cycles) {
     using F = PlaneFmt<FMT>;
     static_assert(!SPLIT || N <= 128, "split accumulators: two N / 2-register accumulators per thread");
     constexpr uint32_t ROWB = F::BK * 2;
@@ -155,11 +203,11 @@ __device__ __forceinline__ void mma_unit(float (&acc)[128], uint8_t* smA, uint8_
     uint32_t prev = 0;
     for (int kb = 0; kb < n_kblk; ++kb) {
         const long long c0 = wait_cycles ? clock64() : 0;
-        g_mbar_wait(&full[stage], phase);
+        g_mbar_wait(&s.full[ring.stage], ring.phase);
         if (wait_cycles) *wait_cycles += clock64() - c0;
         wgmma_fence();
-        const uint32_t a0 = g_smem_u32(smA + stage * a_stage_bytes) + (uint32_t)wg * 64u * ROWB;
-        const uint32_t b0 = g_smem_u32(smB + stage * b_stage_stride);
+        const uint32_t a0 = g_smem_u32(s.a + ring.stage * KPlan<FMT>::kAStage) + (uint32_t)wg * 64u * ROWB;
+        const uint32_t b0 = g_smem_u32(s.b + ring.stage * s.b_stage);
 #pragma unroll
         for (int ks = 0; ks < F::BK / 16; ++ks) {
 #pragma unroll
@@ -175,16 +223,13 @@ __device__ __forceinline__ void mma_unit(float (&acc)[128], uint8_t* smA, uint8_
         wgmma_commit();
         if (kb > 0) {
             wgmma_wait<1>();  // the MMAs of the previous stage have read it
-            if (lane == 0) g_mbar_arrive(&empty[prev]);
+            if (lane == 0) g_mbar_arrive(&s.empty[prev]);
         }
-        prev = stage;
-        if (++stage == n_stages) {
-            stage = 0;
-            phase ^= 1u;
-        }
+        prev = ring.stage;
+        ring.advance();
     }
     wgmma_wait<0>();
-    if (n_kblk > 0 && lane == 0) g_mbar_arrive(&empty[prev]);
+    if (n_kblk > 0 && lane == 0) g_mbar_arrive(&s.empty[prev]);
 }
 
 struct EpiArgs {
@@ -399,6 +444,49 @@ __device__ __forceinline__ void ln_dropout_unit(float (&acc)[128], int N, int rb
     }
 }
 
+// bias_s[c] = mul * bias[n_begin + c] for the 256 columns of a unit (0 at and beyond n_end, or without a bias), by the 256 threads of the
+// consumer warps; the first barrier waits until every consumer warp has left the previous unit's epilogue
+__device__ __forceinline__ void reload_bias(float* bias_s, const float* bias, int n_begin, int n_end, float mul) {
+    bar_sync_named(1, 256);
+    const int col = n_begin + (int)threadIdx.x;
+    bias_s[threadIdx.x] = (bias && col < n_end) ? __ldg(bias + col) * mul : 0.f;
+    bar_sync_named(1, 256);
+}
+
+// Consumer warp of one work unit of the columns [n_begin, n_begin + n_cnt): the MMAs of its K blocks (mma_unit at the unit's width), then
+// after_mma() (the per-layer kernel: the biases of a wide output's unit, the LayerNorm / dropout pre-pass), then the 32-column chunks of the
+// epilogue (split accumulators added first).
+template <int FMT, int SPLIT, bool PRE, typename AfterMma>
+__device__ __forceinline__ void consume_unit(float (&acc)[128], const KSmem& s, Ring& ring, int n_kblk, int n_begin, int n_cnt, int rbase, int wg, int lane,
+                                             long long* wait_cycles, AfterMma&& after_mma, const EpiArgs& e, const CUtensorMap* tmC, uint8_t* my_stage,
+                                             uint32_t& n_stored, float& amax) {
+#define MORL_UNIT(N_) \
+    case N_: mma_unit<FMT, N_, SPLIT>(acc, s, ring, n_kblk, wg, lane, wait_cycles); break;
+    switch (n_cnt) {
+        MORL_UNIT(32) MORL_UNIT(64) MORL_UNIT(96) MORL_UNIT(128)
+        default:
+            if constexpr (!SPLIT) {
+                switch (n_cnt) {
+                    MORL_UNIT(160) MORL_UNIT(192) MORL_UNIT(224) MORL_UNIT(256)
+                    default: __trap();
+                }
+            } else {
+                __trap();
+            }
+    }
+#undef MORL_UNIT
+    after_mma();
+#pragma unroll
+    for (int c = 0; c < (SPLIT ? 4 : 8); ++c) {
+        if (32 * c < n_cnt) {
+            float a[16];
+#pragma unroll
+            for (int j = 0; j < 16; ++j) a[j] = SPLIT ? __fadd_rn(acc[16 * c + j], acc[64 + 16 * c + j]) : acc[16 * c + j];
+            epilogue_chunk<FMT, PRE>(a, n_begin + 32 * c, rbase, lane, e, tmC, my_stage, n_stored, amax);
+        }
+    }
+}
+
 // One CTA per 128-row tile.  SPLIT = 1: see mma_unit; a tile wider than 128 columns is then computed as column units of 128 (the A boxes of
 // the tile are staged once per unit).  SPLIT = 0 and N_pad > 256: two column units [0, 256) and [256, N_pad), each with the stage plan of
 // N_pad = 256 and this unit's 256 biases in shared memory.  EPI = kEpiLn (SPLIT = 0, N = N_pad <= 256): ln_dropout_unit before the chunks.
@@ -406,31 +494,16 @@ template <int FMT, int SPLIT, int EPI = kEpiPlain>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC,
                    const GemmArgs g) {
-    using F = PlaneFmt<FMT>;
     using L = KPlan<FMT>;
-    constexpr int P = F::P;
-    constexpr int BK = F::BK;
-    constexpr int kMaxStages = L::kMaxStages;
-    constexpr uint32_t ROWB = L::kRowB;
-    const uint32_t kStages = (uint32_t)g.n_stages;  // runtime: narrow outputs leave room for a deeper ring (host: morl_gemm_planes_f32)
     extern __shared__ uint8_t gsmem_raw[];
-    // 1 KB alignment by pointer arithmetic ON the shared array (not through an integer cast), so that the compiler keeps every derived
-    // pointer in the shared address space: through the cast the bias / staging accesses were generic LD.E / ST.E (long-scoreboard stalls)
-    uint8_t* gsmem = gsmem_raw + ((1024u - (g_smem_u32(gsmem_raw) & 1023u)) & 1023u);
-    const int BN = g.N_pad;
-    constexpr uint32_t a_stage_bytes = L::kAStage;
-    const uint32_t b_stage_stride = g.b_stage;
-    uint8_t* smA = gsmem;
-    uint8_t* smB = gsmem + kStages * a_stage_bytes;  // (n_stages * (A + B) <= kOffC, checked on the host)
-    uint8_t* stage_c = gsmem + L::kOffC;  // per-consumer-warp staging tiles for the TMA store of the re-split activations
-    uint64_t* full = reinterpret_cast<uint64_t*>(gsmem + L::kOffBar);
-    uint64_t* empty = full + kMaxStages;
-    float* bias_s = reinterpret_cast<float*>(gsmem + L::kOffBias);  // [256]
+    // (ring depth g.n_stages at run time: narrow outputs leave room for a deeper ring, host: morl_gemm_planes_f32)
+    const KSmem s = carve_kplan<FMT>(gsmem_raw, (uint32_t)g.n_stages, g.b_stage);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
+    const int BN = g.N_pad;
     const int n_tiles = (g.M + kGemmBM - 1) / kGemmBM;
-    const int n_kblk = g.K / BK;
+    const int n_kblk = g.K / PlaneFmt<FMT>::BK;
     // Work units: a tile, or its column units of at most kUnitN columns ([0, 128), [128, 256), ... with split accumulators; [0, 256) and
     // [256, BN) for outputs wider than 256 columns).  Both roles enumerate the same sequence.
     constexpr int kUnitN = SPLIT ? 128 : 256;
@@ -445,20 +518,11 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     };
 
     if (threadIdx.x == 0) {
-        for (uint32_t s = 0; s < kStages; ++s) {
-            g_mbar_init(&full[s], 1);
-            g_mbar_init(&empty[s], 8);  // one arrival per consumer warp
-        }
+        init_ring_barriers(s.full, s.empty, (uint32_t)g.n_stages);
         g_mbar_init_fence();
     }
-    if (g.pdl) {
-        // programmatic dependent launch: this grid may have become resident (barrier init above) while the previous kernel
-        // of the stream was still draining its last tiles; let OUR successor do the same, then wait until the predecessor's results are
-        // visible -- nothing above this line reads global memory, everything below may
-        asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        asm volatile("griddepcontrol.wait;" ::: "memory");
-    }
-    for (int t = threadIdx.x; t < 256; t += blockDim.x) bias_s[t] = (g.bias && t < g.N) ? g.bias[t] : 0.f;
+    pdl_enter();  // nothing above reads global memory, everything below may
+    for (int t = threadIdx.x; t < 256; t += blockDim.x) s.bias[t] = (g.bias && t < g.N) ? g.bias[t] : 0.f;
     __syncthreads();
 
     if (warp >= 8) {
@@ -467,33 +531,12 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         if (warp == 8 && lane == 0) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-            uint32_t stage = 0, phase = 0;
+            Ring ring((uint32_t)g.n_stages);
             long long w_empty = 0;
-            const uint64_t pol_a = l2_policy_evict_first(), pol_b = l2_policy_evict_last();
             for (int u = blockIdx.x; u < n_work; u += gridDim.x) {
                 int tile, n_begin, n_cnt;
                 unit_of(u, tile, n_begin, n_cnt);
-                const int row0 = tile * kGemmBM;
-                const uint32_t b_plane = (uint32_t)n_cnt * ROWB;
-                for (int kb = 0; kb < n_kblk; ++kb) {
-                    const long long c0 = g.stats ? clock64() : 0;
-                    g_mbar_wait(&empty[stage], phase ^ 1u);
-                    if (g.stats) w_empty += clock64() - c0;
-                    g_mbar_expect_tx(&full[stage], a_stage_bytes + (uint32_t)P * b_plane);
-                    uint8_t* bs = smB + stage * b_stage_stride;
-                    if (g.l2_hint) tma_load_3d_hint(smA + stage * a_stage_bytes, &tmA, &full[stage], kb * BK, row0, 0, pol_a);
-                    else tma_load_3d(smA + stage * a_stage_bytes, &tmA, &full[stage], kb * BK, row0, 0);
-                    for (int p = 0; p < P; ++p)
-                        for (int r = 0; r < n_cnt; r += kGemmBoxN) {
-                            uint8_t* dst = bs + (uint32_t)p * b_plane + (uint32_t)r * ROWB;
-                            if (g.l2_hint) tma_load_3d_hint(dst, &tmB, &full[stage], kb * BK, n_begin + r, p, pol_b);
-                            else tma_load_3d(dst, &tmB, &full[stage], kb * BK, n_begin + r, p);
-                        }
-                    if (++stage == kStages) {
-                        stage = 0;
-                        phase ^= 1u;
-                    }
-                }
+                w_empty += load_unit<FMT>(s, ring, &tmA, &tmB, tile * kGemmBM, n_begin, n_cnt, n_kblk, g.stats != nullptr);
             }
             if (g.stats) atomicAdd(&g.stats[2], (unsigned long long)w_empty);
         }
@@ -501,7 +544,7 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         // ================= consumer warpgroups (warps 0..7) =================
         warpgroup_reg_inc<kGemmConsumerRegs>();
         const int wg = warp >> 2;
-        uint8_t* my_stage = stage_c + warp * 2 * L::kStageC;
+        uint8_t* my_stage = s.c + warp * 2 * L::kStageC;
         uint32_t n_stored = 0;
         // x = acc / (sA sB) + bias; when only planes are written (the hidden layers) the output scale is FOLDED into the two constants:
         // fold * x = acc * (fold / (sA sB)) + fold * bias (exact, powers of two), and max / mask commute with a positive factor
@@ -510,13 +553,13 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         const bool folded = EPI == kEpiPlain && g.c_f32 == nullptr;
         const float fold = folded ? c_mul : 1.0f;
         if (warp == 0 && folded)  // (bias_s was filled before the CTA barrier; one warp rescales it)
-            for (int t = lane; t < 256; t += 32) bias_s[t] *= fold;
-        asm volatile("bar.sync 1, 256;" ::: "memory");  // the 8 consumer warps only
+            for (int t = lane; t < 256; t += 32) s.bias[t] *= fold;
+        bar_sync_named(1, 256);  // the 8 consumer warps only
         EpiArgs e;
         e.M = g.M; e.N = g.N;
         e.k_acc = fold / (ld_scale(g.a_scale) * ld_scale(g.b_scale));
         e.c_mul = folded ? 1.0f : c_mul;
-        e.bias_s = bias_s; e.relu = g.relu; e.bits_in = g.bits_in; e.bits_out = g.bits_out; e.bits_ld = g.bits_ld; e.mask = g.mask;
+        e.bias_s = s.bias; e.relu = g.relu; e.bits_in = g.bits_in; e.bits_out = g.bits_out; e.bits_ld = g.bits_ld; e.mask = g.mask;
         e.ld_mask = g.ld_mask; e.c_f32 = g.c_f32; e.ldc = g.ldc; e.planes = g.c_planes != nullptr; e.ldp = g.ldp;
         uint32_t key0 = 0, key1 = 0, ctr0 = 0;
         if constexpr (EPI == kEpiLn) {
@@ -529,49 +572,23 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         }
         float amax = 0.f;
         float acc[128];
-        uint32_t stage = 0, phase = 0;
+        Ring ring((uint32_t)g.n_stages);
         long long w_full = 0, busy = 0;
-        long long* wc = g.stats ? &w_full : nullptr;
         const long long t_begin = g.stats ? clock64() : 0;
         for (int u = blockIdx.x; u < n_work; u += gridDim.x) {
             int tile, n_begin, n_cnt;
             unit_of(u, tile, n_begin, n_cnt);
-#define MORL_UNIT(N_) \
-    case N_: mma_unit<FMT, N_, SPLIT>(acc, smA, smB, a_stage_bytes, b_stage_stride, n_kblk, full, empty, stage, phase, kStages, wg, lane, wc); break;
-            switch (n_cnt) {
-                MORL_UNIT(32) MORL_UNIT(64) MORL_UNIT(96) MORL_UNIT(128)
-                default:
-                    if constexpr (!SPLIT) {
-                        switch (n_cnt) {
-                            MORL_UNIT(160) MORL_UNIT(192) MORL_UNIT(224) MORL_UNIT(256)
-                            default: __trap();
-                        }
-                    } else {
-                        __trap();
-                    }
-            }
-#undef MORL_UNIT
-            const long long c1 = g.stats ? clock64() : 0;
-            if (wide) {
-                // this unit's biases (times the folded output scale), indexed by output column: every consumer warp has left the previous
-                // unit's epilogue (both warpgroups have finished the MMAs of this unit)
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-                const int col = n_begin + (int)threadIdx.x;
-                bias_s[threadIdx.x] = (g.bias && col < g.N) ? g.bias[col] * fold : 0.f;
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-                e.bias_s = bias_s - n_begin;
-            }
             const int rbase = tile * kGemmBM + wg * 64 + (warp & 3) * 16;
-            if constexpr (EPI == kEpiLn) ln_dropout_unit(acc, n_cnt, rbase, lane, bias_s, e.k_acc, g, key0, key1, ctr0);
-#pragma unroll
-            for (int c = 0; c < (SPLIT ? 4 : 8); ++c) {
-                if (32 * c < n_cnt) {
-                    float a[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) a[j] = SPLIT ? __fadd_rn(acc[16 * c + j], acc[64 + 16 * c + j]) : acc[16 * c + j];
-                    epilogue_chunk<FMT, EPI == kEpiLn>(a, n_begin + 32 * c, rbase, lane, e, &tmC, my_stage, n_stored, amax);
+            long long c1 = 0;
+            consume_unit<FMT, SPLIT, EPI == kEpiLn>(acc, s, ring, n_kblk, n_begin, n_cnt, rbase, wg, lane, g.stats ? &w_full : nullptr, [&] {
+                c1 = g.stats ? clock64() : 0;
+                if (wide) {
+                    // this unit's biases (times the folded output scale), indexed by output column: both warpgroups have finished the MMAs of this unit
+                    reload_bias(s.bias, g.bias, n_begin, g.N, fold);
+                    e.bias_s = s.bias - n_begin;
                 }
-            }
+                if constexpr (EPI == kEpiLn) ln_dropout_unit(acc, n_cnt, rbase, lane, s.bias, e.k_acc, g, key0, key1, ctr0);
+            }, e, &tmC, my_stage, n_stored, amax);
             if (g.stats) busy += clock64() - c1;
         }
         if (g.stats && warp == 0 && lane == 0) {
@@ -591,9 +608,9 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 // first layer's input is read from HBM, and the launch prologue / drain is paid once instead of per layer.  Work of a CTA: its tiles in
 // groups of `lanes / n_chains`; per group, for every layer, one unit per LANE (lane = (chain, tile
 // of the group)): four lanes keep the dependency distance at four units (unit (l, lane) needs the stores of unit (l-1, lane)), so the
-// producer never waits for the epilogue that has just finished.  Same roles, barriers and arithmetic as gemm_planes_kernel<FMT, 0>
-// (bit-identical outputs: tests/test_gemm_gpu.py); additional barrier stored[lane]: the consumer warps arrive once their bulk
-// stores of the unit have COMPLETED, the producer waits for it before loading the next layer of that lane.
+// producer never waits for the epilogue that has just finished.  The shared-memory carve, the producer's load_unit and the consumer's
+// consume_unit are those of gemm_planes_kernel<FMT, 0> (bit-identical outputs: tests/test_gemm_gpu.py); additional barrier stored[lane]: the
+// consumer warps arrive once their bulk stores of the unit have COMPLETED, the producer waits for it before loading the next layer of that lane.
 // =================================================================================================================
 constexpr int kChainMaxJobs = 8;   // chains x layers
 constexpr int kChainLanes = 4;
@@ -615,37 +632,22 @@ struct ChainArgs {
     const float* a_scale;          // activation scale (input AND output of every layer), device scalar or nullptr
     int relu;                      // max(x, 0) on every job's output (forward chains)
     int n_stages;
-    int pdl;
 };
 
 template <int FMT>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
-    using F = PlaneFmt<FMT>;
     using L = KPlan<FMT>;
-    constexpr int P = F::P;
-    constexpr int BK = F::BK;
     constexpr int BN = 256;
-    constexpr int kMaxStages = L::kMaxStages;
-    constexpr uint32_t ROWB = L::kRowB;
-    const uint32_t kStages = (uint32_t)g.n_stages;
     extern __shared__ uint8_t gsmem_raw[];
-    uint8_t* gsmem = gsmem_raw + ((1024u - (g_smem_u32(gsmem_raw) & 1023u)) & 1023u);
-    constexpr uint32_t a_stage_bytes = L::kAStage;
-    constexpr uint32_t b_stage_bytes = L::kBStage;
-    uint8_t* smA = gsmem;
-    uint8_t* smB = gsmem + kStages * a_stage_bytes;
-    uint8_t* stage_c = gsmem + L::kOffC;
-    uint64_t* full = reinterpret_cast<uint64_t*>(gsmem + L::kOffBar);
-    uint64_t* empty = full + kMaxStages;
-    uint64_t* stored = empty + kMaxStages;  // [kChainLanes]
-    float* bias_s = reinterpret_cast<float*>(gsmem + L::kOffBias);  // [256], refilled per unit by the consumer warps
+    const KSmem s = carve_kplan<FMT>(gsmem_raw, (uint32_t)g.n_stages, L::kBStage);
+    uint64_t* stored = s.empty + L::kMaxStages;  // [kChainLanes]
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int unit = blockIdx.x, n_units = gridDim.x;
     const int n_tiles = (g.M + kGemmBM - 1) / kGemmBM;
-    const int n_kblk_full = g.K / BK, n_kblk_first = g.k_first / BK;
+    const int n_kblk_full = g.K / PlaneFmt<FMT>::BK, n_kblk_first = g.k_first / PlaneFmt<FMT>::BK;
     const int tiles_per_group = kChainLanes / g.n_chains;  // lanes of a group: (tile of the group) x (chain)
     // Tile t of chain c goes to CTA (t + offset_c) mod n_units with a DIFFERENT rotation per chain: when the tiles do not divide evenly, both
     // chains on the same CTAs would give some CTAs two extra tiles and others none; rotated by half the grid the remainders spread.
@@ -661,24 +663,18 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
     };
 
     if (threadIdx.x == 0) {
-        for (uint32_t s = 0; s < kStages; ++s) {
-            g_mbar_init(&full[s], 1);
-            g_mbar_init(&empty[s], 8);
-        }
-        for (int s = 0; s < kChainLanes; ++s) g_mbar_init(&stored[s], 8);  // the 8 consumer warps
+        init_ring_barriers(s.full, s.empty, (uint32_t)g.n_stages);
+        for (int i = 0; i < kChainLanes; ++i) g_mbar_init(&stored[i], 8);  // the 8 consumer warps
         g_mbar_init_fence();
     }
-    if (g.pdl) {
-        asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        asm volatile("griddepcontrol.wait;" ::: "memory");
-    }
+    pdl_enter();
     __syncthreads();
 
     if (warp >= 8) {
         // ================= producer warpgroup: one lane issues TMA =================
         warpgroup_reg_dec<kGemmProducerRegs>();
         if (warp == 8 && lane == 0) {
-            uint32_t stage = 0, phase = 0;
+            Ring ring((uint32_t)g.n_stages);
             uint32_t done_on_lane[kChainLanes] = {0u, 0u, 0u, 0u};  // units already issued on each lane = completions of stored[lane] to expect
             for (int gi = 0; gi < n_groups; ++gi)
                 for (int l = 0; l < g.n_layers; ++l)
@@ -693,60 +689,37 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
                             asm volatile("fence.proxy.async.global;" ::: "memory");
                         }
                         ++done_on_lane[ln];
-                        const int row0 = tile * kGemmBM;
-                        const int n_kblk = l == 0 ? n_kblk_first : n_kblk_full;
-                        for (int kb = 0; kb < n_kblk; ++kb) {
-                            g_mbar_wait(&empty[stage], phase ^ 1u);
-                            g_mbar_expect_tx(&full[stage], a_stage_bytes + b_stage_bytes);
-                            tma_load_3d(smA + stage * a_stage_bytes, &maps.A[job], &full[stage], kb * BK, row0, 0);
-                            for (int p = 0; p < P; ++p)
-                                for (int r = 0; r < BN; r += kGemmBoxN)
-                                    tma_load_3d(smB + stage * b_stage_bytes + (uint32_t)(p * BN + r) * ROWB, &maps.B[job], &full[stage], kb * BK, r, p);
-                            if (++stage == kStages) {
-                                stage = 0;
-                                phase ^= 1u;
-                            }
-                        }
+                        load_unit<FMT>(s, ring, &maps.A[job], &maps.B[job], tile * kGemmBM, 0, BN, l == 0 ? n_kblk_first : n_kblk_full, false);
                     }
         }
     } else {
         // ================= consumer warpgroups (warps 0..7) =================
         warpgroup_reg_inc<kGemmConsumerRegs>();
         const int wg = warp >> 2;
-        uint8_t* my_stage = stage_c + warp * 2 * L::kStageC;
+        uint8_t* my_stage = s.c + warp * 2 * L::kStageC;
         uint32_t n_stored = 0;
         const float s_act = ld_scale(g.a_scale);
         float amax = 0.f;
         float acc[128];
-        uint32_t stage = 0, phase = 0;
+        Ring ring((uint32_t)g.n_stages);
         for (int gi = 0; gi < n_groups; ++gi)
             for (int l = 0; l < g.n_layers; ++l)
                 for (int ln = 0; ln < kChainLanes; ++ln) {
                     int job, tile;
                     unit_of(gi, l, ln, job, tile);
                     if (tile < 0) continue;
-                    // this unit's bias (times the folded output scale) into shared memory: every consumer warp has left the previous unit
-                    asm volatile("bar.sync 1, 256;" ::: "memory");
-                    bias_s[threadIdx.x] = (g.bias[job] ? __ldg(g.bias[job] + threadIdx.x) : 0.f) * s_act;
-                    asm volatile("bar.sync 1, 256;" ::: "memory");
+                    reload_bias(s.bias, g.bias[job], 0, BN, s_act);  // (times the folded output scale)
                     EpiArgs e;
                     e.M = g.M; e.N = BN;
                     // x * s_act = acc * (s_act / (s_act * sB)) + s_act * bias  (powers of two: exact), as gemm_planes_kernel's folded epilogue
                     e.k_acc = s_act / (s_act * ld_scale(g.b_scale[job]));
                     e.c_mul = 1.0f;
-                    e.bias_s = bias_s; e.relu = g.relu; e.bits_in = g.bits_in[job]; e.bits_out = g.bits_out[job]; e.bits_ld = relu_bits_words(BN);
+                    e.bias_s = s.bias; e.relu = g.relu; e.bits_in = g.bits_in[job]; e.bits_out = g.bits_out[job]; e.bits_ld = relu_bits_words(BN);
                     e.mask = nullptr; e.ld_mask = 0;
                     e.c_f32 = nullptr; e.ldc = 0; e.planes = 1; e.ldp = BN;
-                    mma_unit<FMT, BN, 0>(acc, smA, smB, a_stage_bytes, b_stage_bytes, l == 0 ? n_kblk_first : n_kblk_full, full, empty, stage, phase, kStages,
-                                         wg, lane, nullptr);
                     const int rbase = tile * kGemmBM + wg * 64 + (warp & 3) * 16;
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) {
-                        float a[16];
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) a[j] = acc[16 * c + j];
-                        epilogue_chunk<FMT>(a, 32 * c, rbase, lane, e, &maps.C[job], my_stage, n_stored, amax);
-                    }
+                    consume_unit<FMT, 0, false>(acc, s, ring, l == 0 ? n_kblk_first : n_kblk_full, 0, BN, rbase, wg, lane, nullptr, [] {}, e,
+                                                &maps.C[job], my_stage, n_stored, amax);
                     // the lane's next layer loads what this unit stored (bit masks included): signal once the bulk stores of this warp have completed
                     __syncwarp();
                     if (lane == 0) {
@@ -853,9 +826,7 @@ gemm_planes_mn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     constexpr int P = F::P;
     constexpr int kStages = F::kStagesMn;
     extern __shared__ uint8_t gsmem_raw[];
-    // 1 KB alignment by pointer arithmetic ON the shared array (not through an integer cast), so that the compiler keeps every derived
-    // pointer in the shared address space: through the cast the bias / staging accesses were generic LD.E / ST.E (long-scoreboard stalls)
-    uint8_t* gsmem = gsmem_raw + ((1024u - (g_smem_u32(gsmem_raw) & 1023u)) & 1023u);
+    uint8_t* gsmem = align_1k(gsmem_raw);
     constexpr uint32_t chunk_bytes = (uint32_t)P * kMnKT * 128u;   // one 64-element MN chunk, P planes
     constexpr uint32_t a_stage = 2u * chunk_bytes;
     constexpr uint32_t b_stage = 4u * chunk_bytes;                 // (allocated for a k unit of 256 columns)
@@ -870,7 +841,7 @@ gemm_planes_mn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     // 4 KB of 1.0: the B operand of the fused bias-gradient product  colsum(G) = G^T . ones  (N = 16; every element is 1,
     // so the swizzle pattern is irrelevant)
     uint8_t* ones_b = reinterpret_cast<uint8_t*>(empty + kStages);
-    uint32_t* ones = reinterpret_cast<uint32_t*>(ones_b + ((1024u - (g_smem_u32(ones_b) & 1023u)) & 1023u));
+    uint32_t* ones = reinterpret_cast<uint32_t*>(align_1k(ones_b));
     for (int t = threadIdx.x; t < 1024; t += blockDim.x) ones[t] = F::kOnes2;
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 
@@ -882,10 +853,7 @@ gemm_planes_mn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     const int n_kblk = (m_end - m_begin + kMnKT - 1) / kMnKT;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kStages; ++s) {
-            g_mbar_init(&full[s], 1);
-            g_mbar_init(&empty[s], 8);  // one arrival per consumer warp
-        }
+        init_ring_barriers(full, empty, kStages);
         g_mbar_init_fence();
     }
     __syncthreads();
@@ -1514,8 +1482,8 @@ static int make_plane_map_mn(CUtensorMap* map, int fmt, const void* base, int ro
 
 // CTAs of a split-K weight-gradient launch (one per SM); morl_gemm_mn_workspace_bytes and the launcher must agree on it
 static inline int mn_sm_count() {
-    const int n = morl_device_sm_count();
-    return n > 0 && n <= 256 ? n : 132;
+    const int n = sm_count();
+    return n <= 256 ? n : 132;  // (the column-sum tail of the workspace holds 256 splits)
 }
 
 static inline bool fmt_ok(int fmt) { return fmt == MORL_FMT_BF16X3 || fmt == MORL_FMT_F16X2; }
@@ -1589,11 +1557,7 @@ extern "C" int morl_gemm_planes_mn_f32(int fmt, const void* g_planes, long long 
     MORL_DISPATCH_FMT(fmt, {
         using F = PlaneFmt<kFmt>;
         const size_t smem = (size_t)F::kStagesMn * (6u * F::P * kMnKT * 128u) + 256 + 1024 + 64 + 1024 + 4096;
-        static bool attr_set = false;
-        if (!attr_set) {
-            cudaFuncSetAttribute(gemm_planes_mn_kernel<kFmt>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            attr_set = true;
-        }
+        set_smem_limit_once<gemm_planes_mn_kernel<kFmt>>(smem);
         launch_k(gemm_planes_mn_kernel<kFmt>, dim3(n_tiles * k_units * S), dim3(kGemmThreads), smem, st, tmA, tmB, g);
     });
     rc = check_launch("morl_gemm_planes_mn_f32");
@@ -1648,11 +1612,7 @@ extern "C" int morl_pairs_grad_reduce_planes(int fmt, const void* planes, long l
             float* partf = static_cast<float*>(workspace);
             const size_t smemf = (size_t)kPgrMaxB * 8 * 32 * 9 * sizeof(float);  // 73,728 B
             MORL_DISPATCH_FMT(fmt, {
-                static bool configured = false;
-                if (!configured) {
-                    cudaFuncSetAttribute(pairs_grad_reduce_fused_kernel<kFmt>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemf);
-                    configured = true;
-                }
+                set_smem_limit_once<pairs_grad_reduce_fused_kernel<kFmt>>(smemf);
                 launch_k(pairs_grad_reduce_fused_kernel<kFmt>, dim3(dim3((unsigned)nchf, (unsigned)((H + 255) / 256))), dim3(dim3(32, 8)), smemf, st, pl, plane_stride, B, W,
                                                                                                                                      H, bpc, dU, partf, scale);
             });
@@ -1797,25 +1757,10 @@ namespace morl {
 template <int FMT, int SPLIT, int EPI = kEpiPlain>
 static int launch_gemm_planes(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmArgs& g, int sms, cudaStream_t st) {
     constexpr size_t smem = KPlan<FMT>::kBytes;
-    static bool attr_set = false;
-    if (!attr_set) {
-        cudaFuncSetAttribute(gemm_planes_kernel<FMT, SPLIT, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        attr_set = true;
-    }
+    set_smem_limit_once<gemm_planes_kernel<FMT, SPLIT, EPI>>(smem);
     constexpr int kUnitN = SPLIT ? 128 : 256;  // column units per tile: as gemm_planes_kernel
     const int n_work = (g.M + kGemmBM - 1) / kGemmBM * ((g.N_pad + kUnitN - 1) / kUnitN);
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(n_work < sms ? n_work : sms);
-    cfg.blockDim = dim3(kGemmThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = g.pdl ? 1 : 0;
-    cudaLaunchKernelEx(&cfg, gemm_planes_kernel<FMT, SPLIT, EPI>, tmA, tmB, tmC, g);
+    launch_k_pdl(gemm_pdl_enabled(), gemm_planes_kernel<FMT, SPLIT, EPI>, dim3(n_work < sms ? n_work : sms), dim3(kGemmThreads), smem, st, tmA, tmB, tmC, g);
     return check_launch(EPI == kEpiLn ? "morl_gemm_planes_ln_f32" : "morl_gemm_planes_f32");
 }
 
@@ -1839,7 +1784,7 @@ static int gemm_planes_impl(int fmt, const void* a_planes, long long a_plane_str
     MORL_REQUIRE(fmt_ok(fmt), MORL_ERR_UNSUPPORTED, "%s: unknown plane format %d", name, fmt);
     MORL_REQUIRE(a_planes && b_planes && (c_f32 || c_planes), MORL_ERR_NULL, "%s: NULL pointer argument", name);
     MORL_REQUIRE(M > 0 && N > 0 && K > 0 && N_pad >= N, MORL_ERR_SHAPE, "%s: bad shape M=%d N=%d N_pad=%d K=%d", name, M, N, N_pad, K);
-    const int BK = fmt == MORL_FMT_F16X2 ? PlaneFmt<MORL_FMT_F16X2>::BK : PlaneFmt<MORL_FMT_BF16X3>::BK;
+    const int BK = fmt_bk(fmt);
     MORL_REQUIRE(K % BK == 0 && N_pad % 32 == 0 && N_pad <= 512, MORL_ERR_UNSUPPORTED,
                  "%s: need K %% %d == 0, N_pad %% 32 == 0, N_pad <= 512 (K=%d N_pad=%d)", name, BK, K, N_pad);
     MORL_REQUIRE(aligned16(a_planes) && aligned16(b_planes), MORL_ERR_ALIGN, "%s: operand planes must be 16-byte aligned", name);
@@ -1847,8 +1792,6 @@ static int gemm_planes_impl(int fmt, const void* a_planes, long long a_plane_str
     if (c_planes)
         MORL_REQUIRE(ldp % 32 == 0 && ldp >= N && ldp <= N_pad && aligned16(c_planes) && c_plane_stride % 8 == 0, MORL_ERR_SHAPE,
                      "%s: ldp=%d must be a multiple of 32 with N <= ldp <= N_pad", name, ldp);
-    int sms = morl_device_sm_count();
-    if (sms <= 0) sms = 132;
     CUtensorMap tmA, tmB;
     int rc = make_plane_map(&tmA, fmt, a_planes, M, K, a_plane_stride, kGemmBM, BK);
     MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "%s: cuTensorMapEncodeTiled(A) failed (%d)", name, rc);
@@ -1885,12 +1828,6 @@ static int gemm_planes_impl(int fmt, const void* a_planes, long long a_plane_str
     }
     g.a_scale = a_scale; g.b_scale = b_scale; g.c_scale = c_scale;
     g.reverse = reverse_tiles ? 1 : 0;
-    // programmatic dependent launch between consecutive GEMMs of a chain (MORL_GEMM_PDL=0 disables it)
-    static const bool want_pdl = [] { const char* e = getenv("MORL_GEMM_PDL"); return !(e && e[0] == '0'); }();
-    g.pdl = want_pdl ? 1 : 0;
-    // L2 eviction hints on the operand loads are opt-in (MORL_GEMM_L2HINT=1)
-    static const bool want_hint = [] { const char* e = getenv("MORL_GEMM_L2HINT"); return e && e[0] == '1'; }();
-    g.l2_hint = want_hint ? 1 : 0;
     static const bool want_stats = [] { const char* e = getenv("MORL_GEMM_STATS"); return e && e[0] == '1'; }();
     g.stats = nullptr;
     if (want_stats) {
@@ -1899,6 +1836,7 @@ static int gemm_planes_impl(int fmt, const void* a_planes, long long a_plane_str
         g.stats = static_cast<unsigned long long*>(sp);
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int sms = sm_count();
     // accumulator mode (see gemm_planes_kernel): per call; MORL_GEMM_SPLIT_ACC=0 / 1 overrides every call (A/B measurements)
     static const int split_env = [] { const char* e = getenv("MORL_GEMM_SPLIT_ACC"); return e ? (e[0] == '0' ? 0 : 1) : -1; }();
     if (lnd) {
@@ -1979,7 +1917,7 @@ extern "C" int morl_gemm_chain_f32(int fmt, int n_chains, int n_layers, const vo
                  "morl_gemm_chain_f32: need 1 <= n_chains <= 2 and n_chains * n_layers <= %d (got %d x %d)", kChainMaxJobs, n_chains, n_layers);
     MORL_REQUIRE(morl_gemm_chain_supported(fmt, M, K), MORL_ERR_UNSUPPORTED, "morl_gemm_chain_f32: unsupported configuration fmt=%d M=%d K=%d (256-wide layers, M >= 256)",
                  fmt, M, K);
-    const int BK = fmt == MORL_FMT_F16X2 ? PlaneFmt<MORL_FMT_F16X2>::BK : PlaneFmt<MORL_FMT_BF16X3>::BK;
+    const int BK = fmt_bk(fmt);
     if (k_first <= 0) k_first = K;
     MORL_REQUIRE(k_first % BK == 0 && k_first <= K, MORL_ERR_SHAPE, "morl_gemm_chain_f32: k_first=%d must be a multiple of %d and <= K", k_first, BK);
     ChainMaps maps;  // (host staging of the 3 x 8 tensor maps on this thread's stack -- the entry point stays re-entrant; copied into the kernel
@@ -2010,40 +1948,14 @@ extern "C" int morl_gemm_chain_f32(int fmt, int n_chains, int n_layers, const vo
             g.bits_in[job] = relu_bits_in ? static_cast<const uint32_t*>(relu_bits_in[job]) : nullptr;
             MORL_REQUIRE(aligned16(g.bits_out[job]) && aligned16(g.bits_in[job]), MORL_ERR_ALIGN, "morl_gemm_chain_f32: ReLU bit masks must be 16-byte aligned");
         }
-    g.n_stages = fmt == MORL_FMT_F16X2 ? KPlan<MORL_FMT_F16X2>::kStages : KPlan<MORL_FMT_BF16X3>::kStages;
-    static const bool want_pdl = [] { const char* e = getenv("MORL_GEMM_PDL"); return !(e && e[0] == '0'); }();
-    g.pdl = want_pdl ? 1 : 0;
-    int sms = morl_device_sm_count();
-    if (sms <= 0) sms = 132;
+    const int sms = sm_count();
     const int n_tiles = (M + kGemmBM - 1) / kGemmBM;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(n_tiles < sms ? n_tiles : sms);
-    cfg.blockDim = dim3(kGemmThreads);
-    cfg.stream = static_cast<cudaStream_t>(stream);
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = g.pdl ? 1 : 0;
-    if (fmt == MORL_FMT_F16X2) {
-        constexpr size_t smem = KPlan<MORL_FMT_F16X2>::kBytes;
-        static bool attr_set = false;
-        if (!attr_set) {
-            cudaFuncSetAttribute(gemm_chain_kernel<MORL_FMT_F16X2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            attr_set = true;
-        }
-        cfg.dynamicSmemBytes = smem;
-        cudaLaunchKernelEx(&cfg, gemm_chain_kernel<MORL_FMT_F16X2>, maps, g);
-    } else {
-        constexpr size_t smem = KPlan<MORL_FMT_BF16X3>::kBytes;
-        static bool attr_set = false;
-        if (!attr_set) {
-            cudaFuncSetAttribute(gemm_chain_kernel<MORL_FMT_BF16X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            attr_set = true;
-        }
-        cfg.dynamicSmemBytes = smem;
-        cudaLaunchKernelEx(&cfg, gemm_chain_kernel<MORL_FMT_BF16X3>, maps, g);
-    }
+    MORL_DISPATCH_FMT(fmt, {
+        constexpr size_t smem = KPlan<kFmt>::kBytes;
+        g.n_stages = KPlan<kFmt>::kStages;
+        set_smem_limit_once<gemm_chain_kernel<kFmt>>(smem);
+        launch_k_pdl(gemm_pdl_enabled(), gemm_chain_kernel<kFmt>, dim3(n_tiles < sms ? n_tiles : sms), dim3(kGemmThreads), smem,
+                     static_cast<cudaStream_t>(stream), maps, g);
+    });
     return check_launch("morl_gemm_chain_f32");
 }

@@ -51,23 +51,35 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
                  "r"(bytes), "r"(g_smem_u32(bar))
                  : "memory");
 }
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-    return p;
+// named barrier `id` over the first `count` threads of the CTA (barrier 0 is __syncthreads)
+__device__ __forceinline__ void bar_sync_named(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+
+// ---- TMA / mbarrier ring of the warp-specialised kernels: full[s] (one producer arrival + the transaction bytes) and empty[s] (one
+// arrival per consumer warp) for every stage s.  The producer waits on empty[stage] with parity `phase ^ 1`, a consumer on full[stage]
+// with `phase`; both walk the stages in the same order.
+struct Ring {
+    uint32_t depth, stage = 0, phase = 0;
+    __device__ __forceinline__ explicit Ring(uint32_t n) : depth(n) {}
+    __device__ __forceinline__ void advance() {
+        if (++stage == depth) {
+            stage = 0;
+            phase ^= 1u;
+        }
+    }
+};
+
+// by one thread, before g_mbar_init_fence
+__device__ __forceinline__ void init_ring_barriers(uint64_t* full, uint64_t* empty, uint32_t n_stages) {
+    for (uint32_t s = 0; s < n_stages; ++s) {
+        g_mbar_init(&full[s], 1);
+        g_mbar_init(&empty[s], 8);  // one arrival per consumer warp
+    }
 }
-__device__ __forceinline__ uint64_t l2_policy_evict_last() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-    return p;
-}
-// same, with an L2 eviction-priority hint (createpolicy): activations are read once (evict_first), weight planes by every tile (evict_last)
-__device__ __forceinline__ void tma_load_3d_hint(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, uint64_t policy) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(g_smem_u32(dst)),
-        "l"(map), "r"(g_smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "l"(policy)
-        : "memory");
-}
+
+// 1 KB alignment (TMA swizzle atoms) by pointer arithmetic ON the shared array, not through an integer cast, so that the compiler keeps
+// every derived pointer in the shared address space: through the cast the bias / staging accesses were generic LD.E / ST.E
+// (long-scoreboard stalls)
+__device__ __forceinline__ uint8_t* align_1k(uint8_t* smem) { return smem + ((1024u - (g_smem_u32(smem) & 1023u)) & 1023u); }
 
 // ---- warpgroup MMA (wgmma.mma_async, sm_90a): D[64 x N] (+)= A[64 x 16] . B[N x 16]^T, both operands through shared-memory descriptors, fp32
 // accumulators in the registers of the 128 threads of the warpgroup.  Thread t = 32 w + l of the warpgroup holds, for every 8-column group j,
@@ -253,6 +265,7 @@ static inline EncodeTiledFn get_encode_fn() {
 }
 
 static inline int fmt_planes(int fmt) { return fmt == MORL_FMT_F16X2 ? 2 : 3; }
+static inline int fmt_bk(int fmt) { return fmt == MORL_FMT_F16X2 ? PlaneFmt<MORL_FMT_F16X2>::BK : PlaneFmt<MORL_FMT_BF16X3>::BK; }
 static inline CUtensorMapDataType fmt_tm_type(int fmt) { return fmt == MORL_FMT_F16X2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16; }
 
 // [P][rows][K] plane tensor, box = P (or one plane) x box_rows x box_k elements, swizzle span = box_k * 2 bytes (64 or 128)

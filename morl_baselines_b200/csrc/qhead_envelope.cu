@@ -16,8 +16,6 @@
 //              (envelope_wp.cuh: weight-pair FMA-chain filter + exact re-check, first-occurrence ties) of the transitions t = group,
 //              group + 2, ... of the tile and writes  r + (1 - done) gamma Q_tg[b, j*, a*, :].  The producer stages the next tile meanwhile.
 // HBM traffic: the activation planes of both nets (2 x 4 B x B W x K), read once; roofline = HBM (DESIGN.md section 4.1b).
-#include <stdlib.h>
-
 #include "gemm_tc.cuh"
 #include "envelope_wp.cuh"
 
@@ -41,7 +39,6 @@ struct QHeadArgs {
     float gamma;
     int row_order;
     int reverse;
-    int pdl;
     float* target_out;            // [W*B, D]
     int32_t* pref_out;            // [W*B] or nullptr
     int32_t* act_out;             // [W*B] or nullptr
@@ -68,8 +65,6 @@ struct QhPlan {
     }
 };
 
-__device__ __forceinline__ void bar_sync_named(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-
 template <int FMT, int D, int MODE>
 __global__ void __launch_bounds__(kQhThreads, 1)
 qhead_envelope_kernel(const __grid_constant__ CUtensorMap tmA_on, const __grid_constant__ CUtensorMap tmA_tg, const __grid_constant__ CUtensorMap tmB_on,
@@ -79,10 +74,9 @@ qhead_envelope_kernel(const __grid_constant__ CUtensorMap tmA_on, const __grid_c
     constexpr int BK = F::BK;
     constexpr uint32_t ROWB = L::kRowB;
     const L plan(g.K, g.N, g.n_stages);
-    const uint32_t kStages = (uint32_t)g.n_stages;
     const int n_kblk = g.K / BK;
     extern __shared__ uint8_t qsmem_raw[];
-    uint8_t* sm = qsmem_raw + ((1024u - (g_smem_u32(qsmem_raw) & 1023u)) & 1023u);  // (pointer arithmetic on the shared array: see gemm_planes.cu)
+    uint8_t* sm = align_1k(qsmem_raw);
     uint8_t* smB = sm;
     uint8_t* smA = sm + plan.off_a;
     float* Qst = reinterpret_cast<float*>(sm + plan.off_q);  // [2 nets][128 rows][N]
@@ -96,17 +90,11 @@ qhead_envelope_kernel(const __grid_constant__ CUtensorMap tmA_on, const __grid_c
     const int N = g.N;
 
     if (threadIdx.x == 0) {
-        for (uint32_t s = 0; s < kStages; ++s) {
-            g_mbar_init(&full[s], 1);
-            g_mbar_init(&empty[s], 8);  // one arrival per consumer warp (both groups walk every stage)
-        }
+        init_ring_barriers(full, empty, (uint32_t)g.n_stages);  // (both groups walk every stage: 8 consumer warps arrive)
         g_mbar_init(bfull, 1);
         g_mbar_init_fence();
     }
-    if (g.pdl) {  // nothing above reads global memory; everything below may (see gemm_planes_kernel)
-        asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        asm volatile("griddepcontrol.wait;" ::: "memory");
-    }
+    pdl_enter();  // nothing above reads global memory; everything below may
     if (threadIdx.x < 2 * kQhBN) {
         const int net = threadIdx.x >> 5, n = threadIdx.x & 31;
         bias_s[threadIdx.x] = (g.bias[net] && n < N) ? g.bias[net][n] : 0.f;
@@ -122,18 +110,16 @@ qhead_envelope_kernel(const __grid_constant__ CUtensorMap tmA_on, const __grid_c
             for (int net = 0; net < g.n_nets; ++net)
                 for (int kb = 0; kb < n_kblk; ++kb)
                     tma_load_3d(smB + (uint32_t)(net * n_kblk + kb) * L::kBChunk, net ? &tmB_tg : &tmB_on, bfull, kb * BK, 0, 0);
-            uint32_t stage = 0, phase = 0;
+            Ring ring((uint32_t)g.n_stages);
             for (int u = blockIdx.x; u < g.n_tiles; u += gridDim.x) {
                 const int tile = g.reverse ? g.n_tiles - 1 - u : u;
                 for (int net = 0; net < g.n_nets; ++net) {
                     for (int kb = 0; kb < n_kblk; ++kb) {
-                        g_mbar_wait(&empty[stage], phase ^ 1u);
+                        const uint32_t stage = ring.stage;
+                        g_mbar_wait(&empty[stage], ring.phase ^ 1u);
                         g_mbar_expect_tx(&full[stage], L::kAStage);
                         tma_load_3d(smA + stage * L::kAStage, net ? &tmA_tg : &tmA_on, &full[stage], kb * BK, tile * kQhBM, 0);
-                        if (++stage == kStages) {
-                            stage = 0;
-                            phase ^= 1u;
-                        }
+                        ring.advance();
                     }
                 }
             }
@@ -152,7 +138,7 @@ qhead_envelope_kernel(const __grid_constant__ CUtensorMap tmA_on, const __grid_c
         auto sync_g = [&]() { bar_sync_named(2 + grp, 128); };
         constexpr uint32_t a_plane = kQhBM * ROWB, b_plane = kQhBN * ROWB;
         if (grp < g.n_nets) g_mbar_wait(bfull, 0);
-        uint32_t stage = 0, phase = 0;
+        Ring ring((uint32_t)g.n_stages);
         for (int u = blockIdx.x; u < g.n_tiles; u += gridDim.x) {
             const int tile = g.reverse ? g.n_tiles - 1 - u : u;
             // acc[mh]: rows [64 mh, 64 mh + 64) of the tile, 32 columns: the products of a K step in the order of gemm_planes_kernel, so the
@@ -162,7 +148,8 @@ qhead_envelope_kernel(const __grid_constant__ CUtensorMap tmA_on, const __grid_c
             for (int net = 0; net < g.n_nets; ++net) {
                 uint32_t prev = 0;
                 for (int kb = 0; kb < n_kblk; ++kb) {
-                    g_mbar_wait(&full[stage], phase);
+                    const uint32_t stage = ring.stage;
+                    g_mbar_wait(&full[stage], ring.phase);
                     if (net == grp) {
                         wgmma_fence();
                         const uint32_t a0 = g_smem_u32(smA + stage * L::kAStage);
@@ -188,10 +175,7 @@ qhead_envelope_kernel(const __grid_constant__ CUtensorMap tmA_on, const __grid_c
                     } else if (lane == 0) {
                         g_mbar_arrive(&empty[stage]);  // the other group's operand
                     }
-                    if (++stage == kStages) {
-                        stage = 0;
-                        phase ^= 1u;
-                    }
+                    ring.advance();
                 }
                 if (net == grp) {
                     wgmma_wait<0>();
@@ -269,24 +253,8 @@ qhead_envelope_kernel(const __grid_constant__ CUtensorMap tmA_on, const __grid_c
 template <int FMT, int D, int MODE>
 static int launch_qhead(const CUtensorMap& tmA_on, const CUtensorMap& tmA_tg, const CUtensorMap& tmB_on, const CUtensorMap& tmB_tg, const QHeadArgs& g,
                         size_t smem, int grid, cudaStream_t st) {
-    static bool attr_set = false;
-    auto kern = qhead_envelope_kernel<FMT, D, MODE>;
-    if (!attr_set) {
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        attr_set = true;
-    }
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3(kQhThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = g.pdl ? 1 : 0;
-    cudaLaunchKernelEx(&cfg, kern, tmA_on, tmA_tg, tmB_on, tmB_tg, g);
+    set_smem_limit_once<qhead_envelope_kernel<FMT, D, MODE>>(227 * 1024);
+    launch_k_pdl(gemm_pdl_enabled(), qhead_envelope_kernel<FMT, D, MODE>, dim3((unsigned)grid), dim3(kQhThreads), smem, st, tmA_on, tmA_tg, tmB_on, tmB_tg, g);
     return check_launch("morl_qhead_envelope_td_f32");
 }
 
@@ -345,18 +313,13 @@ extern "C" int morl_qhead_envelope_td_f32(int fmt, const void* a_on_planes, cons
     g.target_out = target_out; g.pref_out = pref_out; g.act_out = act_out;
     g.q_out[0] = q_on_out; g.q_out[1] = q_tg_out;
     g.n_nets = 2;
-    static const bool want_pdl = [] { const char* e = getenv("MORL_GEMM_PDL"); return !(e && e[0] == '0'); }();
-    g.pdl = want_pdl ? 1 : 0;
     // activation ring: as many stages as fit beside the resident weight planes, the Q tiles and the scan scratch
     int n_st = kQhMaxStages;
-    static const int st_env = [] { const char* e = getenv("MORL_QHEAD_STAGES"); return e ? atoi(e) : 0; }();
-    if (st_env > 0 && st_env < n_st) n_st = st_env;
     while (n_st > 1 && QhPlan<kFmt>(K, g.N, n_st).bytes > 227u * 1024u) --n_st;
     MORL_REQUIRE(QhPlan<kFmt>(K, g.N, n_st).bytes <= 227u * 1024u, MORL_ERR_UNSUPPORTED, "morl_qhead_envelope_td_f32: shared-memory plan does not fit");
     g.n_stages = n_st;
     const size_t smem = QhPlan<kFmt>(K, g.N, n_st).bytes;
-    int sms = morl_device_sm_count();
-    if (sms <= 0) sms = 132;
+    const int sms = sm_count();
     const int grid = g.n_tiles < sms ? g.n_tiles : sms;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     bool launched = false;
@@ -403,14 +366,11 @@ extern "C" int morl_qhead_gemm_f32(int fmt, const void* a_planes, long long a_pl
     g.reverse = reverse_tiles ? 1 : 0;
     g.q_out[0] = q_out;
     g.n_nets = 1;
-    static const bool want_pdl = [] { const char* e = getenv("MORL_GEMM_PDL"); return !(e && e[0] == '0'); }();
-    g.pdl = want_pdl ? 1 : 0;
     int n_st = kQhMaxStages;
     while (n_st > 1 && QhPlan<kFmt>(K, N, n_st).bytes > 227u * 1024u) --n_st;
     g.n_stages = n_st;
     const size_t smem = QhPlan<kFmt>(K, N, n_st).bytes;
-    int sms = morl_device_sm_count();
-    if (sms <= 0) sms = 132;
+    const int sms = sm_count();
     const int grid = g.n_tiles < sms ? g.n_tiles : sms;
     return launch_qhead<kFmt, 3, MORL_DOT_UNFUSED>(tmA, tmA, tmB, tmB, g, smem, grid, static_cast<cudaStream_t>(stream));
 }

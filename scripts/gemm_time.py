@@ -1,6 +1,7 @@
 """In-graph launch time of the dominant GEMM (bench.time_gemm_kernel) under the environment switches given on the command line, one
-subprocess per variant:   python scripts/gemm_time.py "" MORL_GEMM_SKIPB=1 MORL_GEMM_STAGES=2 "MORL_GEMM_SKIPB=1 MORL_GEMM_STAGES=2"
-(MORL_GEMM_SKIPB is a timing experiment with wrong results: how fast would the layer be if the weight planes stayed in shared memory?)"""
+subprocess per variant:
+    python scripts/gemm_time.py "" MORL_GEMM_STAGES=2 "MORL_GEMM_SPLIT_ACC=1 MORL_GEMM_STAGES=2"
+"""
 import os, subprocess, sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -343,10 +343,9 @@ def test_pairs_grad_reduce(cuda, fmt):
                 assert bool((err <= bound).all()), (H, B, W, axis, float((err / bound).max()))
 
 
-@pytest.mark.parametrize("env_flags", [{"MORL_GEMM_L2HINT": "1"}, {"MORL_GEMM_SPLIT_ACC": "1"}, {"MORL_GEMM_L2HINT": "1", "MORL_GEMM_SPLIT_ACC": "1"}])
+@pytest.mark.parametrize("env_flags", [{"MORL_GEMM_SPLIT_ACC": "1"}])
 def test_gemm_alternative_kernels_still_correct(cuda, env_flags):
-    """MORL_GEMM_L2HINT=1 puts L2 eviction hints on the operand loads and MORL_GEMM_SPLIT_ACC=1
-    forces the split-accumulator mode on every call (a 256-wide output then runs as two 128-column units, a 160-wide one as 128 + 32) -- cross-checks.  The switches are read once per process, hence the subprocess."""
+    """MORL_GEMM_SPLIT_ACC=1 forces the split-accumulator mode on every call (a 256-wide output then runs as two 128-column units, a 160-wide one as 128 + 32) -- cross-checks.  The switches are read once per process, hence the subprocess."""
     import os
     import subprocess
     import sys
