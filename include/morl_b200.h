@@ -183,6 +183,38 @@ MORL_API int morl_td_huber_priority_f32(const float* q_values, int n_nets, const
                                float* grad_q, float* prio_out, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Discrete-action MOSAC (single_policy/ser/mosac_discrete_action.py).  A fourth "min over critics" rule next to the three of
+ * morl_actor_critic_td_f32: the soft value is an expectation under the actor's softmax over ALL actions, not a value at one
+ * sampled action.  Shapes: q_nets f32 [n_nets, N, A, D]; logits f32 [N, A]; w [w_rows, D] under w_map; A <= 256, D <= 8 (larger
+ * shapes return MORL_ERR_UNSUPPORTED).  alpha (and log_alpha) are DEVICE f32 [1], read at run time, so a captured CUDA graph stays
+ * valid while the temperature is tuned.  Per row k, actions walked in ascending order:
+ *   mx = max_a x[a] (NaN propagates);  s = sum_a e^(x[a] - mx);  logp[a] = (x[a] - mx) - log s;  p[a] = e^(x[a] - mx) / s
+ *     (torch's max-subtracted log_softmax / softmax; e^ and log are the library's own portable fp32 routines, <= 2 ulp)
+ *   m[a] = min_n (w . q_n[k, a, :])  scalarised in MORL_DOT_UNFUSED, the arithmetic morl_actor_critic_td_f32 uses for MOSAC's
+ *     th.matmul; the min follows th.min and PROPAGATES NaN (unlike the fminf of MORL_AC_SCALAR_MIN, which ignores a NaN operand)
+ *   -inf logit: p[a] = 0 and logp[a] = -inf; such an action is left out of every sum below and its gradient is 0 (the reference
+ *     would compute 0 * -inf = NaN and poison the row).  A row whose max is +-inf or NaN is NaN throughout, as in torch.
+ * morl_discrete_sac_target_f32 (:452-464):
+ *   v = sum_a p[a] * (m[a] - alpha * logp[a]);  target_out[k] = w.r + ((1 - done) * gamma) * v     reward f32 [N, D], done f32 [N]
+ * morl_discrete_sac_actor_loss_f32 (:478-498), q_nets the ONLINE critics at s evaluated after the critic step:
+ *   f[a] = alpha * logp[a] - m[a];  l_k = sum_a p[a] f[a]
+ *   actor_loss_out[0] = sum_k l_k / (N*A)          (the reference's .mean() of a [N, A] tensor)
+ *   dlogits [N, A] (or NULL) = p[a] * (f[a] - l_k) / (N*A)   (closed form: softmax Jacobian with sum_a p = 1)
+ *   log_alpha non-NULL (autotune): t = -e^log_alpha, u[a] = logp[a] + target_entropy,
+ *     alpha_loss_out[0] = sum_k sum_a p[a] * (t * u[a]) / (N*A);  dlog_alpha_out[0] = t * sum_k sum_a p[a] u[a] / (N*A)
+ *   Row sums are reduced deterministically: fixed 256-row block partials in float, then one final sum in double.
+ *   workspace: device scratch of morl_discrete_sac_workspace_bytes(N) bytes (no initialisation required)
+ */
+MORL_API int morl_discrete_sac_target_f32(const float* q_nets, int n_nets, const float* logits, const float* w, int w_rows, int w_map,
+                                          const float* reward, const float* done, const float* alpha, float gamma, int N, int A, int D,
+                                          float* target_out, void* stream);
+MORL_API size_t morl_discrete_sac_workspace_bytes(int n_rows);
+MORL_API int morl_discrete_sac_actor_loss_f32(const float* logits, const float* q_nets, int n_nets, const float* w, int w_rows,
+                                              int w_map, const float* alpha, const float* log_alpha, float target_entropy, int N,
+                                              int A, int D, float* actor_loss_out, float* dlogits, float* alpha_loss_out,
+                                              float* dlog_alpha_out, void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Host halves of the replay path (CPU code in the same library; no CUDA call, usable without a device).
  *
  * Prioritised replay sum tree, reference common/prioritized_buffer.py:12-82 (class SumTree).  `tree` is ONE float64 array of

@@ -36,6 +36,9 @@ SIGNATURES = {
     "morl_td_workspace_bytes": (_sz, [_i]),
     "morl_td_mse_priority_f32": (_i, [_vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "morl_td_huber_priority_f32": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp, _i, _i, _f, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "morl_discrete_sac_target_f32": (_i, [_vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _f, _i, _i, _i, _vp, _vp]),
+    "morl_discrete_sac_workspace_bytes": (_sz, [_i]),
+    "morl_discrete_sac_actor_loss_f32": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _vp, _f, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "morl_host_sumtree_walk": (_i, [_vp, _i, _vp, _i, _vp]),
     "morl_host_sumtree_batch_set": (_i, [_vp, _i, _vp, _vp, _i]),
     "morl_host_gather_rows": (_i, [_vp, C.c_longlong, _vp, _i, _vp]),

@@ -1,15 +1,15 @@
 """MORL/D (decomposition-based MORL) on the CUDA update engine -- drop-in for reference
-morl_baselines/multi_policy/morld/morld.py with MOSAC inner learners (config 5 of BASELINE.json).
+morl_baselines/multi_policy/morld/morld.py with MOSAC or MOSACDiscrete inner learners (config 5 of BASELINE.json).
 
 What changes under the API (SURVEY.md section 8, rows a13, a18, a19 and 8(e)):
   * the population shards across GPUs: policy p lives on rank ``p % world`` (one process per GPU, torch.distributed / NCCL);
-    ``__update_others`` -- the strictly serial ``update_passes x (pop-1)`` MOSAC updates of the reference (morld.py:423-433) --
+    ``__update_others`` -- the strictly serial ``update_passes x (pop-1)`` learner updates of the reference (morld.py:423-433) --
     runs only over the rank's own policies, with no communication;
   * once per evaluation round every rank prunes its local evaluations + archive with the CUDA dominance kernel and the ranks
     exchange the fronts with ONE all-gather (parallel.allgather_fronts); every rank then holds the identical global front
     used for the metrics (hypervolume etc.);
   * ParetoArchive.add re-filters on the GPU (common/pareto.py).
-Inner learners other than MOSAC (MOSACDiscrete, EUPG: reference morld.py:30-34) are outside the accelerated path.
+EUPG, the reference's third inner learner (morld.py:30-34), is an on-policy ESR learner and is outside the accelerated path.
 Single-process behaviour (world size 1) is the reference's.
 """
 
@@ -33,8 +33,9 @@ from ...common.utils import nearest_neighbors
 from ...common.weights import equally_spaced_weights, random_weights
 from ...parallel import allgather_fronts
 from ...single_policy.ser.mosac_continuous_action import MOSAC
+from ...single_policy.ser.mosac_discrete_action import MOSACDiscrete
 
-POLICIES = {"MOSAC": MOSAC}
+POLICIES = {"MOSAC": MOSAC, "MOSACDiscrete": MOSACDiscrete}
 
 
 class Policy:
@@ -130,7 +131,8 @@ class MORLD(MOAgent):
         if self.transfer:
             self.experiment_name += "+transfer"
         if policy_name not in POLICIES:
-            raise NotImplementedError(f"inner policy {policy_name!r} is outside the accelerated path (only MOSAC; SURVEY.md section 2 #29)")
+            raise NotImplementedError(f"inner policy {policy_name!r} is outside the accelerated path (MOSAC and MOSACDiscrete only; "
+                                      "EUPG is an on-policy ESR learner, SURVEY.md section 2 #29)")
         self.policy_factory = POLICIES[policy_name]
         self.policy_name = policy_name
         self.policy_args = policy_args
@@ -239,10 +241,11 @@ class MORLD(MOAgent):
                     dst_policy = self.population[n]
                     dst = dst_policy.wrapped.get_policy_net()
                     polyak_update(params=src.parameters(), target_params=dst.parameters(), tau=1.0)
-                    if hasattr(dst_policy.wrapped, "_graphs"):  # MOSAC: capture-safe fused Adam; captured graphs reference the old optimiser
+                    if hasattr(dst_policy.wrapped, "_graphs"):  # MOSAC(Discrete): capture-safe fused Adam; captured graphs reference the old optimiser
                         from ...common.fused_adam import FusedClipAdam
 
-                        dst_policy.wrapped.actor_optimizer = FusedClipAdam(dst.parameters(), lr=dst_policy.wrapped.policy_lr)
+                        eps = getattr(dst_policy.wrapped, "ADAM_EPS", 1e-8)  # MOSACDiscrete's optimisers all use eps 1e-4, as its reference
+                        dst_policy.wrapped.actor_optimizer = FusedClipAdam(dst.parameters(), lr=dst_policy.wrapped.policy_lr, eps=eps)
                         dst_policy.wrapped._graphs = {}
                     else:
                         dst_policy.wrapped.actor_optimizer = optim.Adam(dst.parameters(), lr=dst_policy.wrapped.policy_lr)

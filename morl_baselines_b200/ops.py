@@ -151,6 +151,61 @@ def actor_critic_td(q_nets, w, reward, done, logp, alpha: float, gamma: float, v
     return out
 
 
+def _discrete_sac_args(q_nets, logits, w, alpha):
+    q_nets, logits = _dev(q_nets, "q_nets"), _dev(logits, "logits")
+    if q_nets.dim() != 4 or logits.dim() != 2:
+        raise _lib.MorlB200Error(f"q_nets must be [n_nets, N, A, D] and logits [N, A], got {tuple(q_nets.shape)} and {tuple(logits.shape)}")
+    n_nets, N, A, D = q_nets.shape
+    if tuple(logits.shape) != (N, A):
+        raise _lib.MorlB200Error(f"logits {tuple(logits.shape)} do not match q_nets {tuple(q_nets.shape)}")
+    w = _rows(w, D, "w")
+    alpha = _dev(alpha, "alpha").reshape(-1)
+    if alpha.numel() != 1:
+        raise _lib.MorlB200Error("alpha must be a device tensor with one element")
+    return q_nets, logits, w, alpha, (n_nets, N, A, D)
+
+
+def discrete_sac_target(q_nets, logits, w, reward, done, alpha: th.Tensor, gamma: float, w_map: int = MAP_BLOCK, out: Optional[th.Tensor] = None):
+    """Discrete-action MOSAC soft target (reference mosac_discrete_action.py:452-464): q_nets [n_nets, N, A, D] target critics at s',
+    logits [N, A] actor at s', ``alpha`` a device scalar read at run time.  Returns target [N]."""
+    q_nets, logits, w, alpha, (n_nets, N, A, D) = _discrete_sac_args(q_nets, logits, w, alpha)
+    reward, done = _dev(reward, "reward").reshape(-1, D), _dev(done, "done").reshape(-1)
+    if reward.shape[0] != N or done.shape[0] != N:
+        raise _lib.MorlB200Error(f"reward / done must have {N} rows, got {reward.shape[0]} / {done.shape[0]}")
+    out = th.empty(N, device=q_nets.device, dtype=th.float32) if out is None else out
+    rc = _lib.load().morl_discrete_sac_target_f32(_ptr(q_nets), n_nets, _ptr(logits), _ptr(w), w.shape[0], w_map, _ptr(reward), _ptr(done),
+                                                  _ptr(alpha), float(gamma), N, A, D, _ptr(out), _stream())
+    _lib.check(rc, "morl_discrete_sac_target_f32")
+    _count()
+    return out
+
+
+def discrete_sac_actor_loss(logits, q_nets, w, alpha: th.Tensor, log_alpha: Optional[th.Tensor] = None, target_entropy: float = 0.0,
+                            w_map: int = MAP_BLOCK, want_grad: bool = True, workspace: Optional[th.Tensor] = None):
+    """Discrete-action MOSAC actor loss, d loss / d logits and, with ``log_alpha``, the temperature loss and its derivative w.r.t.
+    log_alpha (reference mosac_discrete_action.py:478-498).  Returns (actor_loss [1], dlogits [N, A] or None, alpha_loss [1] or None,
+    dlog_alpha [1] or None)."""
+    q_nets, logits, w, alpha, (n_nets, N, A, D) = _discrete_sac_args(q_nets, logits, w, alpha)
+    if log_alpha is not None:
+        log_alpha = _dev(log_alpha, "log_alpha").reshape(-1)
+        if log_alpha.numel() != 1:
+            raise _lib.MorlB200Error("log_alpha must be a device tensor with one element")
+    dev = logits.device
+    loss = th.empty(1, device=dev, dtype=th.float32)
+    grad = th.empty_like(logits) if want_grad else None
+    aloss = th.empty(1, device=dev, dtype=th.float32) if log_alpha is not None else None
+    dla = th.empty(1, device=dev, dtype=th.float32) if log_alpha is not None else None
+    if workspace is None:
+        nbytes = _lib.load().morl_discrete_sac_workspace_bytes(N)
+        workspace = th.empty((nbytes + 3) // 4, device=dev, dtype=th.float32)
+    rc = _lib.load().morl_discrete_sac_actor_loss_f32(_ptr(logits), _ptr(q_nets), n_nets, _ptr(w), w.shape[0], w_map, _ptr(alpha), _ptr(log_alpha),
+                                                      float(target_entropy), N, A, D, _ptr(loss), _ptr(grad), _ptr(aloss), _ptr(dla), _ptr(workspace),
+                                                      _stream())
+    _lib.check(rc, "morl_discrete_sac_actor_loss_f32")
+    _count(2)
+    return loss, grad, aloss, dla
+
+
 def td_workspace(n_rows: int, device) -> th.Tensor:
     nbytes = _lib.load().morl_td_workspace_bytes(int(n_rows))
     return th.empty((nbytes + 3) // 4, device=device, dtype=th.float32)

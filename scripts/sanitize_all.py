@@ -4,7 +4,7 @@
 
 groups: envelope td gemm optim pareto replay layer1 qhead dyna chain (default: all).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
 every code path: all envelope kernel families, both GEMM operand formats x CTA modes x accumulator modes, MN split-K GEMM with the fused
-column sums, every split / reduction helper, the loss kernels, Adam, polyak, Pareto + front records, replay gather."""
+column sums, every split / reduction helper, the loss kernels (discrete SAC's included), Adam, polyak, Pareto + front records, replay gather."""
 import os
 import sys
 
@@ -57,6 +57,11 @@ if "td" in groups:
     act2 = th.randint(0, A, (B // 2,), device=dev, generator=g, dtype=th.int32)
     ops.td_huber_priority(rn(2, B, A, D, scale=0.02), act2, rn(B, D, scale=0.02), rn(B, D, scale=0.02), th.rand(B, D, device=dev, generator=g), 0.01, B // 2)
     ops.actor_critic_td(rn(2, B, D), th.rand(D, device=dev, generator=g), rn(B, D), th.zeros(B, 1, device=dev), rn(B, 1), 0.2, 0.99, ops.AC_SCALAR_MIN)
+    alpha, log_alpha = th.full((1,), 0.2, device=dev), th.full((1,), -0.5, device=dev)
+    for n_nets, Nd, Ad in [(2, 300, 6), (1, 40, 256)]:  # two blocks with a ragged tail; the widest action count
+        qd, ld, wd = rn(n_nets, Nd, Ad, D), rn(Nd, Ad), th.rand(D, device=dev, generator=g)
+        ops.discrete_sac_target(qd, ld, wd, rn(Nd, D), th.zeros(Nd, device=dev), alpha, 0.99)
+        ops.discrete_sac_actor_loss(ld, qd, wd, alpha, log_alpha, 0.9)
     th.cuda.synchronize()
     print("td ok")
 
