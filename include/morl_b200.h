@@ -269,6 +269,17 @@ MORL_API int morl_front_unpack_f64(const double* gathered, int world, int d, int
  * `ref` in every objective contribute nothing; dominated points are harmless (the volume is that of the union of boxes). */
 MORL_API int morl_hypervolume_f64(const double* pts, const uint8_t* keep, int n, int d, const double* ref, double* out, void* stream);
 
+/* Corner weights of a convex coverage set (OLS / GPI-LS weight selection).  Replaces compute_corner_weights
+ * (multi_policy/linear_support/linear_support.py:295-349), which enumerates with cdd the vertices of
+ *   { (w, u) : V w <= u 1,  w >= 0,  sum w = 1 }.
+ * Exact enumeration over the C(n+d, d) d-subsets of the n + d inequality rows, one d x d float64 solve each; a degenerate vertex is
+ * emitted once (by its lexicographically first basis).  V : f64 [n, d] row-major (the caller rounds it, np.round(., 4));
+ * verts : f64 [cap, d+1], (w, u) per vertex in no particular order (may be NULL iff cap == 0); count : device int [1] = number of
+ * vertices found, NOT clipped to cap (grow the buffer and launch again).  2 <= d <= MORL_MAX_D, n >= 1, and
+ * C(n+d, d) <= MORL_CORNER_MAX_CANDIDATES (2^31: e.g. d 6 with n <= 94, d 8 with n <= 58), else MORL_ERR_UNSUPPORTED. */
+#define MORL_CORNER_MAX_CANDIDATES 2147483648ULL
+MORL_API int morl_corner_weights_f64(const double* V, int n, int d, double* verts, int cap, int* count, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Multi-tensor target-network sync.  Replaces polyak_update (common/networks.py:121-139):
  *   tau == 1 : target <- param;  else target <- fma(tau, param, fl((1 - tau) * target))   (mul_ then ATen's fused add(alpha))

@@ -53,6 +53,7 @@ SIGNATURES = {
     "morl_front_pack_f64": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp]),
     "morl_front_unpack_f64": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "morl_hypervolume_f64": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "morl_corner_weights_f64": (_i, [_vp, _i, _i, _vp, _i, _vp, _vp]),
     "morl_polyak_f32": (_i, [_vp, _vp, _vp, _i, _i64, _d, _vp]),
     "morl_plane_overflow_count": (_i, [_i]),
     "morl_amax_scale_f32": (_i, [_vp, C.c_longlong, _i, _vp, _vp, _vp]),

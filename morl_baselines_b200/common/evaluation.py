@@ -58,7 +58,7 @@ def policy_evaluation_mo(agent, env, w: np.ndarray, scalarization=np.dot, rep: i
             np.mean([e[3] for e in evals], axis=0))
 
 
-def policy_evaluation_mo_batched(agent, env, weights: List[np.ndarray], rep: int = 5, seeds: Optional[List[int]] = None):
+def policy_evaluation_mo_batched(agent, env, weights: List[np.ndarray], rep: int = 5, seeds: Optional[List[int]] = None, weight_dtype=np.float32):
     """All ``len(weights) * rep`` evaluation episodes of an evaluation round in LOCKSTEP on copies of ``env`` (SURVEY.md 8(f)4): the
     reference evaluates one (weight, episode) after the other, one single-row network call per environment step
     (evaluation.py:118-144 called from a python loop, e.g. envelope.py:545-557: 100 weights x 5 episodes); here every environment step
@@ -67,7 +67,8 @@ def policy_evaluation_mo_batched(agent, env, weights: List[np.ndarray], rep: int
     Returns, per weight, the tuple of ``policy_evaluation_mo``: (scalarised return, scalarised discounted return, vector return,
     discounted vector return), each averaged over the ``rep`` episodes (scalarisation: np.dot, as the default of the serial routine).
     Identical to the serial routine for deterministic environments; a stochastic environment's copies share the RNG state of ``env``
-    unless ``seeds`` (one per episode, passed to ``reset``) is given."""
+    unless ``seeds`` (one per episode, passed to ``reset``) is given.  The weights and the return accumulators have ``weight_dtype``
+    (``np.zeros_like(w)`` of the serial routine): pass np.float64 to match serial calls made with float64 weights."""
     from copy import deepcopy
 
     if not hasattr(agent, "eval_batch"):
@@ -75,7 +76,7 @@ def policy_evaluation_mo_batched(agent, env, weights: List[np.ndarray], rep: int
     n_w = len(weights)
     N = n_w * rep
     envs = [deepcopy(env) for _ in range(N)]
-    w_all = np.repeat(np.asarray(weights, dtype=np.float32), rep, axis=0)  # episode e of weight i sits at row i * rep + e
+    w_all = np.repeat(np.asarray(weights, dtype=weight_dtype), rep, axis=0)  # episode e of weight i sits at row i * rep + e
     obs = []
     for k, e in enumerate(envs):
         o, _ = e.reset(seed=None if seeds is None else seeds[k % rep])

@@ -10,9 +10,26 @@ the reference exactly), so the caller lists every tensor the step mutates and th
 
 from __future__ import annotations
 
+import contextlib
+import gc
 from typing import Callable, Iterable, List
 
 import torch as th
+
+
+@contextlib.contextmanager
+def _gc_paused():
+    """Collect cyclic garbage now and keep the collector off during a capture.  A dropped graph that sits in a reference cycle (a step
+    closure that holds its own state dict) is otherwise destroyed by whichever collection happens to run inside a later capture; CUDA
+    forbids that while a stream captures, and the capture is invalidated."""
+    gc.collect()
+    enabled = gc.isenabled()
+    gc.disable()
+    try:
+        yield
+    finally:
+        if enabled:
+            gc.enable()
 
 
 class GraphedStep:
@@ -33,7 +50,7 @@ class GraphedStep:
                 self.fn()
         th.cuda.current_stream().wait_stream(side)
         g = th.cuda.CUDAGraph()
-        with th.cuda.graph(g):
+        with _gc_paused(), th.cuda.graph(g):
             self.fn()
         with th.no_grad():
             for t, s in zip(tensors, snap):
@@ -82,7 +99,7 @@ class PopulationGraph:
                     fn()
         th.cuda.current_stream().wait_stream(side)
         g = th.cuda.CUDAGraph()
-        with th.cuda.graph(g):
+        with _gc_paused(), th.cuda.graph(g):
             self._run_forked(streams)
         with th.no_grad():
             for t, s in zip(tensors, snap):

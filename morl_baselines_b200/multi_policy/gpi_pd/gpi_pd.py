@@ -13,8 +13,8 @@ a9 (``gpi_action``), a10 (``_reset_priorities``).  Under the API:
   * the Dyna path (``dyna=True``, the reference's default; SURVEY 8(f)3): probabilistic ensemble trained from an HBM-resident data set
     (common/model_based/probabilistic_ensemble.py), model rollouts that never leave the device -- batched GPI action, ONE fused
     sampling / uncertainty kernel (morl_ensemble_sample_f32), masked bulk insert of the imagined transitions (gpi_pd.py:367-414).
-Out of scope (SURVEY.md section 2, #21): the LinearSupport weight selector (cvxpy + pycddlib); ``train()`` therefore takes the
-selector as an argument.
+``train()`` selects weights with this package's LinearSupport (multi_policy/linear_support: corner weights on the device), and
+``eval_batch`` gives the batched GPI evaluation that selector's GPI-LS priority runs on.
 """
 
 from __future__ import annotations
@@ -530,6 +530,27 @@ class GPIPD(MOPolicy, MOAgent):
             net.train()
         return action
 
+    @th.no_grad()
+    def eval_batch(self, obs: np.ndarray, w: np.ndarray) -> np.ndarray:
+        """Actions of ``eval`` for N (observation, weight) rows at once -- the batched form used by the lockstep evaluation round
+        (common/evaluation.policy_evaluation_mo_batched).  With ``use_gpi``: one pairwise forward over the N x |M| (state, support weight)
+        pairs and one GPI kernel with per-row weights; otherwise the per-objective minimum over the nets and one greedy kernel.  The
+        nets are in eval mode during the call, as in ``eval``."""
+        obs_t = th.as_tensor(np.asarray(obs)).float().to(self.device).reshape(-1, *self.observation_shape)
+        w_t = th.as_tensor(np.asarray(w)).float().to(self.device).reshape(-1, self.reward_dim)
+        n = obs_t.shape[0]
+        for net in self.q_nets:
+            net.eval()
+        if self.use_gpi:
+            q = self.q_nets[0].forward_pairs(obs_t, self._support_matrix())  # [N, P, A, D]
+            _, _, act = ops.gpi_envelope(q.unsqueeze(0), w_t, dot_mode=self.dot_mode)
+        else:
+            psi = th.min(th.stack([net(obs_t, w_t) for net in self.q_nets]), dim=0)[0]  # [N, A, D]
+            _, _, act = ops.gpi_envelope(psi.view(1, n, 1, self.action_dim, self.reward_dim), w_t, dot_mode=self.dot_mode)
+        for net in self.q_nets:
+            net.train()
+        return act.cpu().numpy()
+
     def _act(self, obs: th.Tensor, w: th.Tensor) -> int:
         if self.np_random.random() < self.epsilon:
             return self.env.action_space.sample()
@@ -636,13 +657,15 @@ class GPIPD(MOPolicy, MOAgent):
               num_eval_weights_for_front: int = 100, num_eval_episodes_for_front: int = 5, num_eval_weights_for_eval: int = 50,
               timesteps_per_iter: int = 10000, weight_selection_algo: str = "gpi-ls", eval_freq: int = 1000, eval_mo_freq: int = 10000,
               checkpoints: bool = True, linear_support=None):
-        """Outer loop of reference gpi_pd.py:790-911.  The weight selector (reference LinearSupport: cvxpy + pycddlib, out of
-        scope) must be supplied as ``linear_support`` -- any object with next_weight / get_weight_support /
-        get_corner_weights / add_solution, e.g. the reference's own class."""
-        if linear_support is None:
-            raise NotImplementedError("GPIPD.train needs a weight selector: pass linear_support=<LinearSupport-like object> "
-                                      "(the cvxpy/pycddlib based selector is outside the accelerated hot path, SURVEY.md section 2 #21)")
+        """Outer loop of reference gpi_pd.py:790-911.  The weight selector is this package's ``LinearSupport``
+        (multi_policy/linear_support: corner weights on the device, GPI-LS's expanded set in one batched evaluation round per call),
+        built as the reference builds it (epsilon 0 for OLS, None for GPI-LS).  A caller-supplied ``linear_support`` -- any object
+        with next_weight / get_weight_support / get_corner_weights / add_solution -- is used instead."""
         from ...common.evaluation import policy_evaluation_mo
+        from ..linear_support.linear_support import LinearSupport
+
+        if linear_support is None:
+            linear_support = LinearSupport(num_objectives=self.reward_dim, epsilon=0.0 if weight_selection_algo == "ols" else None)
 
         max_iter = total_timesteps // timesteps_per_iter
         eval_weights = equally_spaced_weights(self.reward_dim, n=num_eval_weights_for_front)

@@ -333,6 +333,24 @@ class GPIPDContinuousAction(MOAgent, MOPolicy):
             action = action.detach().cpu().numpy()
         return action
 
+    @th.no_grad()
+    def eval_batch(self, obs: np.ndarray, w: np.ndarray) -> np.ndarray:
+        """Actions of ``eval`` for N (observation, weight) rows at once (common/evaluation.policy_evaluation_mo_batched).  With
+        ``use_gpi``: one policy call gives the N x |M| candidate actions pi(s_n, M_a), one critic call covers the N x |M| x |M|
+        (conditioning weight, candidate action) rows, and one GPI kernel over [1, N, |M|, |M|, d] picks each row's action."""
+        obs_t = th.as_tensor(np.asarray(obs)).float().to(self.device).reshape(-1, self.observation_dim)
+        w_t = th.as_tensor(np.asarray(w)).float().to(self.device).reshape(-1, self.reward_dim)
+        if not self.use_gpi:
+            return self.policy(obs_t, w_t).detach().cpu().numpy()
+        N, M, O, D = obs_t.shape[0], len(self.weight_support), self.observation_dim, self.reward_dim
+        Ms = self.stacked_weight_support
+        cand = self.policy(obs_t.unsqueeze(1).expand(N, M, O).reshape(N * M, O), Ms.repeat(N, 1)).view(N, M, -1)  # [n, a] = pi(s_n, M_a)
+        # values[n, p, a] = Q_0(s_n, cand[n, a], M_p)
+        values = self.q_nets[0](obs_t.view(N, 1, 1, O).expand(N, M, M, O), cand.unsqueeze(1).expand(N, M, M, cand.shape[-1]),
+                                Ms.view(1, M, 1, D).expand(N, M, M, D))
+        _, _, act = ops.gpi_envelope(values.reshape(1, N, M, M, D).contiguous(), w_t)
+        return cand[th.arange(N, device=self.device), act.long()].detach().cpu().numpy()
+
     def set_weight_support(self, weight_list: List[np.ndarray]):
         """Set the weight support set (duplicates within tolerance removed, reference :487-492)."""
         weights_no_repeat = unique_tol(weight_list)
@@ -381,13 +399,14 @@ class GPIPDContinuousAction(MOAgent, MOPolicy):
               num_eval_weights_for_front: int = 100, num_eval_episodes_for_front: int = 5, num_eval_weights_for_eval: int = 50,
               weight_selection_algo: str = "gpi-ls", timesteps_per_iter: int = 10000, eval_freq: int = 1000, eval_mo_freq: int = 10000,
               checkpoints: bool = True, linear_support=None):
-        """Outer loop of reference :587-702.  The weight selector (reference LinearSupport: cvxpy + pycddlib, out of scope) must be
-        supplied as ``linear_support`` -- any object with next_weight / get_weight_support / get_corner_weights / add_solution,
-        e.g. the reference's own class."""
-        if linear_support is None:
-            raise NotImplementedError("GPIPDContinuousAction.train needs a weight selector: pass linear_support=<LinearSupport-like object> "
-                                      "(the cvxpy/pycddlib based selector is outside the accelerated hot path, SURVEY.md section 2 #21)")
+        """Outer loop of reference :587-702.  The weight selector is this package's ``LinearSupport`` (multi_policy/linear_support),
+        built as the reference builds it (epsilon 0 for OLS, None for GPI-LS).  A caller-supplied ``linear_support`` -- any object with
+        next_weight / get_weight_support / get_corner_weights / add_solution -- is used instead."""
         from ...common.evaluation import log_all_multi_policy_metrics, policy_evaluation_mo
+        from ..linear_support.linear_support import LinearSupport
+
+        if linear_support is None:
+            linear_support = LinearSupport(num_objectives=self.reward_dim, epsilon=0.0 if weight_selection_algo == "ols" else None)
 
         if self.log:
             self.register_additional_config({"total_timesteps": total_timesteps, "ref_point": ref_point.tolist(), "known_front": known_pareto_front,

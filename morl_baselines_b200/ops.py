@@ -339,6 +339,26 @@ def hypervolume(points: th.Tensor, ref_point: th.Tensor, keep: Optional[th.Tenso
     return out
 
 
+def corner_weights(V: th.Tensor, cap: int = 256) -> th.Tensor:
+    """Vertices (w, u) of { V w <= u, w >= 0, sum w = 1 } for a float64 CUDA tensor V [n, d] (reference linear_support.py:295-349;
+    the caller rounds V).  Returns float64 [K, d+1] in no particular order; one launch, plus a second one with a buffer of the exact size
+    when more than ``cap`` vertices exist (the count is read back: one host sync)."""
+    if not V.is_cuda or V.dtype != th.float64 or V.dim() != 2:
+        raise _lib.MorlB200Error("corner_weights: V must be a float64 CUDA tensor [n, d]")
+    V = V.contiguous()
+    n, d = V.shape
+    count = th.empty(1, dtype=th.int32, device=V.device)
+    while True:
+        verts = th.empty((cap, d + 1), dtype=th.float64, device=V.device)
+        rc = _lib.load().morl_corner_weights_f64(_ptr(V), n, d, _ptr(verts) if cap > 0 else None, cap, _ptr(count), _stream())
+        _lib.check(rc, "morl_corner_weights_f64")
+        _count()
+        k = int(count.item())
+        if k <= cap:
+            return verts[:k]
+        cap = k
+
+
 class PolyakPlan:
     """Device-side (param, target, size) table for morl_polyak_f32; build once per pair of networks."""
 

@@ -2,9 +2,10 @@
 
     compute-sanitizer --tool memcheck|racecheck|synccheck|initcheck python scripts/sanitize_all.py [group ...]
 
-groups: envelope td gemm optim pareto replay layer1 qhead dyna chain (default: all).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
+groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners (default: all).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
 every code path: all envelope kernel families, both GEMM operand formats x CTA modes x accumulator modes, MN split-K GEMM with the fused
-column sums, every split / reduction helper, the loss kernels (discrete SAC's included), Adam, polyak, Pareto + front records, replay gather."""
+column sums, every split / reduction helper, the loss kernels (discrete SAC's included), Adam, polyak, Pareto + front records, replay gather,
+the corner-weight enumeration."""
 import os
 import sys
 
@@ -22,7 +23,7 @@ if os.environ.get("SAN_ZERO_PLANES") == "1":
     # from a genuine read of memory nobody wrote.
     _empty = ops.empty_planes
     ops.empty_planes = lambda *a, **k: _empty(*a, **k).zero_()
-groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain"}
+groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain", "corners"}
 
 
 def rn(*s, scale=1.0):
@@ -199,4 +200,12 @@ if "chain" in groups:
     ops.GemmChain([gb], [ws[0]], None, [sws[0]], None, act_scale=sa, relu=False, bits_in=[bits[0]])()
     th.cuda.synchronize()
     print("chain ok")
+if "corners" in groups:
+    # corner-weight enumeration (csrc/linear_support.cu): every dimension template, a degenerate integer set, and a launch whose count
+    # exceeds its buffer (the writes past cap must be skipped)
+    for d, n in [(2, 7), (3, 9), (4, 6), (5, 5), (6, 4), (7, 3), (8, 3)]:
+        V = th.randint(0, 3, (n, d), device=dev, generator=g).double()
+        ops.corner_weights(V, cap=1)
+    th.cuda.synchronize()
+    print("corners ok")
 print("sanitize run ok")
