@@ -408,6 +408,15 @@ MORL_API int morl_gemm_chain_supported(int fmt, int M, int K);
 MORL_API int morl_gemm_chain_f32(int fmt, int n_chains, int n_layers, const void* const* act_planes, long long act_plane_stride, const float* act_scale,
                                  const void* const* w_planes, long long w_plane_stride, const float* const* w_scales, const float* const* biases,
                                  int relu, const void* const* relu_bits_in, void* const* relu_bits_out, int M, int K, int k_first, void* stream);
+/* f16x2 chains run with the activation tile resident in shared memory (k_first then needs only be a multiple of 32); bf16x3 chains as above.
+ * morl_gemm_chain_pairs_f32: the same forward chains (ReLU, f16x2), started from the separable first layer: the input of chain c is
+ * relu(u[c][b] + v[c][j]) * act_scale for row b * W + j (u[c] [B][256], v[c] [W][256] fp32, 16-byte aligned) -- the planes
+ * morl_pairs_relu_split_planes would write, built on chip instead.  acts[c * n_layers + l] ([P][B W][256]) receives the output of layer l
+ * of chain c only when bit c * n_layers + l of store_mask is set (may be NULL otherwise); the others never leave shared memory. */
+MORL_API int morl_gemm_chain_pairs_f32(int n_chains, int n_layers, const float* const* u, const float* const* v, int B, int W, const void* const* acts,
+                                       long long act_plane_stride, const float* act_scale, const void* const* w_planes, long long w_plane_stride,
+                                       const float* const* w_scales, const float* const* biases, void* const* relu_bits_out, unsigned int store_mask,
+                                       void* stream);
 /* Diagnostics (not part of the reference surface): per-role cycle counters of morl_gemm_planes_f32, summed over CTAs and launches
  * since the last reset; collected only when the environment variable MORL_GEMM_STATS=1 is set before the first GEMM call.
  * out8: [0] MMA thread waiting for TMA data, [1] waiting for the epilogue to free an accumulator, [2] MMA loop total,

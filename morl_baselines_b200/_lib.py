@@ -66,6 +66,7 @@ SIGNATURES = {
     "morl_philox_advance": (_i, [_vp, C.c_uint, _vp]),
     "morl_gemm_chain_supported": (_i, [_i, _i, _i]),
     "morl_gemm_chain_f32": (_i, [_i, _i, _i, _vp, C.c_longlong, _vp, _vp, C.c_longlong, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp]),
+    "morl_gemm_chain_pairs_f32": (_i, [_i, _i, _vp, _vp, _i, _i, _vp, C.c_longlong, _vp, _vp, C.c_longlong, _vp, _vp, _vp, C.c_uint, _vp]),
     "morl_debug_gemm_stats": (_i, [_vp, _i]),
     "morl_ensemble_sample_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "morl_qhead_envelope_supported": (_i, [_i, _i, _i, _i, _i, _i]),

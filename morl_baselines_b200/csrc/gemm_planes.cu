@@ -29,7 +29,8 @@
 // Operands: A [P][M][K] (K-major), B [P][N_pad][K] (K-major), K % BK == 0, N_pad % 32 == 0, N_pad <= 512.  An output wider than 256
 // columns runs as two column units [0, 256) and [256, N_pad) of the same tile, each with the shared-memory plan of N_pad = 256.
 // The chained hidden layers (gemm_chain_kernel) run the same pipeline -- carve_kplan, the producer's load_unit, the consumer's consume_unit and
-// reload_bias -- on their own schedule of units.
+// reload_bias -- on their own schedule of units; f16x2 chains run on gemm_chain_resident_kernel, which keeps a CTA's activation tile in shared
+// memory through all layers and streams only the weights.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -253,15 +254,13 @@ struct EpiArgs {
 // col0 + 8 q + 2 (l % 4) + e of row rbase + l / 4 + 8 h (the wgmma fragment).  The re-split planes leave through the warp's two staging tiles in
 // turn (n_stored counts the warp's bulk stores): a chunk is staged while the TMA store of the previous one is still reading the other tile.
 // PRE: a[] already holds the pre-activation (the LayerNorm epilogue has applied scale, bias, dropout and LayerNorm).
-template <int FMT, bool PRE = false>
-__device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, int rbase, int lane, const EpiArgs& e, const CUtensorMap* tmC,
-                                               uint8_t* my_stage, uint32_t& n_stored, float& amax) {
-    using F = PlaneFmt<FMT>;
-    constexpr int P = F::P;
+// The output values of such a chunk, x[h][2 q + c] = column col0 + 8 q + 2 (l % 4) + c of row rbase + l / 4 + 8 h: scale, bias, ReLU, the
+// ReLU-backward bits applied, the ReLU bits recorded.
+template <bool PRE>
+__device__ __forceinline__ void epilogue_values(const float (&a)[16], int col0, int rbase, int lane, const EpiArgs& e, float (&x)[2][8]) {
     const int l4 = lane & 3, lr = lane >> 2;
     // ReLU bit masks: the word of the row that holds columns [col0, col0 + 32)
     const int wi = relu_bits_word(col0);
-    float x[2][8];
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -297,6 +296,16 @@ __device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, i
             if (l4 == 0 && row < e.M) e.bits_out[(size_t)row * e.bits_ld + wi] = positive;
         }
     }
+}
+
+template <int FMT, bool PRE = false>
+__device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, int rbase, int lane, const EpiArgs& e, const CUtensorMap* tmC,
+                                               uint8_t* my_stage, uint32_t& n_stored, float& amax) {
+    using F = PlaneFmt<FMT>;
+    constexpr int P = F::P;
+    const int l4 = lane & 3, lr = lane >> 2;
+    float x[2][8];
+    epilogue_values<PRE>(a, col0, rbase, lane, e, x);
     if (e.mask) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -728,6 +737,323 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
                     }
                 }
         if (FMT == MORL_FMT_F16X2) note_overflow(amax);
+    }
+}
+
+// =================================================================================================================
+// RESIDENT chain kernel (f16x2): a CTA keeps its 128-row activation tile in shared memory from the first layer of a chain to the last.
+// Layer l's epilogue writes its output chunk c (32 columns) as K-block c of layer l+1's A operand, so no intermediate activation goes
+// through L2 and layer l+1 waits for no global store; the producer streams only weights.  An output leaves by TMA store straight from the
+// tile only when the job's `store` bit is set.  The chain's input is either a TMA load of plane rows (dX chains, GemmChain) or, in pair mode,
+// relu(u[b] + v[j]) s for row b W + j computed by the consumer warps into the tile (the arithmetic of pairs_relu_split_h256_kernel).
+// Schedule of a CTA: its tiles in order, each through every layer of chain 0, then (same tile index, the chain's own rotation) chain 1.
+// Accumulation order = gemm_chain_kernel's: k16 steps in order, products A1B0, A0B1, A0B0 inner (a 32-wide K block issues the same
+// sequence as a 64-wide one), so outputs are bit-identical.
+// =================================================================================================================
+struct ResPlan {
+    static constexpr int P = 2, BK = 32, kStages = 3;
+    static constexpr uint32_t kRowB = BK * 2;                          // 64 B rows, 64-byte swizzle (make_desc_k<64>)
+    static constexpr uint32_t kKBlock = P * kGemmBM * kRowB;           // one K-block of the activation tile: [P][128 rows][64 B] = 16 KB
+    static constexpr uint32_t kPlaneKB = kGemmBM * kRowB;              // 8 KB: one plane of a K-block
+    static constexpr uint32_t kAct = 8 * kKBlock;                      // 256 columns: 128 KB
+    static constexpr uint32_t kBStage = P * 256 * kRowB;               // weights of one K-block: 32 KB
+    static constexpr uint32_t kOffB = kAct;
+    static constexpr uint32_t kOffBias = kOffB + kStages * kBStage;
+    static constexpr uint32_t kOffBar = kOffBias + 1024;
+    static constexpr uint32_t kBytes = kOffBar + 256 + 1024;           // + alignment slack of the dynamic segment
+    static_assert(kBytes <= 232448, "dynamic shared memory of one CTA on sm_90 (227 KB)");
+};
+
+struct alignas(64) ResChainMaps {
+    CUtensorMap A[2];              // planes mode: the chain's input [P][M][k_first], box P x 128 x 32
+    CUtensorMap B[kChainMaxJobs];  // weight planes of the job [P][256][K], box 1 x 256 x 32
+    CUtensorMap C[kChainMaxJobs];  // stored output of the job [P][M][256], box 1 x 16 x 32 (64-byte swizzle)
+};
+
+struct ResChainArgs {
+    int M, K, k_first, n_chains, n_layers;
+    const float* bias[kChainMaxJobs];
+    const float* b_scale[kChainMaxJobs];
+    uint32_t* bits_out[kChainMaxJobs];
+    const uint32_t* bits_in[kChainMaxJobs];
+    const float* a_scale;
+    int relu;
+    uint32_t store;                // bit job: the job's output is written to global memory
+    const float* u[2];             // pair mode (u != nullptr): u[c] [B][256], v[c] [W][256], row r = b W + j
+    const float* v[2];
+    int W;
+    unsigned long long* stats;     // MORL_GEMM_STATS=1: [0] consumer wait on weights, [1] consumer loop, [2] producer wait on free stage,
+                                   // [3] epilogue busy, [4] consumer wait on the input tile (tile boundary)
+};
+
+// Consumer warpgroup of one layer: A = its 64 rows of the resident tile, B = the ring.  Same products in the same order as mma_unit.
+__device__ __forceinline__ void mma_unit_resident(float (&acc)[128], uint32_t act, const KSmem& s, Ring& ring, int n_kblk, int wg, int lane,
+                                                  long long* wait_cycles) {
+    using F = PlaneFmt<MORL_FMT_F16X2>;
+    using R = ResPlan;
+    constexpr uint32_t b_plane = 256u * R::kRowB;
+    const uint32_t a_wg = act + (uint32_t)wg * 64u * R::kRowB;
+    uint32_t prev = 0;
+    for (int kb = 0; kb < n_kblk; ++kb) {
+        const long long c0 = wait_cycles ? clock64() : 0;
+        g_mbar_wait(&s.full[ring.stage], ring.phase);
+        if (wait_cycles) *wait_cycles += clock64() - c0;
+        wgmma_fence();
+        const uint32_t a0 = a_wg + (uint32_t)kb * R::kKBlock;
+        const uint32_t b0 = g_smem_u32(s.b + ring.stage * R::kBStage);
+#pragma unroll
+        for (int ks = 0; ks < R::BK / 16; ++ks) {
+#pragma unroll
+            for (int t = 0; t < F::NPROD; ++t) {
+                const uint64_t ad = make_desc_k<R::kRowB>(a0 + F::pa(t) * R::kPlaneKB + ks * 32);
+                const uint64_t bd = make_desc_k<R::kRowB>(b0 + F::pb(t) * b_plane + ks * 32);
+                Wgmma<256>::template mma<MORL_FMT_F16X2, 0, 0>(acc, ad, bd, (kb | ks | t) != 0 ? 1u : 0u);
+            }
+        }
+        wgmma_commit();
+        if (kb > 0) {
+            wgmma_wait<1>();
+            if (lane == 0) g_mbar_arrive(&s.empty[prev]);
+        }
+        prev = ring.stage;
+        ring.advance();
+    }
+    wgmma_wait<0>();
+    if (n_kblk > 0 && lane == 0) g_mbar_arrive(&s.empty[prev]);
+}
+
+// 16-byte chunk (8 columns, 4 words per plane) of row `row` (of the tile) in K-block kb of the resident tile (64-byte swizzle)
+__device__ __forceinline__ uint8_t* res_chunk(uint8_t* act, int kb, int row, int q) {
+    return act + (uint32_t)kb * ResPlan::kKBlock + (uint32_t)row * ResPlan::kRowB + (uint32_t)((q ^ ((row >> 1) & 3)) << 4);
+}
+
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_chain_resident_kernel(const __grid_constant__ ResChainMaps maps, const ResChainArgs g) {
+    using F = PlaneFmt<MORL_FMT_F16X2>;
+    using R = ResPlan;
+    constexpr int P = R::P, BN = 256;
+    extern __shared__ uint8_t gsmem_raw[];
+    uint8_t* sm = align_1k(gsmem_raw);
+    uint8_t* act = sm;
+    KSmem s;
+    s.a = nullptr;
+    s.b = sm + R::kOffB;
+    s.b_stage = R::kBStage;
+    s.c = nullptr;
+    s.bias = reinterpret_cast<float*>(sm + R::kOffBias);
+    s.full = reinterpret_cast<uint64_t*>(sm + R::kOffBar);
+    s.empty = s.full + R::kStages;
+    uint64_t* act_full = s.empty + R::kStages;  // planes mode: the input tile has landed (TMA transaction bytes)
+    uint64_t* act_empty = act_full + 1;         // planes mode: the 8 consumer warps are done with the tile (MMAs and stores read it)
+    const bool pairs = g.u[0] != nullptr;
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int unit = blockIdx.x, n_units = gridDim.x;
+    const int n_tiles = (g.M + kGemmBM - 1) / kGemmBM;
+    const int n_kblk_full = g.K / R::BK, n_kblk_first = g.k_first / R::BK;
+    // tile t of chain c on CTA (t + offset_c) mod n_units, chain 1 rotated by half the grid (as gemm_chain_kernel: balances ragged tile counts)
+    const int cu0 = unit, cu1 = (unit + n_units / 2) % n_units;
+    const int mt0 = cu0 < n_tiles ? (n_tiles - cu0 + n_units - 1) / n_units : 0;
+    const int mt1 = g.n_chains > 1 ? (cu1 < n_tiles ? (n_tiles - cu1 + n_units - 1) / n_units : 0) : 0;
+    const int n_ti = mt0 > mt1 ? mt0 : mt1;
+    // first row of tile ti of chain c on this CTA, or -1
+    auto tile_row = [&](int ti, int c) { return ti < (c ? mt1 : mt0) ? ((c ? cu1 : cu0) + ti * n_units) * kGemmBM : -1; };
+
+    if (threadIdx.x == 0) {
+        init_ring_barriers(s.full, s.empty, R::kStages);
+        g_mbar_init(act_full, 1);
+        g_mbar_init(act_empty, 8);
+        g_mbar_init_fence();
+    }
+    pdl_enter();
+    __syncthreads();
+
+    if (warp >= 8) {
+        // ================= producer warpgroup: one lane issues TMA (weights; the input tile in planes mode) =================
+        warpgroup_reg_dec<kGemmProducerRegs>();
+        if (warp == 8 && lane == 0) {
+            Ring ring((uint32_t)R::kStages);
+            long long w_empty = 0;
+            uint32_t n_in = 0;  // input tiles loaded
+            for (int ti = 0; ti < n_ti; ++ti)
+                for (int c = 0; c < g.n_chains; ++c) {
+                    const int row0 = tile_row(ti, c);
+                    if (row0 < 0) continue;
+                    for (int l = 0; l < g.n_layers; ++l) {
+                        const int job = c * g.n_layers + l;
+                        const int nkb = l == 0 ? n_kblk_first : n_kblk_full;
+                        for (int kb = 0; kb < nkb; ++kb) {
+                            if (!pairs && l == 0 && kb == (nkb < R::kStages ? nkb - 1 : R::kStages - 1)) {
+                                // the input tile, once the first weight stages are on their way (they only needed free ring slots): wait
+                                // until the consumers are done with the previous tile, then load the k_first / 32 K-blocks of this one
+                                if (n_in > 0) {
+                                    const long long c0 = g.stats ? clock64() : 0;
+                                    g_mbar_wait(act_empty, (n_in - 1u) & 1u);
+                                    if (g.stats) w_empty += clock64() - c0;
+                                }
+                                g_mbar_expect_tx(act_full, (uint32_t)n_kblk_first * R::kKBlock);
+                                for (int k = 0; k < n_kblk_first; ++k) tma_load_3d(act + k * R::kKBlock, &maps.A[c], act_full, k * R::BK, row0, 0);
+                                ++n_in;
+                            }
+                            const long long c0 = g.stats ? clock64() : 0;
+                            g_mbar_wait(&s.empty[ring.stage], ring.phase ^ 1u);
+                            if (g.stats) w_empty += clock64() - c0;
+                            uint64_t* full = &s.full[ring.stage];
+                            g_mbar_expect_tx(full, R::kBStage);
+                            uint8_t* bs = s.b + ring.stage * R::kBStage;
+                            for (int p = 0; p < P; ++p) tma_load_3d(bs + (uint32_t)p * 256u * R::kRowB, &maps.B[job], full, kb * R::BK, 0, p);
+                            ring.advance();
+                        }
+                    }
+                }
+            if (g.stats) atomicAdd(&g.stats[2], (unsigned long long)w_empty);
+        }
+    } else {
+        // ================= consumer warpgroups (warps 0..7) =================
+        warpgroup_reg_inc<kGemmConsumerRegs>();
+        const int wg = warp >> 2, wr = warp & 3;
+        const int l4 = lane & 3, lr = lane >> 2;
+        const int trow = wg * 64 + wr * 16;  // this warp's 16 rows of the tile
+        const float s_act = ld_scale(g.a_scale);
+        const uint32_t act_s = g_smem_u32(act);
+        float amax = 0.f;
+        float acc[128];
+        Ring ring((uint32_t)R::kStages);
+        long long w_full = 0, busy = 0, w_act = 0;
+        const long long t_begin = g.stats ? clock64() : 0;
+        uint32_t n_in = 0;
+        for (int ti = 0; ti < n_ti; ++ti)
+            for (int c = 0; c < g.n_chains; ++c) {
+                const int row0 = tile_row(ti, c);
+                if (row0 < 0) continue;
+                if (pairs) {
+                    // the input tile: relu(u[b] + v[j]) s split into planes, this warp's 16 rows; lane = (row l / 4 + 8 h, 8 columns l % 4 of
+                    // every K-block).  The stores of the previous tile's last layer must have read these rows.
+                    if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+                    __syncwarp();
+                    const float* u = c ? g.u[1] : g.u[0];
+                    const float* v = c ? g.v[1] : g.v[0];
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int rl = trow + lr + 8 * h, row = row0 + rl;
+                        const bool ok = row < g.M;
+                        const int b = ok ? row / g.W : 0, j = ok ? row - b * g.W : 0;
+#pragma unroll 2
+                        for (int kb = 0; kb < 8; ++kb) {
+                            const int col = kb * 32 + 8 * l4;
+                            uint32_t o[P][4];
+                            if (ok) {
+                                const float4* up = reinterpret_cast<const float4*>(u + (size_t)b * BN + col);
+                                const float4* vp = reinterpret_cast<const float4*>(v + (size_t)j * BN + col);
+                                const float4 u0 = __ldg(up), u1 = __ldg(up + 1), v0 = __ldg(vp), v1 = __ldg(vp + 1);
+                                const float x[8] = {u0.x + v0.x, u0.y + v0.y, u0.z + v0.z, u0.w + v0.w, u1.x + v1.x, u1.y + v1.y, u1.z + v1.z, u1.w + v1.w};
+#pragma unroll
+                                for (int t = 0; t < 4; ++t) {
+                                    uint32_t w[P];
+                                    const float r0 = x[2 * t] < 0.f ? 0.f : x[2 * t], r1 = x[2 * t + 1] < 0.f ? 0.f : x[2 * t + 1];  // NaN-propagating ReLU
+                                    F::split2(r0 * s_act, r1 * s_act, w, amax);
+#pragma unroll
+                                    for (int p = 0; p < P; ++p) o[p][t] = w[p];
+                                }
+                            } else {
+#pragma unroll
+                                for (int t = 0; t < 4; ++t)
+#pragma unroll
+                                    for (int p = 0; p < P; ++p) o[p][t] = 0u;
+                            }
+                            uint8_t* dst = res_chunk(act, kb, rl, l4);
+#pragma unroll
+                            for (int p = 0; p < P; ++p) *reinterpret_cast<uint4*>(dst + p * R::kPlaneKB) = make_uint4(o[p][0], o[p][1], o[p][2], o[p][3]);
+                        }
+                    }
+                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                    bar_sync_named(2 + wg, 128);  // the warpgroup's 64 rows are in place before its first MMA
+                }
+                for (int l = 0; l < g.n_layers; ++l) {
+                    const int job = c * g.n_layers + l;
+                    const bool last = l == g.n_layers - 1, store = (g.store >> job) & 1u;
+                    reload_bias(s.bias, g.bias[job], 0, BN, s_act);  // (times the folded output scale; both warpgroups left the previous epilogue)
+                    if (!pairs && l == 0) {
+                        const long long c0 = g.stats ? clock64() : 0;
+                        g_mbar_wait(act_full, n_in & 1u);
+                        if (g.stats) w_act += clock64() - c0;
+                    }
+                    mma_unit_resident(acc, act_s, s, ring, l == 0 ? n_kblk_first : n_kblk_full, wg, lane, g.stats ? &w_full : nullptr);
+                    const long long c1 = g.stats ? clock64() : 0;
+                    EpiArgs e;
+                    e.M = g.M; e.N = BN;
+                    e.k_acc = s_act / (s_act * ld_scale(g.b_scale[job]));  // as gemm_chain_kernel's folded epilogue
+                    e.c_mul = 1.0f;
+                    e.bias_s = s.bias; e.relu = g.relu; e.bits_in = g.bits_in[job]; e.bits_out = g.bits_out[job]; e.bits_ld = relu_bits_words(BN);
+                    e.mask = nullptr; e.ld_mask = 0; e.c_f32 = nullptr; e.ldc = 0; e.planes = 1; e.ldp = BN;
+                    const bool to_tile = !last || store;
+                    if (to_tile) {
+                        // the rows are overwritten: the stores of the previous layer (if any) must have read them
+                        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+                        __syncwarp();
+                    }
+                    const int rbase = row0 + trow;
+#pragma unroll
+                    for (int cc = 0; cc < 8; ++cc) {
+                        float a[16];
+#pragma unroll
+                        for (int jj = 0; jj < 16; ++jj) a[jj] = acc[16 * cc + jj];
+                        float x[2][8];
+                        epilogue_values<false>(a, 32 * cc, rbase, lane, e, x);
+                        if (to_tile) {
+                            // output chunk cc = K-block cc of the next layer, the swizzled layout of a TMA box [P][128][32]
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                const int rl = lr + 8 * h;
+#pragma unroll
+                                for (int q = 0; q < 4; ++q) {
+                                    uint32_t w[P];
+                                    F::split2(x[h][2 * q], x[h][2 * q + 1], w, amax);
+                                    uint8_t* st = res_chunk(act, cc, trow + rl, q) + 4 * l4;
+#pragma unroll
+                                    for (int p = 0; p < P; ++p) *reinterpret_cast<uint32_t*>(st + p * R::kPlaneKB) = w[p];
+                                }
+                            }
+                            if (store) {
+                                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                                __syncwarp();
+                                if (lane == 0) {
+                                    const uint32_t src = act_s + (uint32_t)cc * R::kKBlock + (uint32_t)trow * R::kRowB;
+#pragma unroll
+                                    for (int p = 0; p < P; ++p)
+                                        asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(&maps.C[job]),
+                                                     "r"(src + p * R::kPlaneKB), "r"(32 * cc), "r"(rbase), "r"(p)
+                                                     : "memory");
+                                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+                                }
+                            }
+                        }
+                    }
+                    if (!last) {
+                        // next layer: its A operand (this warpgroup's 64 rows) is complete and visible to the tensor cores
+                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                        bar_sync_named(2 + wg, 128);
+                    } else if (!pairs) {
+                        // the producer may load the next input tile once every warp's stores have read its rows
+                        __syncwarp();
+                        if (lane == 0) {
+                            asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+                            g_mbar_arrive(act_empty);
+                        }
+                    }
+                    if (g.stats) busy += clock64() - c1;
+                }
+                ++n_in;
+            }
+        if (g.stats && warp == 0 && lane == 0) {
+            atomicAdd(&g.stats[0], (unsigned long long)w_full);
+            atomicAdd(&g.stats[1], (unsigned long long)(clock64() - t_begin));
+            atomicAdd(&g.stats[3], (unsigned long long)busy);
+            atomicAdd(&g.stats[4], (unsigned long long)w_act);
+        }
+        note_overflow(amax);
+        if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // all bulk stores of this warp have completed
     }
 }
 
@@ -1900,6 +2226,60 @@ extern "C" int morl_philox_advance(unsigned int* offset, unsigned int inc, void*
 }
 
 
+namespace morl {
+// Launch of gemm_chain_resident_kernel.  g: k_first, store and (pair mode) u / v / W set by the caller; in[c]: planes-mode input of chain c
+// (nullptr in pair mode); acts[c (n_layers + 1) + l + 1]: output of job (c, l), needed when its store bit is set.
+static int launch_chain_resident(ResChainArgs& g, int n_chains, int n_layers, const void* const* in, const void* const* acts, long long act_plane_stride,
+                                 const float* act_scale, const void* const* w_planes, long long w_plane_stride, const float* const* w_scales,
+                                 const float* const* biases, int relu, const void* const* relu_bits_in, void* const* relu_bits_out, int M, int K,
+                                 const char* name, void* stream) {
+    constexpr int fmt = MORL_FMT_F16X2;
+    ResChainMaps maps;
+    memset(&maps, 0, sizeof(maps));
+    g.M = M; g.K = K; g.n_chains = n_chains; g.n_layers = n_layers; g.a_scale = act_scale; g.relu = relu ? 1 : 0;
+    for (int c = 0; c < n_chains; ++c) {
+        if (!g.u[0]) {
+            MORL_REQUIRE(in[c] && aligned16(in[c]), MORL_ERR_NULL, "%s: NULL or misaligned input planes (chain %d)", name, c);
+            // [P][M][k_first] (plane stride M * k_first), box P x 128 rows x 32
+            const int rc = make_plane_map(&maps.A[c], fmt, in[c], M, g.k_first, (long long)M * g.k_first, kGemmBM, ResPlan::BK);
+            MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "%s: cuTensorMapEncodeTiled(A) failed (%d)", name, rc);
+        }
+        for (int l = 0; l < n_layers; ++l) {
+            const int job = c * n_layers + l;
+            const int kj = l == 0 ? g.k_first : K;
+            const long long w_stride = l == 0 ? (long long)256 * g.k_first : w_plane_stride;
+            MORL_REQUIRE(w_planes[job] && aligned16(w_planes[job]), MORL_ERR_NULL, "%s: NULL or misaligned weight planes (chain %d, layer %d)", name, c, l);
+            int rc = make_plane_map(&maps.B[job], fmt, w_planes[job], 256, kj, w_stride, 256, ResPlan::BK, true);
+            MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "%s: cuTensorMapEncodeTiled(B) failed (%d)", name, rc);
+            if ((g.store >> job) & 1u) {
+                const void* out = acts[c * (n_layers + 1) + l + 1];
+                MORL_REQUIRE(out && aligned16(out), MORL_ERR_NULL, "%s: NULL or misaligned output planes (chain %d, layer %d)", name, c, l);
+                rc = make_plane_map(&maps.C[job], fmt, out, M, 256, act_plane_stride, 16, 32, true);
+                MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "%s: cuTensorMapEncodeTiled(C) failed (%d)", name, rc);
+            }
+            g.bias[job] = biases ? biases[job] : nullptr;
+            g.b_scale[job] = w_scales ? w_scales[job] : nullptr;
+            g.bits_out[job] = relu_bits_out ? static_cast<uint32_t*>(relu_bits_out[job]) : nullptr;
+            g.bits_in[job] = relu_bits_in ? static_cast<const uint32_t*>(relu_bits_in[job]) : nullptr;
+            MORL_REQUIRE(aligned16(g.bits_out[job]) && aligned16(g.bits_in[job]), MORL_ERR_ALIGN, "%s: ReLU bit masks must be 16-byte aligned", name);
+        }
+    }
+    static const bool want_stats = [] { const char* e = getenv("MORL_GEMM_STATS"); return e && e[0] == '1'; }();
+    if (want_stats) {
+        void* sp = nullptr;
+        cudaGetSymbolAddress(&sp, g_gemm_stats);
+        g.stats = static_cast<unsigned long long*>(sp);
+    }
+    const int sms = sm_count();
+    const int n_tiles = (M + kGemmBM - 1) / kGemmBM;
+    constexpr size_t smem = ResPlan::kBytes;
+    set_smem_limit_once<gemm_chain_resident_kernel>(smem);
+    launch_k_pdl(gemm_pdl_enabled(), gemm_chain_resident_kernel, dim3(n_tiles < sms ? n_tiles : sms), dim3(kGemmThreads), smem,
+                 static_cast<cudaStream_t>(stream), maps, g);
+    return check_launch(name);
+}
+}  // namespace morl
+
 extern "C" int morl_gemm_chain_supported(int fmt, int M, int K) {
     using namespace morl;
     return fmt_ok(fmt) && M >= 2 * kGemmBM && K == 256;
@@ -1917,9 +2297,20 @@ extern "C" int morl_gemm_chain_f32(int fmt, int n_chains, int n_layers, const vo
                  "morl_gemm_chain_f32: need 1 <= n_chains <= 2 and n_chains * n_layers <= %d (got %d x %d)", kChainMaxJobs, n_chains, n_layers);
     MORL_REQUIRE(morl_gemm_chain_supported(fmt, M, K), MORL_ERR_UNSUPPORTED, "morl_gemm_chain_f32: unsupported configuration fmt=%d M=%d K=%d (256-wide layers, M >= 256)",
                  fmt, M, K);
-    const int BK = fmt_bk(fmt);
+    // f16x2 runs on the resident kernel (32-wide K blocks), bf16x3 on gemm_chain_kernel
+    const int BK = fmt == MORL_FMT_F16X2 ? ResPlan::BK : fmt_bk(fmt);
     if (k_first <= 0) k_first = K;
     MORL_REQUIRE(k_first % BK == 0 && k_first <= K, MORL_ERR_SHAPE, "morl_gemm_chain_f32: k_first=%d must be a multiple of %d and <= K", k_first, BK);
+    if (fmt == MORL_FMT_F16X2) {
+        ResChainArgs g;
+        memset(&g, 0, sizeof(g));
+        g.k_first = k_first;
+        g.store = (1u << (n_chains * n_layers)) - 1u;  // every output
+        const void* in[2] = {nullptr, nullptr};
+        for (int c = 0; c < n_chains; ++c) in[c] = act_planes[c * (n_layers + 1)];
+        return launch_chain_resident(g, n_chains, n_layers, in, act_planes, act_plane_stride, act_scale, w_planes, w_plane_stride, w_scales, biases,
+                                     relu, relu_bits_in, relu_bits_out, M, K, "morl_gemm_chain_f32", stream);
+    }
     ChainMaps maps;  // (host staging of the 3 x 8 tensor maps on this thread's stack -- the entry point stays re-entrant; copied into the kernel
                      // parameters by the launch)
     ChainArgs g;
@@ -1958,4 +2349,37 @@ extern "C" int morl_gemm_chain_f32(int fmt, int n_chains, int n_layers, const vo
                      static_cast<cudaStream_t>(stream), maps, g);
     });
     return check_launch("morl_gemm_chain_f32");
+}
+
+// Hidden layers 2.. of one or two pair networks in ONE launch, starting from the separable first layer: the input tile of chain c is
+// relu(u[c][b] + v[c][j]) * act_scale (row b W + j, exactly morl_pairs_relu_split_planes' planes) built in shared memory, so the first hidden
+// activation never reaches global memory.  Job (c, l) = layer l of chain c; its output planes acts[c n_layers + l] ([P][B W][256]) are written
+// only when bit (c n_layers + l) of store_mask is set (NULL otherwise).  f16x2 only (csrc: gemm_chain_resident_kernel).
+extern "C" int morl_gemm_chain_pairs_f32(int n_chains, int n_layers, const float* const* u, const float* const* v, int B, int W, const void* const* acts,
+                                         long long act_plane_stride, const float* act_scale, const void* const* w_planes, long long w_plane_stride,
+                                         const float* const* w_scales, const float* const* biases, void* const* relu_bits_out, unsigned int store_mask,
+                                         void* stream) {
+    using namespace morl;
+    MORL_REQUIRE(u && v && w_planes, MORL_ERR_NULL, "morl_gemm_chain_pairs_f32: NULL pointer argument");
+    MORL_REQUIRE(n_chains >= 1 && n_chains <= 2 && n_layers >= 1 && n_chains * n_layers <= kChainMaxJobs, MORL_ERR_SHAPE,
+                 "morl_gemm_chain_pairs_f32: need 1 <= n_chains <= 2 and n_chains * n_layers <= %d (got %d x %d)", kChainMaxJobs, n_chains, n_layers);
+    MORL_REQUIRE(B > 0 && W > 0 && (long long)B * W <= 0x7fffffffLL && morl_gemm_chain_supported(MORL_FMT_F16X2, B * W, 256), MORL_ERR_SHAPE,
+                 "morl_gemm_chain_pairs_f32: bad shape B=%d W=%d (need B W >= 256)", B, W);
+    MORL_REQUIRE(store_mask < (1u << (n_chains * n_layers)), MORL_ERR_SHAPE, "morl_gemm_chain_pairs_f32: store_mask 0x%x names jobs beyond %d x %d", store_mask,
+                 n_chains, n_layers);
+    MORL_REQUIRE(store_mask == 0 || acts, MORL_ERR_NULL, "morl_gemm_chain_pairs_f32: stored outputs need their planes");
+    ResChainArgs g;
+    memset(&g, 0, sizeof(g));
+    g.k_first = 256;
+    g.store = store_mask;
+    g.W = W;
+    const void* outs[2 * (kChainMaxJobs + 1)] = {};
+    for (int c = 0; c < n_chains; ++c) {
+        MORL_REQUIRE(u[c] && v[c] && aligned16(u[c]) && aligned16(v[c]), MORL_ERR_ALIGN, "morl_gemm_chain_pairs_f32: u / v of chain %d NULL or not 16-byte aligned", c);
+        g.u[c] = u[c];
+        g.v[c] = v[c];
+        for (int l = 0; l < n_layers; ++l) outs[c * (n_layers + 1) + l + 1] = acts ? acts[c * n_layers + l] : nullptr;
+    }
+    return launch_chain_resident(g, n_chains, n_layers, nullptr, outs, act_plane_stride, act_scale, w_planes, w_plane_stride, w_scales, biases, 1, nullptr,
+                                 relu_bits_out, B * W, 256, "morl_gemm_chain_pairs_f32", stream);
 }

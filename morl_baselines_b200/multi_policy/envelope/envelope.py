@@ -428,9 +428,19 @@ class Envelope(MOPolicy, MOAgent):
                 if fused_head:
                     # output layers of both nets + envelope operator + Bellman line in ONE kernel: Q_on / Q_tg (envelope.py:420, :429) exist
                     # in tensor / shared memory only (csrc/qhead_envelope.cu; bit-identical to the three-launch chain below)
-                    if self._tc_on.chain_supported() and self._tc_tg.chain_supported():
-                        # hidden layers 2.. of BOTH nets in one persistent launch: a CTA takes each of its row tiles through all layers of
-                        # both nets, re-reading every intermediate activation from L2 (csrc/gemm_planes.cu: gemm_chain_kernel)
+                    if self._tc_on.pair_chain_supported() and self._tc_tg.pair_chain_supported():
+                        # layers 1.. of BOTH nets in one persistent launch from the first layer's (u, v): a CTA keeps each of its row
+                        # tiles in shared memory through all layers of a net, and only the last hidden activation of each net is
+                        # written (csrc/gemm_planes.cu: gemm_chain_resident_kernel)
+                        if self._nograd_chain is None:
+                            self._nograd_chain = TCPairMlp.make_pair_chain([self._tc_on, self._tc_tg])
+                        u_on, v_on = self._tc_on.layer1_uv(nobs, wset)
+                        u_tg, v_tg = self._tc_tg.layer1_uv(nobs, wset)
+                        self._nograd_chain([u_on, u_tg], [v_on, v_tg])
+                        h_on, h_tg = self._tc_on.h[-1], self._tc_tg.h[-1]
+                        head_reverse = _HEAD_REVERSE  # the chain wrote its highest tiles last: start the head on them (still in L2)
+                    elif self._tc_on.chain_supported() and self._tc_tg.chain_supported():
+                        # hidden layers 2.. of BOTH nets in one persistent launch (bf16x3: csrc/gemm_planes.cu: gemm_chain_kernel)
                         if self._nograd_chain is None:
                             self._nograd_chain = TCPairMlp.make_chain([self._tc_on, self._tc_tg])
                         self._tc_on.layer1(nobs, wset)

@@ -698,6 +698,61 @@ class GemmChain:
         _count()
 
 
+class GemmChainPairs:
+    """Static plan of a chained launch that starts from the separable first layer (f16x2): the input of chain c is
+    relu(u[c][b] + v[c][j]) * act_scale for row b*W + j, built in shared memory (the planes :func:`pairs_relu_split` would write), then the
+    hidden layers as :class:`GemmChain`.  ``outs[c]``: per layer, the output plane tensor [P, B*W, 256], or None when that output is not
+    needed -- only the others are written to memory; ``weights`` / ``biases`` / ``w_scales`` / ``bits`` as :class:`GemmChain`.  A call takes
+    the per-chain u [B, 256] and v [W, 256] (fp32, contiguous) of that pass."""
+
+    def __init__(self, outs, weights, B: int, W: int, biases=None, w_scales=None, bits=None, act_scale=None):
+        import ctypes as C
+
+        self.n_chains, self.n_layers = len(outs), len(weights[0])
+        self.B, self.W, self.M = int(B), int(W), int(B) * int(W)
+        flat_o = [t for ch in outs for t in ch]
+        flat_w = [t for ch in weights for t in ch]
+        flat_b = [None] * len(flat_w) if biases is None else [t.detach() for ch in biases for t in ch]
+        flat_s = [None] * len(flat_w) if w_scales is None else [t for ch in w_scales for t in ch]
+        flat_m = [None] * len(flat_w) if bits is None else [t for ch in bits for t in ch]
+        if len(flat_o) != len(flat_w) or any(len(w) != self.n_layers for w in weights) or any(len(o) != self.n_layers for o in outs):
+            raise _lib.MorlB200Error("GemmChainPairs: every chain needs n_layers outputs (or None) and n_layers weight tensors")
+        for t in flat_w:
+            if fmt_of(t) != FMT_F16X2 or tuple(t.shape[1:]) != (256, 256) or not t.is_contiguous():
+                raise _lib.MorlB200Error("GemmChainPairs: weight planes must be contiguous f16x2 [2, 256, 256]")
+        stored = [t for t in flat_o if t is not None]
+        for t in stored:
+            if fmt_of(t) != FMT_F16X2 or tuple(t.shape[1:]) != (self.M, 256) or not t.is_contiguous() or not t.is_cuda:
+                raise _lib.MorlB200Error(f"GemmChainPairs: output planes must be contiguous CUDA f16x2 tensors [2, {self.M}, 256]")
+        if any(t.stride(0) != stored[0].stride(0) for t in stored):
+            raise _lib.MorlB200Error("GemmChainPairs: output planes need one plane stride")
+        for t in flat_m:
+            if t is not None and (t.dtype != th.int32 or tuple(t.shape) != (self.M, relu_bits_words(256)) or not t.is_contiguous()):
+                raise _lib.MorlB200Error(f"GemmChainPairs: ReLU bit masks must be contiguous int32 [{self.M}, {relu_bits_words(256)}]")
+        self.store = sum(1 << i for i, t in enumerate(flat_o) if t is not None)
+        self._keep = (flat_o, flat_w, flat_b, flat_s, flat_m, act_scale)
+        arr = lambda ts: (C.c_void_p * len(ts))(*[None if t is None else t.data_ptr() for t in ts])  # noqa: E731
+        self._po, self._pw, self._pb, self._ps, self._pm = arr(flat_o), arr(flat_w), arr(flat_b), arr(flat_s), arr(flat_m)
+        self._o_stride = stored[0].stride(0) if stored else 0
+        self._w_stride, self._act_scale = flat_w[0].stride(0), act_scale
+
+    def __call__(self, us, vs):
+        import ctypes as C
+
+        if len(us) != self.n_chains or len(vs) != self.n_chains:
+            raise _lib.MorlB200Error(f"GemmChainPairs: need u and v of {self.n_chains} chains")
+        for u, v in zip(us, vs):
+            if (u.dtype != th.float32 or v.dtype != th.float32 or tuple(u.shape) != (self.B, 256) or tuple(v.shape) != (self.W, 256)
+                    or not u.is_contiguous() or not v.is_contiguous() or not u.is_cuda or not v.is_cuda):
+                raise _lib.MorlB200Error(f"GemmChainPairs: u / v must be contiguous CUDA float32 [{self.B}, 256] / [{self.W}, 256]")
+        pu = (C.c_void_p * self.n_chains)(*[u.data_ptr() for u in us])
+        pv = (C.c_void_p * self.n_chains)(*[v.data_ptr() for v in vs])
+        rc = _lib.load().morl_gemm_chain_pairs_f32(self.n_chains, self.n_layers, pu, pv, self.B, self.W, self._po, self._o_stride, _ptr(self._act_scale),
+                                                   self._pw, self._w_stride, self._ps, self._pb, self._pm, self.store, _stream())
+        _lib.check(rc, "morl_gemm_chain_pairs_f32")
+        _count()
+
+
 def qhead_gemm_supported(fmt: int, M: int, N: int, K: int) -> bool:
     return bool(_lib.load().morl_qhead_gemm_supported(int(fmt), int(M), int(N), int(K)))
 

@@ -5,8 +5,9 @@
 
     layer 1   : u = feats @ W1[:, :F]^T (B rows), v = wset @ W1[:, F:]^T + b1 (W rows)  -- one launch (morl_pair_layer1_uv_f32) --
                  h1[b*W + j] = relu(u[b] + v[j]) written straight into operand planes (morl_pairs_relu_split_planes);
-    layers 2..: the 256-wide hidden layers of a pass as ONE chained launch (morl_gemm_chain_f32: a CTA takes its row tiles through
-                 all layers, intermediate activations re-read from L2; both no-grad nets together) -- or, for other widths, one
+    layers 2..: the 256-wide hidden layers of a pass as ONE chained launch (morl_gemm_chain_f32: a CTA keeps its row tile in shared
+                 memory through all layers; the no-grad passes of both nets together start from (u, v) and write only the last hidden
+                 activation, morl_gemm_chain_pairs_f32) -- or, for other widths, one
                  morl_gemm_planes_f32 launch per layer (TMA -> wgmma -> register accumulators -> epilogue, activation re-split fused in the epilogue);
                  the last layer writes fp32 Q-values (morl_qhead_gemm_f32 when it is <= 32 wide) or is consumed, together with the other
                  network's, by the fused head (morl_qhead_envelope_td_f32: Q never reaches HBM).
@@ -232,6 +233,24 @@ class TCPairMlp:
         u, v = ops.pair_layer1_uv(feats, wset, first.weight.detach(), first.bias.detach())
         hb = self.hbits if self.trainable else [None] * len(self.h)
         return ops.pairs_relu_split(u, v, out=self.h[0], scale=self.s_act, relu_bits_out=hb[0])
+
+    def layer1_uv(self, feats: th.Tensor, wset: th.Tensor):
+        """(u, v) of the separable first layer: the input of :meth:`make_pair_chain`'s launch."""
+        first = self.lin[0]
+        return ops.pair_layer1_uv(feats, wset, first.weight.detach(), first.bias.detach())
+
+    def pair_chain_supported(self) -> bool:
+        """Layers 1 .. n-1 of a no-grad pass as ONE launch from (u, v) (ops.GemmChainPairs, f16x2)."""
+        return self.fmt == ops.FMT_F16X2 and self.chain_supported()
+
+    @staticmethod
+    def make_pair_chain(plans):
+        """One launch for layers 1 .. n-1 of one plan or of two plans of equal shape (the two no-grad passes), started from each plan's
+        (u, v): h[0] is built in shared memory and only the LAST hidden activation h[-1] is written (the operand of the output layer)."""
+        specs = [p.chain_spec() for p in plans]
+        outs = [[None] * (len(sp[0]) - 2) + [sp[0][-1]] for sp in specs]
+        return ops.GemmChainPairs(outs, [sp[1] for sp in specs], plans[0].B, plans[0].W, [sp[2] for sp in specs], [sp[3] for sp in specs],
+                                  act_scale=plans[0].s_act)
 
     def chain_spec(self):
         """(activations, weight planes, biases, weight scales, ReLU bit tensors) of the hidden layers 2.. for ops.GemmChain."""
