@@ -517,6 +517,41 @@ MORL_API size_t morl_adam_workspace_bytes(int n_tensors, int64_t max_size);
 MORL_API int morl_adam_clip_f32(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,
                                 float* const* steps, const int64_t* sizes, int n_tensors, int64_t max_size, float max_grad_norm,
                                 float lr, float beta1, float beta2, float eps, void* workspace, void* stream);
+/* morl_adam_clip_lr_f32: the same step with the learning rate read at run time from the device double *lr (a CUDA graph captured once
+ * follows a learning-rate schedule); step_size = (float)(*lr / (1 - beta1^t)) as Python forms it from a float lr. */
+MORL_API int morl_adam_clip_lr_f32(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,
+                                   float* const* steps, const int64_t* sizes, int n_tensors, int64_t max_size, float max_grad_norm,
+                                   const double* lr, float beta1, float beta2, float eps, void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * MO-PPO (reference single_policy/ser/mo_ppo.py), csrc/ppo.cu.
+ *
+ * morl_vector_gae_f32 (:439-476): rewards, values f32 [T, E, D], dones f32 [T, E], next_value f32 [E, D], next_done f32 [E],
+ *   weights f32 [D].  With nnt_t = 1 - dones[t + 1] (1 - next_done for t = T - 1) and nv_t = values[t + 1] (next_value for T - 1),
+ *   every operation rounded once, in the reference's order (g = (float)gamma, gl = (float)(gamma * gae_lambda)):
+ *     use_gae = 1: delta = (r + (g * nv) * nnt) - v;  lastgaelam = delta + (gl * nnt) * lastgaelam  (0 before the last step);
+ *                  returns = lastgaelam + v;  advantage vector = lastgaelam
+ *     use_gae = 0: returns[t] = r + (g * nnt) * returns[t + 1]  (next_value for T - 1);  advantage vector = returns - v
+ *   so returns [T, E, D] are bit-exact against the reference.  advantages [T, E] = advantage vector . weights, summed in double and
+ *   rounded once (the reference's matmul may round differently).  D <= MORL_MAX_D.
+ *
+ * morl_ppo_loss_f32 (:514-549): one minibatch of M rows in ONE CTA.  mean f32 [M, A] (actor output), logstd f32 [A], value f32 [M, D]
+ *   (critic output), actions [M, A], old_logprob [M], advantages [M] (raw, scalarised), returns and old_values [M, D] (old_values
+ *   may be NULL without clip_vloss).  sigma = exp(logstd); logp = sum_j Normal(mean, sigma).log_prob(action); ratio = exp(logp - old);
+ *   advantages normalised by torch's unbiased std() + 1e-8 when norm_adv (refused for M < 2); pg_loss = mean max(-adv ratio,
+ *   -adv clamp(ratio, 1 -+ clip)); v_loss = 0.5 mean over M*D of (v - R)^2, or of max((v - R)^2, (clip(v) - R)^2) with clip_vloss;
+ *   entropy = sum_j (0.5 + 0.5 log 2pi + logstd_j);  loss_out[0] = pg_loss - ent_coef * entropy + v_loss * vf_coef.
+ *   dmean [M, A], dlogstd [A], dvalue [M, D]: d loss_out / d input, with torch's backward rules: th.max splits the gradient half and
+ *   half on a tie, clamp passes it on its closed interval.  stats f32 [6]: pg_loss, v_loss, entropy, old_approx_kl, approx_kl are
+ *   written; stats[5] += the clip fraction (a sum over the minibatches of an update; zero it before the first).  Reductions are fixed
+ *   block trees in double (deterministic).  A <= 32, D <= MORL_MAX_D. */
+MORL_API int morl_vector_gae_f32(const float* rewards, const float* values, const float* dones, const float* next_value, const float* next_done,
+                                 const float* weights, int T, int E, int D, double gamma, double gae_lambda, int use_gae, float* returns,
+                                 float* advantages, void* stream);
+MORL_API int morl_ppo_loss_f32(const float* mean, const float* logstd, const float* value, const float* actions, const float* old_logprob,
+                               const float* advantages, const float* returns, const float* old_values, int M, int A, int D, float clip_coef,
+                               float ent_coef, float vf_coef, int norm_adv, int clip_vloss, float* loss_out, float* dmean, float* dlogstd,
+                               float* dvalue, float* stats, void* stream);
 
 #ifdef __cplusplus
 }

@@ -86,6 +86,9 @@ SIGNATURES = {
     "morl_pair_layer1_grad_f32": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "morl_adam_workspace_bytes": (_sz, [_i, _i64]),
     "morl_adam_clip_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i64, _f, _f, _f, _f, _f, _vp, _vp]),
+    "morl_adam_clip_lr_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i64, _f, _vp, _f, _f, _f, _vp, _vp]),
+    "morl_vector_gae_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _d, _d, _i, _vp, _vp, _vp]),
+    "morl_ppo_loss_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _f, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
 }
 
 SPLIT_MAX_JOBS = 16

@@ -23,6 +23,9 @@ class FusedClipAdam(optim.Adam):
         self._tables = None
         self._cache = {}   # tables referenced by captured CUDA graphs (one per capture)
         self._eager = None  # the single overwritable table of the eager path
+        # optional float64 device scalar: when set, step_fused reads the learning rate from it at run time instead of from param_groups,
+        # so a captured graph follows a schedule written into it
+        self.lr_device: Optional[th.Tensor] = None
 
     def load_state_dict(self, state_dict):
         """``optim.Adam.load_state_dict`` replaces the state tensors: the cached pointer tables (which hold their addresses) are dropped."""
@@ -102,6 +105,16 @@ class FusedClipAdam(optim.Adam):
             self._build_tables(params)
         t = self._tables
         b1, b2 = group["betas"]
+        if self.lr_device is not None:
+            if not (self.lr_device.is_cuda and self.lr_device.dtype == th.float64 and self.lr_device.numel() == 1):
+                raise _lib.MorlB200Error("FusedClipAdam.lr_device must be a float64 CUDA tensor with one element")
+            rc = _lib.load().morl_adam_clip_lr_f32(t["p"].data_ptr(), t["g"].data_ptr(), t["m"].data_ptr(), t["v"].data_ptr(), t["s"].data_ptr(),
+                                                   t["n"].data_ptr(), len(params), t["max"],
+                                                   float(max_grad_norm) if max_grad_norm is not None else 0.0, self.lr_device.data_ptr(),
+                                                   float(b1), float(b2), float(group["eps"]), t["ws"].data_ptr(), th.cuda.current_stream().cuda_stream)
+            _lib.check(rc, "morl_adam_clip_lr_f32")
+            ops._count(2)
+            return
         rc = _lib.load().morl_adam_clip_f32(t["p"].data_ptr(), t["g"].data_ptr(), t["m"].data_ptr(), t["v"].data_ptr(), t["s"].data_ptr(),
                                             t["n"].data_ptr(), len(params), t["max"], float(max_grad_norm) if max_grad_norm is not None else 0.0,
                                             float(group["lr"]), float(b1), float(b2), float(group["eps"]), t["ws"].data_ptr(),

@@ -78,7 +78,7 @@ __global__ void __launch_bounds__(kOptBlock) adam_clip_kernel(float* const* __re
                                                               float* const* __restrict__ exp_avg, float* const* __restrict__ exp_avg_sq,
                                                               float* const* __restrict__ steps, const int64_t* __restrict__ sizes,
                                                               const float* __restrict__ partials, int n_partials, float max_norm, float lr,
-                                                              float beta1, float beta2, float eps) {
+                                                              const double* __restrict__ lr_dev, float beta1, float beta2, float eps) {
     pdl_enter();
     __shared__ float s_coef;
     __shared__ double s_red[kOptBlock / 32];
@@ -107,7 +107,7 @@ __global__ void __launch_bounds__(kOptBlock) adam_clip_kernel(float* const* __re
     const double step = (double)*steps[t];
     const double bc1 = 1.0 - pow((double)beta1, step);
     const double bc2 = 1.0 - pow((double)beta2, step);
-    const float step_size = (float)((double)lr / bc1);
+    const float step_size = (float)((lr_dev ? *lr_dev : (double)lr) / bc1);
     const float bc2_sqrt = (float)sqrt(bc2);
     float* __restrict__ p = params[t];
     const float* __restrict__ g = grads[t];
@@ -134,9 +134,9 @@ extern "C" size_t morl_adam_workspace_bytes(int n_tensors, int64_t max_size) {
     return (size_t)n_tensors * (size_t)bx * sizeof(float);
 }
 
-extern "C" int morl_adam_clip_f32(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,
-                                  float* const* steps, const int64_t* sizes, int n_tensors, int64_t max_size, float max_grad_norm, float lr,
-                                  float beta1, float beta2, float eps, void* workspace, void* stream) {
+static int adam_clip(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq, float* const* steps,
+                     const int64_t* sizes, int n_tensors, int64_t max_size, float max_grad_norm, float lr, const double* lr_dev, float beta1,
+                     float beta2, float eps, void* workspace, void* stream) {
     using namespace morl;
     MORL_REQUIRE(params && grads && exp_avg && exp_avg_sq && steps && sizes && workspace, MORL_ERR_NULL, "morl_adam_clip_f32: NULL pointer argument");
     MORL_REQUIRE(n_tensors > 0 && n_tensors <= 65535 && max_size > 0, MORL_ERR_SHAPE, "morl_adam_clip_f32: bad n_tensors=%d max_size=%lld", n_tensors,
@@ -149,7 +149,23 @@ extern "C" int morl_adam_clip_f32(float* const* params, const float* const* grad
     launch_k(grad_sqnorm_kernel, dim3(grid), dim3(kOptBlock), 0, st, grads, sizes, steps, partials);
     int rc = check_launch("morl_adam_clip_f32(norm)");
     if (rc) return rc;
-    launch_k(adam_clip_kernel, dim3(grid), dim3(kOptBlock), 0, st, params, grads, exp_avg, exp_avg_sq, steps, sizes, partials, (int)(bx * n_tensors), max_grad_norm, lr, beta1,
-                                                 beta2, eps);
+    launch_k(adam_clip_kernel, dim3(grid), dim3(kOptBlock), 0, st, params, grads, exp_avg, exp_avg_sq, steps, sizes, partials, (int)(bx * n_tensors), max_grad_norm, lr, lr_dev,
+                                                 beta1, beta2, eps);
     return check_launch("morl_adam_clip_f32");
+}
+
+extern "C" int morl_adam_clip_f32(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,
+                                  float* const* steps, const int64_t* sizes, int n_tensors, int64_t max_size, float max_grad_norm, float lr,
+                                  float beta1, float beta2, float eps, void* workspace, void* stream) {
+    return adam_clip(params, grads, exp_avg, exp_avg_sq, steps, sizes, n_tensors, max_size, max_grad_norm, lr, nullptr, beta1, beta2, eps, workspace,
+                     stream);
+}
+
+// The same update with the learning rate read from a device double at run time, so a captured graph follows a schedule (PPO's anneal_lr)
+// without a re-capture.  A double keeps the Python float the reference's optimiser divides by its bias correction.
+extern "C" int morl_adam_clip_lr_f32(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,
+                                     float* const* steps, const int64_t* sizes, int n_tensors, int64_t max_size, float max_grad_norm,
+                                     const double* lr, float beta1, float beta2, float eps, void* workspace, void* stream) {
+    MORL_REQUIRE(lr, MORL_ERR_NULL, "morl_adam_clip_lr_f32: NULL learning rate");
+    return adam_clip(params, grads, exp_avg, exp_avg_sq, steps, sizes, n_tensors, max_size, max_grad_norm, 0.f, lr, beta1, beta2, eps, workspace, stream);
 }

@@ -206,6 +206,64 @@ def discrete_sac_actor_loss(logits, q_nets, w, alpha: th.Tensor, log_alpha: Opti
     return loss, grad, aloss, dla
 
 
+def vector_gae(rewards, values, dones, next_value, next_done, weights, gamma: float, gae_lambda: float, gae: bool = True,
+               returns_out: Optional[th.Tensor] = None, adv_out: Optional[th.Tensor] = None):
+    """MO-PPO's reverse GAE recursion (reference mo_ppo.py:439-476) in one launch.  rewards / values [T, E, D], dones [T, E],
+    next_value [E, D], next_done [E], weights [D]; ``gae=False`` gives the plain discounted returns.  Returns (returns [T, E, D],
+    scalarised advantages [T, E]), written into ``returns_out`` / ``adv_out`` when given."""
+    rewards, values, dones = _dev(rewards, "rewards"), _dev(values, "values"), _dev(dones, "dones")
+    if rewards.dim() != 3 or values.shape != rewards.shape:
+        raise _lib.MorlB200Error(f"rewards / values must both be [T, E, D], got {tuple(rewards.shape)} and {tuple(values.shape)}")
+    T, E, D = rewards.shape
+    if tuple(dones.shape) != (T, E):
+        raise _lib.MorlB200Error(f"dones must be [{T}, {E}], got {tuple(dones.shape)}")
+    next_value, next_done, weights = _dev(next_value, "next_value").reshape(-1), _dev(next_done, "next_done").reshape(-1), _dev(weights, "weights").reshape(-1)
+    if next_value.numel() != E * D or next_done.numel() != E or weights.numel() != D:
+        raise _lib.MorlB200Error(f"next_value / next_done / weights must have {E * D} / {E} / {D} elements")
+    ret = th.empty_like(rewards) if returns_out is None else returns_out
+    adv = th.empty((T, E), device=rewards.device, dtype=th.float32) if adv_out is None else adv_out
+    for t, shape, name in ((ret, (T, E, D), "returns_out"), (adv, (T, E), "adv_out")):
+        if t.dtype != th.float32 or not t.is_cuda or not t.is_contiguous() or t.numel() != T * E * (D if name == "returns_out" else 1):
+            raise _lib.MorlB200Error(f"{name} must be a contiguous float32 CUDA tensor of shape {shape}")
+    rc = _lib.load().morl_vector_gae_f32(_ptr(rewards), _ptr(values), _ptr(dones), _ptr(next_value), _ptr(next_done), _ptr(weights), T, E, D,
+                                         float(gamma), float(gae_lambda), int(bool(gae)), _ptr(ret), _ptr(adv), _stream())
+    _lib.check(rc, "morl_vector_gae_f32")
+    _count()
+    return ret, adv
+
+
+def ppo_loss(mean, logstd, value, actions, old_logprob, advantages, returns, old_values, clip_coef: float, ent_coef: float, vf_coef: float,
+             norm_adv: bool, clip_vloss: bool, stats: th.Tensor, out: Optional[Tuple[th.Tensor, th.Tensor, th.Tensor, th.Tensor]] = None):
+    """One minibatch's MO-PPO loss and its gradients (reference mo_ppo.py:514-549) in one launch.  mean [M, A], logstd [A] (or [1, A]),
+    value [M, D], actions [M, A], old_logprob [M], advantages [M], returns / old_values [M, D]; ``stats`` a float32 device vector of 6
+    (pg_loss, v_loss, entropy, old_approx_kl, approx_kl written; clip fraction added).  Returns (loss [1], dmean [M, A], dlogstd [A],
+    dvalue [M, D]), written into ``out`` when given."""
+    mean, value, actions = _dev(mean, "mean"), _dev(value, "value"), _dev(actions, "actions")
+    M, A = mean.shape
+    D = value.shape[-1]
+    logstd = _dev(logstd, "logstd").reshape(-1)
+    value = value.reshape(-1, D)
+    old_logprob, advantages = _dev(old_logprob, "old_logprob").reshape(-1), _dev(advantages, "advantages").reshape(-1)
+    returns = _dev(returns, "returns").reshape(-1, D)
+    old_values = _dev(old_values, "old_values").reshape(-1, D) if old_values is not None else None
+    if (tuple(actions.shape) != (M, A) or logstd.numel() != A or value.shape[0] != M or old_logprob.numel() != M or advantages.numel() != M
+            or returns.shape[0] != M or (old_values is not None and old_values.shape[0] != M)):
+        raise _lib.MorlB200Error("ppo_loss: inconsistent shapes")
+    stats = _dev(stats, "stats")
+    if stats.numel() != 6:
+        raise _lib.MorlB200Error("ppo_loss: stats must have 6 elements")
+    dev = mean.device
+    if out is None:
+        out = (th.empty(1, device=dev), th.empty_like(mean), th.empty(A, device=dev), th.empty((M, D), device=dev))
+    loss, dmean, dlogstd, dvalue = out
+    rc = _lib.load().morl_ppo_loss_f32(_ptr(mean), _ptr(logstd), _ptr(value), _ptr(actions), _ptr(old_logprob), _ptr(advantages), _ptr(returns),
+                                       _ptr(old_values), M, A, D, float(clip_coef), float(ent_coef), float(vf_coef), int(bool(norm_adv)),
+                                       int(bool(clip_vloss)), _ptr(loss), _ptr(dmean), _ptr(dlogstd), _ptr(dvalue), _ptr(stats), _stream())
+    _lib.check(rc, "morl_ppo_loss_f32")
+    _count()
+    return loss, dmean, dlogstd, dvalue
+
+
 def td_workspace(n_rows: int, device) -> th.Tensor:
     nbytes = _lib.load().morl_td_workspace_bytes(int(n_rows))
     return th.empty((nbytes + 3) // 4, device=device, dtype=th.float32)

@@ -2,10 +2,10 @@
 
     compute-sanitizer --tool memcheck|racecheck|synccheck|initcheck python scripts/sanitize_all.py [group ...]
 
-groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners (default: all).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
+groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners ppo (default: all).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
 every code path: all envelope kernel families, both GEMM operand formats x CTA modes x accumulator modes, MN split-K GEMM with the fused
 column sums, every split / reduction helper, the loss kernels (discrete SAC's included), Adam, polyak, Pareto + front records, replay gather,
-the corner-weight enumeration."""
+the corner-weight enumeration, MO-PPO's vector GAE and loss (racecheck: the loss kernel's CTA reductions)."""
 import os
 import sys
 
@@ -23,7 +23,7 @@ if os.environ.get("SAN_ZERO_PLANES") == "1":
     # from a genuine read of memory nobody wrote.
     _empty = ops.empty_planes
     ops.empty_planes = lambda *a, **k: _empty(*a, **k).zero_()
-groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain", "corners"}
+groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain", "corners", "ppo"}
 
 
 def rn(*s, scale=1.0):
@@ -208,4 +208,16 @@ if "corners" in groups:
         ops.corner_weights(V, cap=1)
     th.cuda.synchronize()
     print("corners ok")
+if "ppo" in groups:
+    # vector GAE (csrc/ppo.cu): more steps than one shared-memory chunk, env counts that leave a CTA partly idle, both modes; the loss:
+    # more rows than threads, A at its limit, both value-loss forms, and a device learning rate for the Adam that follows it
+    for T, E, D in [(130, 5, 3), (1, 1, 8), (64, 33, 1)]:
+        for gae in (True, False):
+            ops.vector_gae(rn(T, E, D), rn(T, E, D), (th.rand(T, E, device=dev, generator=g) < 0.1).float(), rn(E, D), th.ones(E, device=dev),
+                           th.rand(D, device=dev, generator=g), 0.99, 0.95, gae)
+    stats = th.zeros(6, device=dev)
+    for M, A, D, cv in [(300, 32, 2, True), (2, 1, 1, False), (257, 6, 3, True)]:
+        ops.ppo_loss(rn(M, A), rn(A, scale=0.3), rn(M, D), rn(M, A), rn(M), rn(M), rn(M, D), rn(M, D), 0.2, 0.01, 0.5, True, cv, stats)
+    th.cuda.synchronize()
+    print("ppo ok")
 print("sanitize run ok")
