@@ -432,6 +432,26 @@ MORL_API int morl_debug_gemm_stats(unsigned long long* out8, int reset);
 MORL_API int morl_ensemble_sample_f32(const float* out, const float* max_logvar, const float* min_logvar, const int32_t* model_idx, const float* noise,
                                       const float* obs, int rew_dim, int E, int N, int O, float* sample_out, float* var_out, float* uncertainty_out,
                                       void* stream);
+/* One imagined Dyna step, from the raw ensemble output to rows of the model replay buffer, in two launches (csrc/dyna.cu): the sample and
+ * uncertainty of morl_ensemble_sample_f32 (same per-row arithmetic, same bits; obs always added), the termination rule, the uncertainty gate, the
+ * ring append of the kept rows and the compaction of the alive rows (reference gpi_pd_continuous_action.py:346-366).
+ *   out, max_logvar, min_logvar, model_idx, noise: as morl_ensemble_sample_f32;  obs [N, S], act [N, A]: the step's inputs, S = O - rew_dim;
+ *   rule: MORL_TERM_* on (obs, act, s' = sample[rew_dim:], r = sample[:rew_dim]); a rule whose columns S / rew_dim lack is MORL_ERR_SHAPE;
+ *   a row is kept iff uncertainty < max_uncertainty (strict: NaN is never kept);
+ *   st_obs [capacity, S], st_next_obs [capacity, S], st_act [capacity, A], st_rew [capacity, rew_dim], st_done [capacity] (0.0 / 1.0): the ring,
+ *     written as `kept` sequential adds starting at slot ptr would leave it (with kept > capacity only the last capacity rows; no slot twice);
+ *   next_alive [N, S]: s' of the rows with done == 0, in row order;  uncertainty_out [N];  counts_out [2] = {kept, alive}, on the device.
+ * Deterministic, no host synchronisation, capture-safe.  workspace: morl_dyna_commit_workspace_bytes(N) bytes, no initialisation required. */
+#define MORL_TERM_NONE 0        /* halfcheetah, reacher, highway */
+#define MORL_TERM_HOPPER 1      /* done unless s' finite, s'[1:] < 100, s'[0] > 0.7, |s'[1]| < 0.2 */
+#define MORL_TERM_HUMANOID 2    /* done unless 1 < s'[0] < 2 */
+#define MORL_TERM_MOUNTAINCAR 3 /* done iff s'[0] >= 0.45 and s'[1] >= 0 */
+#define MORL_TERM_LUNARLANDER 4 /* done iff |s'[0]| >= 1, or r[0] != 0 and s'[6] >= 0.95 and s'[7] >= 0.95 */
+MORL_API size_t morl_dyna_commit_workspace_bytes(int N);
+MORL_API int morl_dyna_commit_f32(const float* out, const float* max_logvar, const float* min_logvar, const int32_t* model_idx, const float* noise,
+                                  const float* obs, const float* act, int rew_dim, int E, int N, int O, int A, int rule, float max_uncertainty,
+                                  float* st_obs, float* st_next_obs, float* st_act, float* st_rew, float* st_done, int capacity, int ptr,
+                                  float* next_alive, float* uncertainty_out, int32_t* counts_out, void* workspace, void* stream);
 
 /* Output layer of BOTH Q-networks + envelope operator + Bellman line as ONE kernel (csrc/qhead_envelope.cu): replaces, for the two no-grad
  * passes of Envelope.update (reference envelope.py:420, :429, :422-440, :298),

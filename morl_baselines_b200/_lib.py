@@ -69,6 +69,8 @@ SIGNATURES = {
     "morl_gemm_chain_pairs_f32": (_i, [_i, _i, _vp, _vp, _i, _i, _vp, C.c_longlong, _vp, _vp, C.c_longlong, _vp, _vp, _vp, C.c_uint, _vp]),
     "morl_debug_gemm_stats": (_i, [_vp, _i]),
     "morl_ensemble_sample_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "morl_dyna_commit_workspace_bytes": (_sz, [_i]),
+    "morl_dyna_commit_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "morl_qhead_envelope_supported": (_i, [_i, _i, _i, _i, _i, _i]),
     "morl_qhead_gemm_supported": (_i, [_i, _i, _i, _i]),
     "morl_qhead_gemm_f32": (_i, [_i, _vp, C.c_longlong, _vp, _vp, C.c_longlong, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),

@@ -12,6 +12,8 @@ from typing import Tuple
 import numpy as np
 import torch as th
 
+from ... import ops
+
 
 def termination_fn_false(obs, act, next_obs, rew):
     return th.zeros((obs.shape[0], 1), dtype=th.bool, device=obs.device)
@@ -52,27 +54,40 @@ def termination_fn_humanoid(obs, act, next_obs, rew):
     return (~not_done)[:, None]
 
 
+# env id -> (rule, rule id of the fused device step ``ops.dyna_commit`` or None where it has none): the reference's ModelEnv.__init__ table
+# (utils.py:119-138), first match wins.  Minecart and deep-sea-treasure are discrete-action environments and have no device rule.
+_RULE_TABLE = (
+    (lambda e: "hopper" in e, termination_fn_hopper, ops.TERM_HOPPER),
+    (lambda e: "halfcheetah" in e, termination_fn_false, ops.TERM_NONE),
+    (lambda e: "humanoid" in e, termination_fn_humanoid, ops.TERM_HUMANOID),
+    (lambda e: "lunar-lander" in e, termination_fn_lunarlander, ops.TERM_LUNARLANDER),
+    (lambda e: "mo-reacher" in e, termination_fn_false, ops.TERM_NONE),
+    (lambda e: "mountaincar" in e, termination_fn_mountaincar, ops.TERM_MOUNTAINCAR),
+    (lambda e: "minecart" in e, termination_fn_minecart, None),
+    (lambda e: e == "mo-highway-fast-v0" or e == "mo-highway-v0", termination_fn_false, ops.TERM_NONE),
+    (lambda e: e == "deep-sea-treasure-v0", termination_fn_dst, None),
+)
+
+
+def _rule_entry(env_id: str):
+    for matches, fn, rule_id in _RULE_TABLE:
+        if matches(env_id):
+            return fn, rule_id
+    raise NotImplementedError(f"no termination rule for environment {env_id!r}")
+
+
 def termination_fn_for(env_id: str):
     """Rule table of the reference's ModelEnv.__init__ (utils.py:119-138)."""
-    if "hopper" in env_id:
-        return termination_fn_hopper
-    if "halfcheetah" in env_id:
-        return termination_fn_false
-    if "humanoid" in env_id:
-        return termination_fn_humanoid
-    if "lunar-lander" in env_id:
-        return termination_fn_lunarlander
-    if "mo-reacher" in env_id:
-        return termination_fn_false
-    if "mountaincar" in env_id:
-        return termination_fn_mountaincar
-    if "minecart" in env_id:
-        return termination_fn_minecart
-    if env_id == "mo-highway-fast-v0" or env_id == "mo-highway-v0":
-        return termination_fn_false
-    if env_id == "deep-sea-treasure-v0":
-        return termination_fn_dst
-    raise NotImplementedError
+    return _rule_entry(env_id)[0]
+
+
+def termination_rule_id(env_id: str) -> int:
+    """The ``ops.TERM_*`` id of ``env_id``'s termination rule, for the fused rollout step; NotImplementedError when the environment has no
+    rule, or only one that the device step does not implement (minecart, deep-sea-treasure)."""
+    rule_id = _rule_entry(env_id)[1]
+    if rule_id is None:
+        raise NotImplementedError(f"the termination rule of {env_id!r} has no device form (discrete-action environments only)")
+    return rule_id
 
 
 class ModelEnv:

@@ -15,8 +15,13 @@ Hot-path row a11 of SURVEY.md section 8 (BASELINE.json configs[2]: GPI-PD on mo-
   the delayed actor step -- is captured in CUDA graphs over static index / weight / noise buffers (``use_cuda_graph``,
   common/graphed.py); per update the host only walks the PER sum-tree, replays one graph and writes the priorities back.
 
-The Dyna path (probabilistic ensemble + ModelEnv, :348-391 and :545-562) is outside the accelerated hot path (SURVEY.md section 2,
-component 20): ``dyna=True`` raises, use ``GPILSContinuousAction`` / ``dyna=False``.
+The Dyna path (``dyna=True``, the reference's default; :216-235, :336-371, :548-562): the probabilistic ensemble is fitted on the real
+transitions (``ProbabilisticEnsemble.fit``, device-resident), and every imagined step of ``_rollout_dynamics`` is one actor forward, one
+ensemble forward and ONE fused commit (``morl_dyna_commit_f32``: sample, termination rule, uncertainty gate, ring append into the model
+buffer's HBM store, compaction of the alive rows) followed by a read-back of two counts -- the reference appends the survivors row by row in
+a python loop.  Mixed real / imagined minibatches take the same CUDA-graph path as real ones (two gathers into one batch).  The termination
+rule is resolved at construction (``termination_rule_id``): an environment without one raises there, not at the first rollout.
+``visualize_eval`` (matplotlib) is not mirrored.
 """
 
 from __future__ import annotations
@@ -35,6 +40,8 @@ from ... import ops
 from ...common.buffer import ReplayBuffer
 from ...common.fused_adam import FusedClipAdam
 from ...common.graphed import GraphedStep, optimizer_tensors
+from ...common.model_based.probabilistic_ensemble import ProbabilisticEnsemble
+from ...common.model_based.utils import termination_rule_id
 from ...common.morl_algorithm import MOAgent, MOPolicy
 from ...common.networks import layer_init, mlp, polyak_update
 from ...common.prioritized_buffer import PrioritizedReplayBuffer
@@ -96,9 +103,6 @@ class GPIPDContinuousAction(MOAgent, MOPolicy):
         if self.device.type != "cuda":
             raise ops._lib.MorlB200Error("morl_baselines_b200.GPIPDContinuousAction needs a CUDA device: the update path is CUDA-only "
                                          "(no CPU fallback)")
-        if dyna:
-            raise NotImplementedError("dyna=True (probabilistic ensemble + ModelEnv planning) is outside the accelerated hot path "
-                                      "(SURVEY.md section 2, component 20); use dyna=False / GPILSContinuousAction")
         ops._lib.load()
         self.learning_rate, self.tau, self.gamma = learning_rate, tau, gamma
         self.use_gpi, self.policy_noise, self.noise_clip = use_gpi, policy_noise, noise_clip
@@ -130,7 +134,15 @@ class GPIPDContinuousAction(MOAgent, MOPolicy):
         self.use_cuda_graph = use_cuda_graph
         self._graphs = {}
 
-        self.dyna, self.dynamics, self.dynamics_buffer = False, None, None  # Dyna is out of scope; the knobs are kept for get_config()
+        self.dyna, self.dynamics, self.dynamics_buffer = dyna, None, None
+        if self.dyna:
+            # resolved here, so that an environment without a termination rule fails at construction (the reference fails at the first rollout)
+            self._termination_rule = termination_rule_id(self.env.unwrapped.spec.id)
+            self.dynamics = ProbabilisticEnsemble(input_dim=self.observation_dim + self.action_dim, output_dim=self.observation_dim + self.reward_dim,
+                                                  arch=self.dynamics_net_arch, device=self.device)
+            self.dynamics_buffer = ReplayBuffer(self.observation_shape, self.action_dim, rew_dim=self.reward_dim, max_size=dynamics_buffer_size,
+                                                device=self.device)
+        self.dynamics_buffer_size = dynamics_buffer_size
         self.dynamics_train_freq, self.dynamics_rollout_len, self.dynamics_rollout_starts = dynamics_train_freq, dynamics_rollout_len, dynamics_rollout_starts
         self.dynamics_rollout_freq, self.dynamics_rollout_batch_size = dynamics_rollout_freq, dynamics_rollout_batch_size
         self.dynamics_min_uncertainty, self.dynamics_real_ratio = dynamics_min_uncertainty, dynamics_real_ratio
@@ -166,6 +178,8 @@ class GPIPDContinuousAction(MOAgent, MOPolicy):
             saved_params["target_q_net_" + str(i) + "_state_dict"] = target_q_net.state_dict()
         saved_params["q_nets_optimizer_state_dict"] = self.q_optim.state_dict()
         saved_params["M"] = self.weight_support
+        if self.dyna:
+            saved_params["dynamics_state_dict"] = self.dynamics.state_dict()
         if save_replay_buffer:
             saved_params["replay_buffer"] = self.replay_buffer
         filename = getattr(self, "experiment_name", "GPI-PD Continuous Action") if filename is None else filename
@@ -181,6 +195,8 @@ class GPIPDContinuousAction(MOAgent, MOPolicy):
             q_net.load_state_dict(params["q_net_" + str(i) + "_state_dict"])
             target_q_net.load_state_dict(params["target_q_net_" + str(i) + "_state_dict"])
         self.q_optim.load_state_dict(params["q_nets_optimizer_state_dict"])
+        if self.dyna:
+            self.dynamics.load_state_dict(params["dynamics_state_dict"])
         if load_replay_buffer and "replay_buffer" in params:
             self.replay_buffer = params["replay_buffer"]
             if hasattr(self.replay_buffer, "to"):
@@ -188,8 +204,95 @@ class GPIPDContinuousAction(MOAgent, MOPolicy):
         self._graphs = {}  # optimiser state tensors / the buffer / the support may have been replaced
 
     # ------------------------------------------------------------------------------------------ the update
+    def _uses_model_samples(self) -> bool:
+        return self.dyna and self.global_step >= self.dynamics_rollout_starts and len(self.dynamics_buffer) > 0
+
+    def _num_real(self) -> int:
+        return int(self.batch_size * self.dynamics_real_ratio) if self._uses_model_samples() else self.batch_size
+
     def _sample_batch_experiences(self):
-        return self.replay_buffer.sample(self.batch_size, to_tensor=True, device=self.device)
+        """Real minibatch, or -- once the model has been rolled out -- ``dynamics_real_ratio`` real rows followed by imagined ones (reference
+        :311-334).  Always a 6-tuple; the indices are those of the real rows."""
+        if not self._uses_model_samples():
+            return self.replay_buffer.sample(self.batch_size, to_tensor=True, device=self.device)
+        num_real = self._num_real()
+        parts, idxes = [], th.zeros(0, dtype=th.int64)
+        if num_real > 0:
+            *real, idxes = self.replay_buffer.sample(num_real, to_tensor=True, device=self.device)
+            parts.append(real)
+        if self.batch_size > num_real:
+            parts.append(self.dynamics_buffer.sample(self.batch_size - num_real, to_tensor=True, device=self.device)[:5])
+        return tuple(th.cat(cols, dim=0) for cols in zip(*parts)) + (idxes,)
+
+    @th.no_grad()
+    def _rollout_dynamics(self, weight: th.Tensor):
+        """Dyna planning (reference :336-371): ``ceil(batch / 10000)`` chunks of up to 10,000 replayed states, each rolled through the model
+        for ``dynamics_rollout_len`` steps under the target-noised policy.  A step is one actor forward, one ensemble forward, one fused
+        commit into the model buffer's device store and one read-back of {kept, alive}; the host only moves ``ptr`` / ``size``.  Random
+        numbers are consumed as in the reference: numpy for the start states and the elite draws, torch for the policy and model noise.  The
+        written ring range is copied back into the buffer's numpy arrays once, at the end."""
+        num_times = int(np.ceil(self.dynamics_rollout_batch_size / 10000))
+        batch_size = min(self.dynamics_rollout_batch_size, 10000)
+        dev, db, model, hook = self.device, self.dynamics_buffer, self.dynamics, self._noise_hook
+        S, A, D, E = self.observation_dim, self.action_dim, self.reward_dim, model.ensemble_size
+        db.flush()
+        stores = db._dev
+        ws = ops.dyna_commit_workspace(batch_size, dev)
+        alive_bufs = (th.empty(batch_size, S, device=dev), th.empty(batch_size, S, device=dev))
+        unc = th.empty(batch_size, device=dev)
+        counts = th.empty(2, dtype=th.int32, device=dev)
+        counts_pin = th.empty(2, dtype=th.int32).pin_memory()
+        stream = th.cuda.current_stream()
+        start, written, last_n = db.ptr, 0, 0
+        for _ in range(num_times):
+            obs = th.from_numpy(self.replay_buffer.sample_obs(batch_size)).to(dev)
+            n = batch_size
+            for plan_step in range(self.dynamics_rollout_len):
+                w = weight.reshape(1, -1).repeat(n, 1)
+                actions = self.policy(obs, w, noise=self.policy_noise, noise_clip=self.noise_clip, eps=hook((n, A)) if hook is not None else None)
+                out = model._raw(th.cat((obs, actions), dim=-1))
+                model_inds = np.random.choice(model.elites, size=n)
+                idx = th.from_numpy(np.ascontiguousarray(model_inds, dtype=np.int32)).to(dev, non_blocking=True)
+                noise = model._randn((E, n, S + D)).contiguous()
+                nxt = alive_bufs[plan_step % 2]
+                ops.dyna_commit(out, model.max_logvar, model.min_logvar, idx, noise, obs, actions, D, self._termination_rule, self.dynamics_min_uncertainty,
+                                stores, db.ptr, nxt[:n], unc[:n], counts, ws)
+                counts_pin.copy_(counts, non_blocking=True)
+                stream.synchronize()
+                kept, alive = (int(c) for c in counts_pin)
+                db.ptr = (db.ptr + kept) % db.max_size
+                db.size = min(db.size + kept, db.max_size)
+                written += kept
+                last_n = n
+                if alive == 0:
+                    break
+                obs, n = nxt[:alive], alive
+        # the rows written on the device form one ring interval from `start`: mirror it into the numpy arrays (async copies, one sync)
+        cnt = min(written, db.max_size)
+        first = min(cnt, db.max_size - start)
+        for h, d in zip(db._host_tensors(), stores):
+            for a, b in ((start, start + first), (0, cnt - first)):
+                if b > a:
+                    h[a:b].copy_(d[a:b], non_blocking=True)
+        stream.synchronize()
+        if self.log and last_n > 0:
+            import wandb
+
+            u = unc[:last_n].cpu().numpy()
+            wandb.log({"dynamics/uncertainty_mean": u.mean(), "dynamics/uncertainty_max": u.max(), "dynamics/uncertainty_min": u.min(),
+                       "global_step": self.global_step})
+
+    def _train_dynamics(self):
+        """Fit the ensemble on every real transition: X = [s | a], Y = [r | s' - s] (reference :548-555)."""
+        m_obs, m_actions, m_rewards, m_next_obs, _ = self.replay_buffer.get_all_data()
+        X = np.hstack((m_obs, m_actions))
+        Y = np.hstack((m_rewards, m_next_obs - m_obs))
+        mean_holdout_loss = self.dynamics.fit(X, Y)
+        if self.log:
+            import wandb
+
+            wandb.log({"dynamics/mean_holdout_loss": mean_holdout_loss, "global_step": self.global_step})
+        return mean_holdout_loss
 
     def _tile_weights(self, weight, picks, B0):
         """Effective-batch weights: ``weight`` for the first B0 rows, support weights ``picks`` for the doubled half (:381-391)."""
@@ -256,34 +359,49 @@ class GPIPDContinuousAction(MOAgent, MOPolicy):
                     s_obs, s_actions, s_rewards, s_next_obs, s_dones = (s_obs.repeat(2, 1), s_actions.repeat(2, 1), s_rewards.repeat(2, 1),
                                                                         s_next_obs.repeat(2, 1), s_dones.repeat(2, 1))
                 w = self._tile_weights(weight, picks, B0)
+                n_prio = len(idxes) if self.per else 0
                 prio = self._device_update(s_obs, s_actions, s_rewards, s_next_obs, s_dones, w, with_policy,
-                                           hook((N, self.action_dim)) if hook is not None else None, len(idxes) if self.per else 0)
-                if self.per:
+                                           hook((N, self.action_dim)) if hook is not None else None, n_prio)
+                if n_prio > 0:
                     priority = prio.cpu().numpy().flatten().clip(min=self.min_priority) ** self.alpha
                     rb.update_priorities(np.asarray(idxes.cpu() if th.is_tensor(idxes) else idxes), priority)
             else:
                 # graph path: the host walks the PER tree / draws the support picks (same RNG consumption and order as the reference),
                 # fills the static buffers, replays one graph, and writes the priorities back
-                key = (P > 1, with_policy, hook is not None, id(rb), id(self.stacked_weight_support) if P > 1 else 0)
+                # with model samples the first num_real rows of the static index buffer are real indices, the rest model-buffer indices
+                db = self.dynamics_buffer if self._uses_model_samples() else None
+                nr = self._num_real()
+                n_prio = nr if self.per else 0
+                key = (P > 1, with_policy, hook is not None, id(rb), id(self.stacked_weight_support) if P > 1 else 0, db is not None, id(db))
                 st = self._graphs.get(key)
                 if st is None:
                     st = {"host": th.zeros(2 * B0, dtype=th.int64).pin_memory(), "dev": th.zeros(2 * B0, dtype=th.int64, device=self.device),
                           "w": th.zeros(D, device=self.device), "eps": th.zeros(N, self.action_dim, device=self.device) if hook is not None else None,
                           "prio": th.zeros(B0, device=self.device), "prio_pin": th.zeros(B0).pin_memory()}
 
-                    def step(st=st, doubled=P > 1, with_policy=with_policy):
-                        obs_s, nobs_s, act_s, rew_s, done_s = rb._dev
-                        obs, act, rew, nobs, done = ops.replay_gather(obs_s, nobs_s, act_s, rew_s, done_s, st["dev"][:B0])
+                    def step(st=st, doubled=P > 1, with_policy=with_policy, nr=nr, n_prio=n_prio, db=db):
+                        if db is None:
+                            obs, act, rew, nobs, done = ops.replay_gather(*rb._dev, st["dev"][:B0])
+                        else:  # two gathers into one batch: real rows, then imagined rows
+                            obs, nobs = th.empty(B0, self.observation_dim, device=self.device), th.empty(B0, self.observation_dim, device=self.device)
+                            act, rew = th.empty(B0, self.action_dim, device=self.device), th.empty(B0, D, device=self.device)
+                            done = th.empty(B0, 1, device=self.device)
+                            for store, lo, hi in ((rb, 0, nr), (db, nr, B0)):
+                                if hi > lo:
+                                    ops.replay_gather(*store._dev, st["dev"][lo:hi], outs=(obs[lo:hi], act[lo:hi], rew[lo:hi], nobs[lo:hi], done[lo:hi]))
                         if doubled:
                             obs, act, rew, nobs, done = obs.repeat(2, 1), act.repeat(2, 1), rew.repeat(2, 1), nobs.repeat(2, 1), done.repeat(2, 1)
                         w = self._tile_weights(st["w"], st["dev"][B0:] if doubled else None, B0)
-                        self._device_update(obs, act, rew, nobs, done, w, with_policy, st["eps"], B0 if self.per else 0, st["prio"])
+                        self._device_update(obs, act, rew, nobs, done, w, with_policy, st["eps"], n_prio, st["prio"][:n_prio])
 
                     st["graph"] = GraphedStep(step, self._mutated_tensors)
                     self._graphs[key] = st
                 hostv = st["host"].numpy()
-                idxes = rb.tree.sample(B0) if self.per else rb._draw(B0)
-                hostv[:B0] = idxes
+                # host draws in the reference's order: PER tree (or uniform real draw), model-buffer draw, support picks
+                idxes = rb.tree.sample(nr) if self.per else rb._draw(nr)
+                hostv[:nr] = idxes
+                if db is not None:
+                    hostv[nr:B0] = db._draw(B0 - nr)
                 if P > 1:
                     hostv[B0:] = random.choices(range(P), k=B0)
                 st["dev"].copy_(st["host"], non_blocking=True)
@@ -291,11 +409,13 @@ class GPIPDContinuousAction(MOAgent, MOPolicy):
                 if hook is not None:
                     st["eps"].copy_(hook((N, self.action_dim)))
                 rb.flush()
+                if db is not None:
+                    db.flush()
                 st["graph"]()
-                if self.per:
-                    st["prio_pin"].copy_(st["prio"], non_blocking=True)
+                if n_prio > 0:
+                    st["prio_pin"][:n_prio].copy_(st["prio"][:n_prio], non_blocking=True)
                     th.cuda.current_stream().synchronize()
-                    priority = st["prio_pin"].numpy().copy().clip(min=self.min_priority) ** self.alpha
+                    priority = st["prio_pin"][:n_prio].numpy().copy().clip(min=self.min_priority) ** self.alpha
                     rb.update_priorities(np.asarray(idxes), priority)
             self._n_updates += 1
 
@@ -379,6 +499,11 @@ class GPIPDContinuousAction(MOAgent, MOPolicy):
             next_obs, vector_reward, terminated, truncated, info = self.env.step(action)
             self.replay_buffer.add(obs, action, vector_reward, next_obs, terminated)
             if self.global_step >= self.learning_starts:
+                if self.dyna:
+                    if self.global_step % self.dynamics_train_freq == 0:
+                        self._train_dynamics()
+                    if self.global_step >= self.dynamics_rollout_starts and self.global_step % self.dynamics_rollout_freq == 0:
+                        self._rollout_dynamics(tensor_w)
                 self.update(tensor_w)
             if eval_env is not None and self.log and self.global_step % eval_freq == 0:
                 self.policy_eval(eval_env, weights=weight, log=self.log)

@@ -666,6 +666,57 @@ def ensemble_sample(out: th.Tensor, max_logvar: th.Tensor, min_logvar: th.Tensor
     return sample, var, unc
 
 
+TERM_NONE, TERM_HOPPER, TERM_HUMANOID, TERM_MOUNTAINCAR, TERM_LUNARLANDER = 0, 1, 2, 3, 4  # MORL_TERM_* of include/morl_b200.h
+
+
+def dyna_commit_workspace(n_rows: int, device) -> th.Tensor:
+    nbytes = _lib.load().morl_dyna_commit_workspace_bytes(int(n_rows))
+    return th.empty((nbytes + 3) // 4, device=device, dtype=th.int32)
+
+
+def dyna_commit(out: th.Tensor, max_logvar: th.Tensor, min_logvar: th.Tensor, model_idx: th.Tensor, noise: Optional[th.Tensor], obs: th.Tensor,
+                act: th.Tensor, rew_dim: int, rule: int, max_uncertainty: float, stores, ptr: int, next_alive: th.Tensor, uncertainty_out: th.Tensor,
+                counts_out: th.Tensor, workspace: Optional[th.Tensor] = None):
+    """One imagined Dyna step (``morl_dyna_commit_f32``, two launches, no host synchronisation): ensemble sample + uncertainty (as
+    :func:`ensemble_sample`, with ``obs`` added), termination ``rule`` (``TERM_*``), the gate ``uncertainty < max_uncertainty``, the ring append
+    of the kept rows into ``stores`` = (obs [C, S], next_obs [C, S], act [C, A], rew [C, rew_dim], done [C, 1]) from slot ``ptr``, and the
+    alive rows' s' compacted into ``next_alive`` [N, S].  ``counts_out`` (int32 [2]) receives {kept, alive} on the device."""
+    out = _dev(out, "out")
+    E, N, O2 = out.shape
+    O = O2 // 2
+    S = O - int(rew_dim)
+    max_logvar, min_logvar = _dev(max_logvar, "max_logvar").reshape(-1), _dev(min_logvar, "min_logvar").reshape(-1)
+    model_idx = _dev(model_idx, "model_idx", th.int32)
+    obs, act = _dev(obs, "obs"), _dev(act, "act")
+    if (O2 != 2 * O or max_logvar.numel() != O or min_logvar.numel() != O or model_idx.numel() != N or obs.dim() != 2 or tuple(obs.shape) != (N, S)
+            or act.dim() != 2 or act.shape[0] != N):
+        raise _lib.MorlB200Error(f"dyna_commit: bad shapes out {tuple(out.shape)}, logvar bounds {max_logvar.numel()}, model_idx {tuple(model_idx.shape)}, "
+                                 f"obs {tuple(obs.shape)} (want [{N}, {S}]), act {tuple(act.shape)}")
+    A = act.shape[1]
+    if noise is not None:
+        noise = _dev(noise, "noise")
+        if tuple(noise.shape) != (E, N, O):
+            raise _lib.MorlB200Error(f"dyna_commit: noise must be [{E}, {N}, {O}]")
+    st_obs, st_nobs, st_act, st_rew, st_done = stores
+    C = st_obs.shape[0]
+    for name, t, cols in (("obs", st_obs, S), ("next_obs", st_nobs, S), ("actions", st_act, A), ("rewards", st_rew, rew_dim), ("dones", st_done, 1)):
+        if not (isinstance(t, th.Tensor) and t.is_cuda and t.dtype == th.float32 and t.is_contiguous() and t.dim() == 2 and tuple(t.shape) == (C, cols)):
+            raise _lib.MorlB200Error(f"dyna_commit: store {name} must be a contiguous float32 CUDA tensor [{C}, {cols}]")
+    for name, t, shape, dt in (("next_alive", next_alive, (N, S), th.float32), ("uncertainty_out", uncertainty_out, (N,), th.float32),
+                               ("counts_out", counts_out, (2,), th.int32)):
+        if not (isinstance(t, th.Tensor) and t.is_cuda and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape):
+            raise _lib.MorlB200Error(f"dyna_commit: {name} must be a contiguous {dt} CUDA tensor {list(shape)}")
+    ws = dyna_commit_workspace(N, out.device) if workspace is None else workspace
+    if ws.numel() * ws.element_size() < _lib.load().morl_dyna_commit_workspace_bytes(N):
+        raise _lib.MorlB200Error("dyna_commit: workspace too small")
+    rc = _lib.load().morl_dyna_commit_f32(_ptr(out), _ptr(max_logvar), _ptr(min_logvar), _ptr(model_idx), _ptr(noise), _ptr(obs), _ptr(act), int(rew_dim), E, N,
+                                          O, A, int(rule), float(max_uncertainty), _ptr(st_obs), _ptr(st_nobs), _ptr(st_act), _ptr(st_rew), _ptr(st_done), C,
+                                          int(ptr), _ptr(next_alive), _ptr(uncertainty_out), _ptr(counts_out), _ptr(ws), _stream())
+    _lib.check(rc, "morl_dyna_commit_f32")
+    _count(2)
+    return counts_out
+
+
 def qhead_envelope_supported(fmt: int, B: int, W: int, A: int, D: int, K: int) -> bool:
     """True if :func:`qhead_envelope_td` covers the configuration (else use gemm_planes x 2 + envelope_td)."""
     return bool(_lib.load().morl_qhead_envelope_supported(int(fmt), int(B), int(W), int(A), int(D), int(K)))

@@ -2,7 +2,7 @@
 
     compute-sanitizer --tool memcheck|racecheck|synccheck|initcheck python scripts/sanitize_all.py [group ...]
 
-groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners ppo (default: all).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
+groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners ppo (default: all; dyna includes the fused Dyna commit).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
 every code path: all envelope kernel families, both GEMM operand formats x CTA modes x accumulator modes, MN split-K GEMM with the fused
 column sums, every split / reduction helper, the loss kernels (discrete SAC's included), Adam, polyak, Pareto + front records, replay gather,
 the corner-weight enumeration, MO-PPO's vector GAE and loss (racecheck: the loss kernel's CTA reductions)."""
@@ -178,6 +178,17 @@ if "dyna" in groups:
     smp, var, unc = ops.ensemble_sample(raw, th.zeros(O, device=dev), th.full((O,), -5.0, device=dev), idx, rn(E, N, O), rn(N, O - 3), 3)
     th.cuda.synchronize()
     assert bool(th.isfinite(smp).all()) and bool((var > 0).all()) and bool((unc > 0).all())
+    # fused commit: N = 77 leaves a partial last tile, ptr near the end of a 50-slot ring with every row kept wraps it; every rule
+    S, A, cap = O - 3, 4, 50
+    stores = tuple(th.zeros(cap, c, device=dev) for c in (S, S, A, 3, 1))
+    na, unc_c, counts = th.empty(N, S, device=dev), th.empty(N, device=dev), th.empty(2, dtype=th.int32, device=dev)
+    obs_c, act_c = rn(N, S), rn(N, A)
+    for rule in (ops.TERM_NONE, ops.TERM_HOPPER, ops.TERM_HUMANOID, ops.TERM_MOUNTAINCAR, ops.TERM_LUNARLANDER):
+        for thr in (1e30, float(unc.median())):
+            ops.dyna_commit(raw, th.zeros(O, device=dev), th.full((O,), -5.0, device=dev), idx, rn(E, N, O), obs_c, act_c, 3, rule, thr, stores, cap - 3,
+                            na, unc_c, counts)
+    th.cuda.synchronize()
+    assert int(counts[0]) == int((unc_c < thr).sum()) and 0 <= int(counts[1]) <= N
     print("dyna ok")
 if "chain" in groups:
     # chained hidden layers (gemm_chain_kernel): 2 chains x 2 layers on 5 tiles (groups of 2 + a ragged last group), then a 1-chain dX chain with masks
