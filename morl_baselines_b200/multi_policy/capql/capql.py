@@ -26,7 +26,7 @@ import torch.nn.functional as F
 
 from ... import ops
 from ...common.fused_adam import FusedClipAdam
-from ...common.graphed import GraphedStep, optimizer_tensors
+from ...common.graphed import GraphCache, Staging, Variant, optimizer_tensors
 from ...common.morl_algorithm import MOAgent, MOPolicy
 from ...common.networks import layer_init, mlp, polyak_update
 from ...common.weights import equally_spaced_weights
@@ -235,7 +235,7 @@ class CAPQL(MOAgent, MOPolicy):
         self._n_updates = 0
         self._noise_hook = None  # tests may set a callable(shape) -> standard-normal tensor to make rsample reproducible
         self.use_cuda_graph = use_cuda_graph
-        self._graphs = {}
+        self._graphs = GraphCache()
         self.log = log
         if self.log:
             self.setup_wandb(project_name, experiment_name, wandb_entity)
@@ -269,7 +269,7 @@ class CAPQL(MOAgent, MOPolicy):
         self.q_optim.load_state_dict(params["q_nets_optimizer_state_dict"])
         if load_replay_buffer and "replay_buffer" in params:
             self.replay_buffer = params["replay_buffer"]
-        self._graphs = {}  # optimiser state tensors / the buffer may have been replaced
+        self._graphs.clear()  # optimiser state tensors / the buffer may have been replaced
 
     def _sample_batch_experiences(self):
         return self.replay_buffer.sample(self.batch_size, to_tensor=True, device=self.device)
@@ -314,25 +314,25 @@ class CAPQL(MOAgent, MOPolicy):
                                     (lambda k: hook((B, self.action_dim))) if hook is not None else (lambda k: None))
             else:
                 key = (hook is not None, id(rb))
-                st = self._graphs.get(key)
-                if st is None:
-                    st = {"idx_pin": th.zeros(B, dtype=th.int64).pin_memory(), "idx": th.zeros(B, dtype=th.int64, device=self.device),
-                          "noise": [th.zeros(B, self.action_dim, device=self.device) for _ in range(2)] if hook is not None else None}
 
-                    def step(st=st):
-                        parts = rb._split(rb._dev.index_select(0, st["idx"]))
-                        nz = st["noise"]
-                        self._device_update(*parts, (lambda k: nz[k]) if nz is not None else (lambda k: None))
+                def build():
+                    idx = Staging(B, th.int64, self.device)
+                    noise = [th.zeros(B, self.action_dim, device=self.device) for _ in range(2)] if hook is not None else None
 
-                    st["graph"] = GraphedStep(step, self._mutated_tensors)
-                    self._graphs[key] = st
-                st["idx_pin"].numpy()[:] = rb.draw(B)  # python `random`, as the reference's random.sample(self.buffer, batch_size)
-                st["idx"].copy_(st["idx_pin"], non_blocking=True)
+                    def step():
+                        parts = rb._split(rb._dev.index_select(0, idx.dev))
+                        self._device_update(*parts, (lambda k: noise[k]) if noise is not None else (lambda k: None))
+
+                    return Variant(key, step, self._mutated_tensors, idx=idx, noise=noise)
+
+                v = self._graphs.get_or_build(key, build)
+                v.idx.host()[:] = rb.draw(B)  # python `random`, as the reference's random.sample(self.buffer, batch_size)
+                v.idx.upload()
                 if hook is not None:
-                    for t in st["noise"]:
+                    for t in v.noise:
                         t.copy_(hook((B, self.action_dim)))
                 rb.flush()
-                st["graph"]()
+                v.graph()
             self._n_updates += 1
         if self.log and self.global_step % 100 == 0:
             import wandb

@@ -31,7 +31,7 @@ import torch.nn.functional as F
 
 from ... import ops
 from ...common.fused_adam import FusedClipAdam
-from ...common.graphed import GraphedStep, optimizer_tensors
+from ...common.graphed import GraphCache, Staging, Variant, optimizer_tensors
 from ...common.buffer import ReplayBuffer
 from ...common.model_based.probabilistic_ensemble import ProbabilisticEnsemble
 from ...common.model_based.utils import ModelEnv
@@ -198,7 +198,7 @@ class GPIPD(MOPolicy, MOAgent):
             tg += [TCProductMlp(n, 128, self._tc_fmt, share_buffers_with=tg[0]) for n in self.target_q_nets[1:]]
             self._tc_plans = (TCProductMlp(self.q_nets[0], 128, self._tc_fmt, share_buffers_with=tg[0]), tg)
             self._tc_rows = 128
-        self._graphs = {}
+        self._graphs = GraphCache()
         self._support_cache = None
         self.per = per
         self.gpi_pd = gpi_pd
@@ -280,7 +280,8 @@ class GPIPD(MOPolicy, MOAgent):
             self.replay_buffer = params["replay_buffer"]
             if hasattr(self.replay_buffer, "to"):
                 self.replay_buffer.to(self.device)
-        self._graphs, self._support_cache = {}, None  # optimiser state / buffer / support may have been replaced
+        self._graphs.clear()  # optimiser state / buffer / support may have been replaced
+        self._support_cache = None
 
     # ------------------------------------------------------------------------------------------ the update
     def _uses_model_samples(self) -> bool:
@@ -361,7 +362,7 @@ class GPIPD(MOPolicy, MOAgent):
         for p in tg[1:] + [q0]:
             p.reserve(cap, share_buffers_with=tg[0])
         self._tc_rows = cap
-        self._graphs = {}
+        self._graphs.clear()
 
     def _tc(self, rows: int):
         """(plan of q_nets[0], plans of the target nets) with room for ``rows`` pair rows."""
@@ -373,7 +374,7 @@ class GPIPD(MOPolicy, MOAgent):
         c = self._support_cache
         if c is None or c[0] is not self.weight_support or c[1].shape[0] != len(self.weight_support):
             self._support_cache = c = (self.weight_support, th.stack(self.weight_support))
-            self._graphs = {}
+            self._graphs.clear()
         return c[1]
 
     def _device_update(self, s_obs, s_actions, s_rewards, s_next_obs, s_dones, weight, picks, sampled_idx, p_rows: int, prio_out=None):
@@ -444,35 +445,32 @@ class GPIPD(MOPolicy, MOAgent):
                 # reference), fills the static buffers, replays one graph, and reads the raw priorities back
                 M = self._support_matrix() if P > 0 else None
                 key = (P > 1, P > 5, P, id(rb), id(M))
-                st = self._graphs.get(key)
-                if st is None:
-                    st = {"host": th.zeros(2 * B0 + 4, dtype=th.int64).pin_memory(), "dev": th.zeros(2 * B0 + 4, dtype=th.int64, device=self.device),
-                          "w": th.zeros(D, device=self.device), "prio": th.zeros(B0, device=self.device), "prio_pin": th.zeros(B0).pin_memory()}
 
-                    def step(st=st, doubled=P > 1, sampled=P > 5, want_prio=want_prio):
+                def build(doubled=P > 1, sampled=P > 5, want_prio=want_prio):
+                    inds = Staging(2 * B0 + 4, th.int64, self.device)  # replay indices, support picks, sampled support indices
+                    w, prio = th.zeros(D, device=self.device), Staging(B0, th.float32, self.device)
+
+                    def step():
                         obs_s, nobs_s, act_s, rew_s, done_s = rb._dev
-                        obs, act, rew, nobs, done = ops.replay_gather(obs_s, nobs_s, act_s, rew_s, done_s, st["dev"][:B0])
-                        self._device_update(obs, act.reshape(-1), rew, nobs, done, st["w"], st["dev"][B0:2 * B0] if doubled else None,
-                                            st["dev"][2 * B0:] if sampled else None, B0 if want_prio else 0, st["prio"])
+                        obs, act, rew, nobs, done = ops.replay_gather(obs_s, nobs_s, act_s, rew_s, done_s, inds.dev[:B0])
+                        self._device_update(obs, act.reshape(-1), rew, nobs, done, w, inds.dev[B0:2 * B0] if doubled else None,
+                                            inds.dev[2 * B0:] if sampled else None, B0 if want_prio else 0, prio.dev)
 
-                    st["graph"] = GraphedStep(step, self._mutated_tensors)
-                    self._graphs[key] = st
-                hostv = st["host"].numpy()
+                    return Variant(key, step, self._mutated_tensors, inds=inds, w=w, prio=prio)
+
+                v = self._graphs.get_or_build(key, build)
+                hostv = v.inds.host()
                 idxes = rb.tree.sample(B0) if self.per else rb._draw(B0)
                 hostv[:B0] = idxes
                 if P > 1:
                     hostv[B0:2 * B0] = random.choices(range(P), k=B0)
                 if P > 5:
                     hostv[2 * B0:] = random.sample(range(P), k=4)
-                st["dev"].copy_(st["host"], non_blocking=True)
-                st["w"].copy_(weight.reshape(-1))
+                v.inds.upload()
+                v.w.copy_(weight.reshape(-1))
                 rb.flush()
-                st["graph"]()
-                pr = None
-                if want_prio:
-                    st["prio_pin"].copy_(st["prio"], non_blocking=True)
-                    th.cuda.current_stream().synchronize()
-                    pr = st["prio_pin"].numpy().copy()
+                v.graph()
+                pr = v.prio.fetch() if want_prio else None
             critic_losses.append(self._last_loss)
             if want_prio:
                 # priorities: |w . max_n err_n| of the first len(idxes) rows, clip(min)^alpha on the host (gpi_pd.py:507-525)

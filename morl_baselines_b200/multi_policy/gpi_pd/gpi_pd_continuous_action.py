@@ -39,7 +39,7 @@ import torch.nn.functional as F
 from ... import ops
 from ...common.buffer import ReplayBuffer
 from ...common.fused_adam import FusedClipAdam
-from ...common.graphed import GraphedStep, optimizer_tensors
+from ...common.graphed import GraphCache, Staging, Variant, optimizer_tensors
 from ...common.model_based.probabilistic_ensemble import ProbabilisticEnsemble
 from ...common.model_based.utils import termination_rule_id
 from ...common.morl_algorithm import MOAgent, MOPolicy
@@ -132,7 +132,7 @@ class GPIPDContinuousAction(MOAgent, MOPolicy):
         self.q_optim = FusedClipAdam(chain(*[net.parameters() for net in self.q_nets]), lr=self.learning_rate)
         self.policy_optim = FusedClipAdam(list(self.policy.parameters()), lr=self.learning_rate)
         self.use_cuda_graph = use_cuda_graph
-        self._graphs = {}
+        self._graphs = GraphCache()
 
         self.dyna, self.dynamics, self.dynamics_buffer = dyna, None, None
         if self.dyna:
@@ -201,7 +201,7 @@ class GPIPDContinuousAction(MOAgent, MOPolicy):
             self.replay_buffer = params["replay_buffer"]
             if hasattr(self.replay_buffer, "to"):
                 self.replay_buffer.to(self.device)
-        self._graphs = {}  # optimiser state tensors / the buffer / the support may have been replaced
+        self._graphs.clear()  # optimiser state tensors / the buffer / the support may have been replaced
 
     # ------------------------------------------------------------------------------------------ the update
     def _uses_model_samples(self) -> bool:
@@ -373,30 +373,31 @@ class GPIPDContinuousAction(MOAgent, MOPolicy):
                 nr = self._num_real()
                 n_prio = nr if self.per else 0
                 key = (P > 1, with_policy, hook is not None, id(rb), id(self.stacked_weight_support) if P > 1 else 0, db is not None, id(db))
-                st = self._graphs.get(key)
-                if st is None:
-                    st = {"host": th.zeros(2 * B0, dtype=th.int64).pin_memory(), "dev": th.zeros(2 * B0, dtype=th.int64, device=self.device),
-                          "w": th.zeros(D, device=self.device), "eps": th.zeros(N, self.action_dim, device=self.device) if hook is not None else None,
-                          "prio": th.zeros(B0, device=self.device), "prio_pin": th.zeros(B0).pin_memory()}
 
-                    def step(st=st, doubled=P > 1, with_policy=with_policy, nr=nr, n_prio=n_prio, db=db):
+                def build(doubled=P > 1, with_policy=with_policy, nr=nr, n_prio=n_prio, db=db):
+                    inds = Staging(2 * B0, th.int64, self.device)  # replay indices (real, then imagined), support picks
+                    w_in, prio = th.zeros(D, device=self.device), Staging(B0, th.float32, self.device)
+                    eps = th.zeros(N, self.action_dim, device=self.device) if hook is not None else None
+
+                    def step():
                         if db is None:
-                            obs, act, rew, nobs, done = ops.replay_gather(*rb._dev, st["dev"][:B0])
+                            obs, act, rew, nobs, done = ops.replay_gather(*rb._dev, inds.dev[:B0])
                         else:  # two gathers into one batch: real rows, then imagined rows
                             obs, nobs = th.empty(B0, self.observation_dim, device=self.device), th.empty(B0, self.observation_dim, device=self.device)
                             act, rew = th.empty(B0, self.action_dim, device=self.device), th.empty(B0, D, device=self.device)
                             done = th.empty(B0, 1, device=self.device)
                             for store, lo, hi in ((rb, 0, nr), (db, nr, B0)):
                                 if hi > lo:
-                                    ops.replay_gather(*store._dev, st["dev"][lo:hi], outs=(obs[lo:hi], act[lo:hi], rew[lo:hi], nobs[lo:hi], done[lo:hi]))
+                                    ops.replay_gather(*store._dev, inds.dev[lo:hi], outs=(obs[lo:hi], act[lo:hi], rew[lo:hi], nobs[lo:hi], done[lo:hi]))
                         if doubled:
                             obs, act, rew, nobs, done = obs.repeat(2, 1), act.repeat(2, 1), rew.repeat(2, 1), nobs.repeat(2, 1), done.repeat(2, 1)
-                        w = self._tile_weights(st["w"], st["dev"][B0:] if doubled else None, B0)
-                        self._device_update(obs, act, rew, nobs, done, w, with_policy, st["eps"], n_prio, st["prio"][:n_prio])
+                        w = self._tile_weights(w_in, inds.dev[B0:] if doubled else None, B0)
+                        self._device_update(obs, act, rew, nobs, done, w, with_policy, eps, n_prio, prio.dev[:n_prio])
 
-                    st["graph"] = GraphedStep(step, self._mutated_tensors)
-                    self._graphs[key] = st
-                hostv = st["host"].numpy()
+                    return Variant(key, step, self._mutated_tensors, inds=inds, w=w_in, eps=eps, prio=prio)
+
+                v = self._graphs.get_or_build(key, build)
+                hostv = v.inds.host()
                 # host draws in the reference's order: PER tree (or uniform real draw), model-buffer draw, support picks
                 idxes = rb.tree.sample(nr) if self.per else rb._draw(nr)
                 hostv[:nr] = idxes
@@ -404,18 +405,16 @@ class GPIPDContinuousAction(MOAgent, MOPolicy):
                     hostv[nr:B0] = db._draw(B0 - nr)
                 if P > 1:
                     hostv[B0:] = random.choices(range(P), k=B0)
-                st["dev"].copy_(st["host"], non_blocking=True)
-                st["w"].copy_(weight.reshape(-1))
+                v.inds.upload()
+                v.w.copy_(weight.reshape(-1))
                 if hook is not None:
-                    st["eps"].copy_(hook((N, self.action_dim)))
+                    v.eps.copy_(hook((N, self.action_dim)))
                 rb.flush()
                 if db is not None:
                     db.flush()
-                st["graph"]()
+                v.graph()
                 if n_prio > 0:
-                    st["prio_pin"][:n_prio].copy_(st["prio"][:n_prio], non_blocking=True)
-                    th.cuda.current_stream().synchronize()
-                    priority = st["prio_pin"][:n_prio].numpy().copy().clip(min=self.min_priority) ** self.alpha
+                    priority = v.prio.fetch(n_prio).clip(min=self.min_priority) ** self.alpha
                     rb.update_priorities(np.asarray(idxes), priority)
             self._n_updates += 1
 
@@ -477,7 +476,7 @@ class GPIPDContinuousAction(MOAgent, MOPolicy):
         self.weight_support = [th.tensor(w).float().to(self.device) for w in weights_no_repeat]
         if len(self.weight_support) > 0:
             self.stacked_weight_support = th.stack(self.weight_support)
-        self._graphs = {}  # captured graphs read the previous support matrix
+        self._graphs.clear()  # captured graphs read the previous support matrix
 
     def train_iteration(self, total_timesteps: int, weight: np.ndarray, weight_support: List[np.ndarray],
                         change_weight_every_episode: bool = False, eval_env=None, eval_freq: int = 1000, reset_num_timesteps: bool = False):

@@ -25,6 +25,7 @@ import torch as th
 import torch.distributed as dist
 from torch import optim
 
+from ...common.graphed import GraphCache, PopulationGraph
 from ...common.morl_algorithm import MOAgent, MOPolicy
 from ...common.networks import polyak_update
 from ...common.pareto import ParetoArchive
@@ -148,7 +149,7 @@ class MORLD(MOAgent):
         self.archive = ParetoArchive()
         self.global_front = None
         self.population_graph = True  # replay a rank's learners as one multi-branch CUDA graph in _update_others
-        self._pop_graphs = {}
+        self._pop_graphs = GraphCache()
         self._front_prune = None  # dominance test of the front exchange: None = the CUDA kernel (tests on CPU/gloo inject one)
         if self.log:
             self.setup_wandb(project_name=self.project_name, experiment_name=self.experiment_name, entity=wandb_entity)
@@ -246,7 +247,7 @@ class MORLD(MOAgent):
 
                         eps = getattr(dst_policy.wrapped, "ADAM_EPS", 1e-8)  # MOSACDiscrete's optimisers all use eps 1e-4, as its reference
                         dst_policy.wrapped.actor_optimizer = FusedClipAdam(dst.parameters(), lr=dst_policy.wrapped.policy_lr, eps=eps)
-                        dst_policy.wrapped._graphs = {}
+                        dst_policy.wrapped._graphs.clear()
                     else:
                         dst_policy.wrapped.actor_optimizer = optim.Adam(dst.parameters(), lr=dst_policy.wrapped.policy_lr)
 
@@ -289,14 +290,10 @@ class MORLD(MOAgent):
                 for p in pols:
                     p.wrapped.update()
                 continue
-            states = [p.wrapped._prepare_graph_update() for p in pols]
-            key = tuple((p.id, st["key"]) for p, st in zip(pols, states))
-            pg = self._pop_graphs.get(key)
-            if pg is None:
-                from ...common.graphed import PopulationGraph
-
-                pg = self._pop_graphs[key] = PopulationGraph([st["step"] for st in states],
-                                                             lambda pols=pols: [t for p in pols for t in p.wrapped._mutated_tensors()])
+            variants = [p.wrapped._prepare_graph_update() for p in pols]
+            key = tuple((p.id, v.key) for p, v in zip(pols, variants))
+            pg = self._pop_graphs.get_or_build(key, lambda: PopulationGraph([v.step for v in variants],
+                                                                            lambda pols=pols: [t for p in pols for t in p.wrapped._mutated_tensors()]))
             pg()
 
     def save(self, save_dir="weights/", filename=None, save_replay_buffer=True):

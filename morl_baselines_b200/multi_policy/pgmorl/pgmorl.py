@@ -283,7 +283,7 @@ class PGMORL(MOAgent):
             for a in self.agents:
                 a.update()
             return
-        steps = [a.prepare_update()["step"] for a in self.agents]  # host: shuffles drawn in agent order
+        steps = [a.prepare_update().step for a in self.agents]  # host: shuffles drawn in agent order
         if self._population_graph is None:
             agents = list(self.agents)
             self._population_graph = PopulationGraph(steps, lambda: [t for a in agents for t in a._mutated_tensors()])

@@ -32,7 +32,7 @@ from torch.distributions import Normal
 
 from ... import ops
 from ...common.fused_adam import FusedClipAdam
-from ...common.graphed import GraphedStep, optimizer_tensors
+from ...common.graphed import GraphCache, Staging, Variant, optimizer_tensors
 from ...common.morl_algorithm import MOPolicy
 from ...common.networks import layer_init, mlp
 
@@ -177,10 +177,8 @@ class MOPPO(MOPolicy):
         self.returns = th.zeros_like(self.batch.rewards)
         self.advantages = th.zeros((self.steps_per_iteration, self.num_envs), device=self.device)
         self._stats = th.zeros(6, device=self.device)
-        self._perm_pin = th.zeros((self.update_epochs, self.batch_size), dtype=th.int64).pin_memory()
-        self._perm = th.zeros((self.update_epochs, self.batch_size), dtype=th.int64, device=self.device)
-        self._perm_copied = th.cuda.Event()
-        self._graphs = {}
+        self._perm = Staging((self.update_epochs, self.batch_size), th.int64, self.device)
+        self._graphs = GraphCache()
 
     def __deepcopy__(self, memo):
         """The reference's deep copy (mo_ppo.py:343-376): an independent network, a FRESH Adam, a deep-copied batch, the step count; the
@@ -264,7 +262,7 @@ class MOPPO(MOPolicy):
         b_advantages, b_returns = self.advantages.reshape(-1), self.returns.reshape(-1, d)
         for e in epochs:
             for start in range(0, self.batch_size, self.minibatch_size):
-                idx = self._perm[e, start:start + self.minibatch_size]
+                idx = self._perm.dev[e, start:start + self.minibatch_size]
                 mb_obs = b_obs.index_select(0, idx)
                 mean = net.actor_mean(mb_obs)
                 value = net.critic(mb_obs).view(-1, d)
@@ -282,8 +280,7 @@ class MOPPO(MOPolicy):
 
     def _variant(self, key):
         """Per-variant device step: "all" runs every epoch (zeroing the clip-fraction sum first), "epoch" runs one epoch from row 0."""
-        st = self._graphs.get(key)
-        if st is None:
+        def build():
             if key == "all":
                 def step():
                     self._stats[5].zero_()
@@ -291,19 +288,17 @@ class MOPPO(MOPolicy):
             else:
                 def step():
                     self._epochs([0])
-            st = {"step": step, "graph": GraphedStep(step, self._mutated_tensors)}
-            self._graphs[key] = st
-        return st
+            return Variant(key, step, self._mutated_tensors)
+
+        return self._graphs.get_or_build(key, build)
 
     def _upload_permutations(self, n_epochs: int):
         """Draw ``n_epochs`` shuffles of the running index order (in place, as the reference does) and copy them to the device."""
-        self._perm_copied.synchronize()  # the previous asynchronous copy has read the pinned rows
-        rows = self._perm_pin.numpy()
+        rows = self._perm.host()
         for e in range(n_epochs):
             self.np_random.shuffle(self._b_inds)
             rows[e] = self._b_inds
-        self._perm[:n_epochs].copy_(self._perm_pin[:n_epochs], non_blocking=True)
-        self._perm_copied.record()
+        self._perm.upload(n_epochs)
 
     def prepare_update(self):
         """Host half of a full update without early stopping: draws and uploads every epoch's shuffle; returns the device step."""
@@ -313,9 +308,9 @@ class MOPPO(MOPolicy):
 
     def _run(self, st):
         if self.use_cuda_graph:
-            st["graph"]()
+            st.graph()
         else:
-            st["step"]()
+            st.step()
 
     def update(self):
         if self.target_kl is None:

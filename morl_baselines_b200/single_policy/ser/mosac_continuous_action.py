@@ -26,7 +26,7 @@ import torch.nn.functional as F
 from ... import ops
 from ...common.buffer import ReplayBuffer
 from ...common.fused_adam import FusedClipAdam
-from ...common.graphed import GraphedStep, optimizer_tensors
+from ...common.graphed import GraphCache, Staging, Variant, optimizer_tensors
 from ...common.morl_algorithm import MOPolicy
 from ...common.networks import layer_init, mlp, polyak_update
 
@@ -133,7 +133,7 @@ class MOSAC(MOPolicy):
             alpha0 = alpha
         self.alpha_tensor = th.scalar_tensor(alpha0).to(self.device)  # updated IN PLACE (captured graphs read it)
         self.use_cuda_graph = use_cuda_graph
-        self._graphs = {}
+        self._graphs = GraphCache()
         self.buffer = ReplayBuffer(obs_shape=self.obs_shape, action_dim=self.action_shape[0], rew_dim=self.reward_dim, max_size=self.buffer_size,
                                    device=self.device)
         self._linear = scalarization is th.matmul
@@ -174,7 +174,7 @@ class MOSAC(MOPolicy):
             c.a_optimizer = FusedClipAdam([c.log_alpha], lr=self.q_lr)
         with th.no_grad():
             c.alpha_tensor.copy_(self.alpha_tensor)
-        c._graphs = {}
+        c._graphs.clear()
         c.buffer = self.buffer if memo.get("share_buffer") else deepcopy(self.buffer)
         return c
 
@@ -183,7 +183,7 @@ class MOSAC(MOPolicy):
 
     def set_buffer(self, buffer):
         self.buffer = buffer
-        self._graphs = {}  # captured graphs read the previous buffer's device stores
+        self._graphs.clear()  # captured graphs read the previous buffer's device stores
 
     def get_policy_net(self) -> th.nn.Module:
         return self.actor
@@ -226,7 +226,7 @@ class MOSAC(MOPolicy):
                 self.buffer.to(self.device)
         self.set_weights(save_dict["weights"])
         self.alpha = save_dict["alpha"]
-        self._graphs = {}  # optimiser state tensors may have been replaced
+        self._graphs.clear()  # optimiser state tensors may have been replaced
 
     def eval(self, obs: np.ndarray, w: Optional[np.ndarray] = None):
         obs = th.as_tensor(obs).float().to(self.device).unsqueeze(0)
@@ -301,14 +301,13 @@ class MOSAC(MOPolicy):
         with_actor = self.global_step % self.policy_freq == 0
         with_target = self.global_step % self.target_net_freq == 0
         B, act_dim = self.batch_size, int(np.prod(self.action_shape))
-        has_mirror = getattr(self.buffer, "_dev", None) is not None
         hook = self._noise_hook
-        if not (self.use_cuda_graph and has_mirror):
+        if not self.graph_update_ready():
             smp = self.buffer.sample(B, to_tensor=True, device=self.device)
             self._device_update(smp[0], smp[1], smp[2], smp[3], smp[4], with_actor, with_target,
                                 (lambda k: hook((B, act_dim))) if hook is not None else (lambda k: None))
             return
-        self._prepare_graph_update()["graph"]()
+        self._prepare_graph_update().graph()
 
     def graph_update_ready(self) -> bool:
         """True when ``update()`` takes the CUDA-graph path (so a population of learners can be replayed as ONE graph, morld.py)."""
@@ -316,35 +315,34 @@ class MOSAC(MOPolicy):
 
     def _prepare_graph_update(self):
         """Host half of one graph-path update: draw the replay indices (global numpy RNG, as the reference's buffer.sample), stage them and
-        any injected noise into the static device buffers, flush new transitions to the HBM mirror.  Returns the per-(flags) state whose
-        ``step`` closure is the device half (captured by ``st["graph"]`` for this learner alone, or by a PopulationGraph for many)."""
+        any injected noise into the static device buffers, flush new transitions to the HBM mirror.  Returns the variant whose ``step``
+        closure is the device half (captured by its ``graph`` for this learner alone, or by a PopulationGraph for many)."""
         with_actor = self.global_step % self.policy_freq == 0
         with_target = self.global_step % self.target_net_freq == 0
         B, act_dim = self.batch_size, int(np.prod(self.action_shape))
         hook = self._noise_hook
         key = (with_actor, with_target, hook is not None, id(self.buffer))
-        st = self._graphs.get(key)
-        if st is None:
-            st = {"idx_pin": th.zeros(B, dtype=th.int64).pin_memory(), "idx": th.zeros(B, dtype=th.int64, device=self.device), "key": key,
-                  "noise": [th.zeros(B, act_dim, device=self.device) for _ in range(self._n_noise_sites(with_actor))] if hook is not None else None}
 
-            def step(st=st, with_actor=with_actor, with_target=with_target):
+        def build():
+            idx = Staging(B, th.int64, self.device)
+            noise = [th.zeros(B, act_dim, device=self.device) for _ in range(self._n_noise_sites(with_actor))] if hook is not None else None
+
+            def step():
                 obs_s, nobs_s, act_s, rew_s, done_s = self.buffer._dev
-                obs, act, rew, nobs, done = ops.replay_gather(obs_s, nobs_s, act_s, rew_s, done_s, st["idx"])
-                nz = st["noise"]
-                self._device_update(obs, act, rew, nobs, done, with_actor, with_target, (lambda k: nz[k]) if nz is not None else (lambda k: None))
+                obs, act, rew, nobs, done = ops.replay_gather(obs_s, nobs_s, act_s, rew_s, done_s, idx.dev)
+                self._device_update(obs, act, rew, nobs, done, with_actor, with_target, (lambda k: noise[k]) if noise is not None else (lambda k: None))
 
-            st["step"] = step
-            st["graph"] = GraphedStep(step, self._mutated_tensors)
-            self._graphs[key] = st
+            return Variant(key, step, self._mutated_tensors, idx=idx, noise=noise)
+
+        v = self._graphs.get_or_build(key, build)
         inds = self.buffer._draw(B)
-        st["idx_pin"].numpy()[:] = inds
-        st["idx"].copy_(st["idx_pin"], non_blocking=True)
+        v.idx.host()[:] = inds
+        v.idx.upload()
         if hook is not None:
-            for t in st["noise"]:
+            for t in v.noise:
                 t.copy_(hook((B, act_dim)))
         self.buffer.flush()
-        return st
+        return v
 
     def train(self, total_timesteps: int, eval_env=None, start_time=None):
         """Interaction loop (reference mosac_continuous_action.py:509-572)."""

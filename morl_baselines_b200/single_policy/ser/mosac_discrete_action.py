@@ -30,7 +30,7 @@ from torch.distributions.categorical import Categorical
 from ... import ops
 from ...common.buffer import ReplayBuffer
 from ...common.fused_adam import FusedClipAdam
-from ...common.graphed import GraphedStep, optimizer_tensors
+from ...common.graphed import GraphCache, Staging, Variant, optimizer_tensors
 from ...common.morl_algorithm import MOPolicy
 from ...common.networks import NatureCNN, layer_init, mlp, polyak_update
 
@@ -139,7 +139,7 @@ class MOSACDiscrete(MOPolicy):
             alpha0 = alpha
         self.alpha_tensor = th.scalar_tensor(alpha0).to(self.device)  # updated IN PLACE (captured graphs read it)
         self.use_cuda_graph = use_cuda_graph
-        self._graphs = {}
+        self._graphs = GraphCache()
         env.observation_space.dtype = np.float32
         self.buffer = ReplayBuffer(obs_shape=self.obs_shape, action_dim=1, rew_dim=self.reward_dim, max_size=self.buffer_size, device=self.device)
         self._linear = scalarization is th.matmul
@@ -179,7 +179,7 @@ class MOSACDiscrete(MOPolicy):
         c.q_optimizer = FusedClipAdam(list(c.qf1.parameters()) + list(c.qf2.parameters()), lr=self.q_lr, eps=self.ADAM_EPS)
         if self.autotune:
             c.a_optimizer = FusedClipAdam([c.log_alpha], lr=self.q_lr, eps=self.ADAM_EPS)
-        c._graphs = {}
+        c._graphs.clear()
         c.buffer = self.buffer if memo.get("share_buffer") else deepcopy(self.buffer)
         return c
 
@@ -188,7 +188,7 @@ class MOSACDiscrete(MOPolicy):
 
     def set_buffer(self, buffer):
         self.buffer = buffer
-        self._graphs = {}  # captured graphs read the previous buffer's device stores
+        self._graphs.clear()  # captured graphs read the previous buffer's device stores
 
     def get_policy_net(self) -> th.nn.Module:
         return self.actor
@@ -234,7 +234,7 @@ class MOSACDiscrete(MOPolicy):
                 self.buffer.to(self.device)
         self.set_weights(save_dict["weights"])
         self.alpha = save_dict["alpha"]
-        self._graphs = {}  # optimiser state tensors may have been replaced
+        self._graphs.clear()  # optimiser state tensors may have been replaced
 
     def eval(self, obs: np.ndarray, w: Optional[np.ndarray] = None, **kwargs):
         obs = th.as_tensor(obs).float().to(self.device).unsqueeze(0)
@@ -311,7 +311,7 @@ class MOSACDiscrete(MOPolicy):
             smp = self.buffer.sample(self.batch_size, to_tensor=True, device=self.device)
             self._device_update(smp[0], smp[1], smp[2], smp[3], smp[4], with_target)
             return
-        self._prepare_graph_update()["graph"]()
+        self._prepare_graph_update().graph()
 
     def graph_update_ready(self) -> bool:
         """True when ``update()`` takes the CUDA-graph path (so a population of learners can be replayed as ONE graph, morld.py)."""
@@ -319,33 +319,28 @@ class MOSACDiscrete(MOPolicy):
 
     def _prepare_graph_update(self):
         """Host half of one graph-path update: draw the replay indices (global numpy RNG, as the reference's buffer.sample), stage them into
-        the static device buffer, flush new transitions to the HBM mirror.  Returns the per-variant state whose ``step`` closure is the device
-        half (captured by ``st["graph"]`` for this learner alone, or by a PopulationGraph for many)."""
+        the static device buffer, flush new transitions to the HBM mirror.  Returns the variant whose ``step`` closure is the device half
+        (captured by its ``graph`` for this learner alone, or by a PopulationGraph for many)."""
         with_target = self.global_step % self.target_net_freq == 0
         B = self.batch_size
         key = (with_target, id(self.buffer))
-        st = self._graphs.get(key)
-        if st is None:
-            st = {"idx_pin": th.zeros(B, dtype=th.int64).pin_memory(), "idx": th.zeros(B, dtype=th.int64, device=self.device), "key": key,
-                  "copied": th.cuda.Event()}
 
-            def step(st=st, with_target=with_target):
+        def build():
+            idx = Staging(B, th.int64, self.device)
+
+            def step():
                 obs_s, nobs_s, act_s, rew_s, done_s = self.buffer._dev
-                obs, act, rew, nobs, done = ops.replay_gather(obs_s, nobs_s, act_s, rew_s, done_s, st["idx"])
+                obs, act, rew, nobs, done = ops.replay_gather(obs_s, nobs_s, act_s, rew_s, done_s, idx.dev)
                 self._device_update(obs, act, rew, nobs, done, with_target)
 
-            st["step"] = step
-            st["graph"] = GraphedStep(step, self._mutated_tensors)
-            self._graphs[key] = st
+            return Variant(key, step, self._mutated_tensors, idx=idx)
+
+        v = self._graphs.get_or_build(key, build)
         inds = self.buffer._draw(B)
-        # the asynchronous copy of the previous update must have read the pinned indices before they are overwritten: with a population
-        # graph (or a queue of replays) the host runs ahead of the device by more than one update
-        st["copied"].synchronize()
-        st["idx_pin"].numpy()[:] = inds
-        st["idx"].copy_(st["idx_pin"], non_blocking=True)
-        st["copied"].record()
+        v.idx.host()[:] = inds
+        v.idx.upload()
         self.buffer.flush()
-        return st
+        return v
 
     def train(self, total_timesteps: int, eval_env=None, start_time=None, verbose: bool = False):
         """Interaction loop (reference mosac_discrete_action.py:531-611)."""

@@ -131,7 +131,7 @@ def main():
                           text=True).stdout.strip()
 
     graph_pop, eager_pop, ref_pop = make_population(dev, True), make_population(dev, False), make_population(dev, False)
-    pg = PopulationGraph([a._variant("all")["step"] for a in graph_pop], lambda: [t for a in graph_pop for t in a._mutated_tensors()])
+    pg = PopulationGraph([a._variant("all").step for a in graph_pop], lambda: [t for a in graph_pop for t in a._mutated_tensors()])
 
     def run_graph():
         for a in graph_pop:
