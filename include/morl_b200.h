@@ -573,6 +573,36 @@ MORL_API int morl_ppo_loss_f32(const float* mean, const float* logstd, const flo
                                float ent_coef, float vf_coef, int norm_adv, int clip_vloss, float* loss_out, float* dmean, float* dlogstd,
                                float* dvalue, float* stats, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * PCN / LCN (reference multi_policy/pcn/pcn.py, multi_policy/lcn/lcn.py), csrc/pcn.cu.
+ *
+ * The default model (pcn.py:51-103): c = [desired_return || horizon] * scaling [d + 1], s = sigmoid(Ls obs + bs),
+ *   e = sigmoid(Lc c + bc), h = relu(W1 (s * e) + b1), y = W2 h + b2; log_softmax(y) for discrete actions, y for continuous ones.
+ *   params / grads: HOST arrays of 8 device pointers, in state-dict order: Ls [H, S], bs [H], Lc [H, d + 1], bc [H], W1 [H, H], b1 [H],
+ *   W2 [A, H], b2 [A] (A = number of actions, or the action dimension when continuous).
+ * Supported range (morl_pcn_supported): 1 <= S <= 256, 1 <= d <= MORL_MAX_D, H in {32, 64, 128, 256}, 1 <= A <= 32, and for the update
+ *   1 <= B <= MORL_PCN_MAX_BATCH; anything else returns MORL_ERR_UNSUPPORTED.
+ *
+ * morl_pcn_update_f32 (pcn.py:202-236): one minibatch gathered from the episode store, f32 [N, ld_store] with the columns
+ *   [obs (S) | return-to-go (d) | action]; the action is one int32 (its bits stored in the f32 column) for discrete actions, A floats
+ *   for continuous ones.  Row b of the batch reads store row rows[b] (obs, desired return = return-to-go, action) and horizon = horizons[b].
+ *   loss_out[0] = mean over rows of -log_softmax(y)[a] (discrete) or mse_loss(action, y) (continuous); entropy_out[0] (discrete, nullable)
+ *   = sum over the batch of -exp(lp) lp; pred_out (nullable) [B, A] = the log-probabilities or predictions.  grads[t] are OVERWRITTEN with
+ *   d loss / d params[t].  Deterministic: per-tile partials over 16 rows in row order, then a fixed-order sum over the tiles (no float
+ *   atomics), so repeated launches and graph replays are bit-identical.  Two launches.  workspace: morl_pcn_workspace_bytes(...) bytes.
+ * morl_pcn_forward_f32 (pcn.py:309-322): the forward on N rows with their own commands: obs [N, S], ret [N, d], hor [N] -> out [N, A]
+ *   (log-probabilities when log_softmax, else predictions); argmax_out (nullable) int32 [N] = first index of the row maximum.  obs, ret,
+ *   hor, out and argmax_out may be pinned host memory (read and written through unified addressing).  One launch. */
+#define MORL_PCN_MAX_BATCH 4096
+MORL_API int morl_pcn_supported(int obs_dim, int d, int hidden, int n_out, int batch);
+MORL_API size_t morl_pcn_workspace_bytes(int obs_dim, int d, int hidden, int n_out, int batch);
+MORL_API int morl_pcn_update_f32(const float* const* params, float* const* grads, const float* scaling, const float* store, int ld_store,
+                                 const int32_t* rows, const int32_t* horizons, int B,
+                                 int obs_dim, int d, int hidden, int n_out, int continuous, float* loss_out, float* entropy_out,
+                                 float* pred_out, void* workspace, void* stream);
+MORL_API int morl_pcn_forward_f32(const float* const* params, const float* scaling, const float* obs, const float* ret, const float* hor, int N,
+                                  int obs_dim, int d, int hidden, int n_out, int log_softmax, float* out, int32_t* argmax_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

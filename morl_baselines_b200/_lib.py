@@ -19,6 +19,7 @@ MAP_TILE, MAP_BLOCK = 0, 1
 ROWS_REFERENCE, ROWS_BMAJOR = 0, 1
 AC_ELEMENTWISE_MIN, AC_SCALAR_MIN, AC_ARGMIN_GATHER = 0, 1, 2
 MAX_D = 8
+PCN_MAX_BATCH = 4096
 FMT_BF16X3, FMT_F16X2 = 0, 1
 
 _vp, _i, _f, _d, _i64, _sz = C.c_void_p, C.c_int, C.c_float, C.c_double, C.c_int64, C.c_size_t
@@ -91,6 +92,10 @@ SIGNATURES = {
     "morl_adam_clip_lr_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i64, _f, _vp, _f, _f, _f, _vp, _vp]),
     "morl_vector_gae_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _d, _d, _i, _vp, _vp, _vp]),
     "morl_ppo_loss_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _f, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "morl_pcn_supported": (_i, [_i, _i, _i, _i, _i]),
+    "morl_pcn_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
+    "morl_pcn_update_f32": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "morl_pcn_forward_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
 }
 
 SPLIT_MAX_JOBS = 16

@@ -1063,3 +1063,73 @@ def pairs_grad_reduce(planes: th.Tensor, B: int, W: int, workspace: Optional[th.
     _lib.check(rc, "morl_pairs_grad_reduce_planes")
     _count(2)
     return dU, dV
+
+
+# ---- PCN / LCN (csrc/pcn.cu) ---------------------------------------------------------------------------------------------------------
+def pcn_supported(obs_dim: int, d: int, hidden: int, n_out: int, batch: int = 1) -> bool:
+    """Whether the fused PCN kernels cover this model and batch: 1 <= obs_dim <= 256, 1 <= d <= 8, hidden in {32, 64, 128, 256},
+    1 <= n_out <= 32, 1 <= batch <= 4096 (include/morl_b200.h)."""
+    return bool(_lib.load().morl_pcn_supported(int(obs_dim), int(d), int(hidden), int(n_out), int(batch)))
+
+
+def pcn_workspace(obs_dim: int, d: int, hidden: int, n_out: int, batch: int, device) -> th.Tensor:
+    nbytes = int(_lib.load().morl_pcn_workspace_bytes(int(obs_dim), int(d), int(hidden), int(n_out), int(batch)))
+    if nbytes == 0:
+        raise _lib.MorlB200Error(f"pcn_workspace: unsupported configuration obs_dim={obs_dim} d={d} hidden={hidden} n_out={n_out} batch={batch}")
+    return th.empty((nbytes + 7) // 8, device=device, dtype=th.float64)
+
+
+def pcn_pointer_table(tensors) -> "ctypes.Array":
+    """Host array of the 8 device pointers (Ls, bs, Lc, bc, W1, b1, W2, b2) the PCN kernels take; build it once per set of storages."""
+    import ctypes
+
+    ts = list(tensors)
+    if len(ts) != 8:
+        raise _lib.MorlB200Error(f"PCN kernels take 8 parameter tensors, got {len(ts)}")
+    for i, t in enumerate(ts):
+        _dev(t, f"pcn tensor {i}")
+        if not t.is_contiguous():
+            raise _lib.MorlB200Error(f"pcn tensor {i} must be contiguous")
+    return (ctypes.c_void_p * 8)(*[t.data_ptr() for t in ts])
+
+
+def pcn_update(params, grads, scaling: th.Tensor, store: th.Tensor, obs_dim: int, d: int, rows: th.Tensor, horizons: th.Tensor, batch: int,
+               hidden: int, n_out: int, continuous: bool, loss_out: th.Tensor, entropy_out: Optional[th.Tensor], pred_out: Optional[th.Tensor],
+               workspace: th.Tensor):
+    """One PCN minibatch (reference pcn.py:202-236): gather ``rows`` [batch] int32 of the episode store f32 [N, ld] (columns obs | return-to-go
+    | action, a discrete action as int32 bits) with ``horizons`` [batch] int32, forward, loss, backward.  ``params`` / ``grads``: pointer
+    tables of ``pcn_pointer_table``; the gradients are overwritten.  ``loss_out`` / ``entropy_out`` / ``pred_out`` are device views written
+    in place."""
+    _dev(scaling, "scaling")
+    _dev(store, "store")
+    _dev(rows, "rows", th.int32)
+    _dev(horizons, "horizons", th.int32)
+    rc = _lib.load().morl_pcn_update_f32(params, grads, _ptr(scaling), _ptr(store), int(store.shape[1]), _ptr(rows), _ptr(horizons), int(batch),
+                                         int(obs_dim), int(d), int(hidden), int(n_out), int(bool(continuous)), _ptr(loss_out), _ptr(entropy_out),
+                                         _ptr(pred_out), _ptr(workspace), _stream())
+    _lib.check(rc, "morl_pcn_update_f32")
+    _count(2)
+
+
+def _dev_or_pinned(t: th.Tensor, name: str, dtype=th.float32) -> th.Tensor:
+    if not isinstance(t, th.Tensor) or not (t.is_cuda or t.is_pinned()) or t.dtype != dtype or not t.is_contiguous():
+        raise _lib.MorlB200Error(f"{name} must be a contiguous {dtype} CUDA or pinned host tensor")
+    return t
+
+
+def pcn_forward(params, scaling: th.Tensor, obs: th.Tensor, ret: th.Tensor, hor: th.Tensor, hidden: int, log_softmax: bool, out: th.Tensor,
+                argmax_out: Optional[th.Tensor] = None):
+    """The PCN model on N rows with their own commands (reference pcn.py:309-322 on one row): obs [N, S], ret [N, d], hor [N] ->
+    ``out`` [N, A] (log-probabilities or predictions), optionally the first-occurrence argmax into ``argmax_out`` int32 [N].  The row
+    tensors and outputs may be CUDA tensors or pinned host tensors (the kernel reads and writes pinned memory directly); with pinned
+    outputs the caller synchronises the stream before reading them."""
+    _dev(scaling, "scaling")
+    for t, n in ((obs, "obs"), (ret, "ret"), (hor, "hor"), (out, "out")):
+        _dev_or_pinned(t, n)
+    if argmax_out is not None:
+        _dev_or_pinned(argmax_out, "argmax_out", th.int32)
+    N, S = obs.shape
+    rc = _lib.load().morl_pcn_forward_f32(params, _ptr(scaling), _ptr(obs), _ptr(ret), _ptr(hor), int(N), int(S), int(ret.shape[1]), int(hidden),
+                                          int(out.shape[1]), int(bool(log_softmax)), _ptr(out), _ptr(argmax_out), _stream())
+    _lib.check(rc, "morl_pcn_forward_f32")
+    _count()

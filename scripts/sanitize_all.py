@@ -2,10 +2,10 @@
 
     compute-sanitizer --tool memcheck|racecheck|synccheck|initcheck python scripts/sanitize_all.py [group ...]
 
-groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners ppo (default: all; dyna includes the fused Dyna commit).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
+groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners ppo pcn (default: all; dyna includes the fused Dyna commit).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
 every code path: all envelope kernel families, both GEMM operand formats x CTA modes x accumulator modes, MN split-K GEMM with the fused
 column sums, every split / reduction helper, the loss kernels (discrete SAC's included), Adam, polyak, Pareto + front records, replay gather,
-the corner-weight enumeration, MO-PPO's vector GAE and loss (racecheck: the loss kernel's CTA reductions)."""
+the corner-weight enumeration, MO-PPO's vector GAE and loss (racecheck: the loss kernel's CTA reductions), PCN's update and forward."""
 import os
 import sys
 
@@ -23,7 +23,7 @@ if os.environ.get("SAN_ZERO_PLANES") == "1":
     # from a genuine read of memory nobody wrote.
     _empty = ops.empty_planes
     ops.empty_planes = lambda *a, **k: _empty(*a, **k).zero_()
-groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain", "corners", "ppo"}
+groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain", "corners", "ppo", "pcn"}
 
 
 def rn(*s, scale=1.0):
@@ -231,4 +231,26 @@ if "ppo" in groups:
         ops.ppo_loss(rn(M, A), rn(A, scale=0.3), rn(M, D), rn(M, A), rn(M), rn(M), rn(M, D), rn(M, D), 0.2, 0.01, 0.5, True, cv, stats)
     th.cuda.synchronize()
     print("ppo ok")
+if "pcn" in groups:
+    # PCN (csrc/pcn.cu): a ragged last tile, one row, the largest hidden width, both action kinds; the forward on device and pinned rows
+    from morl_baselines_b200.multi_policy.pcn import pcn as pcn_mod
+
+    for S, d, H, A, B, cont in [(7, 3, 64, 6, 37, False), (3, 8, 256, 32, 1, False), (11, 3, 32, 3, 20, True)]:
+        m = (pcn_mod.ContinuousActionsDefaultModel if cont else pcn_mod.DiscreteActionsDefaultModel)(S, A, d, np.ones(d + 1, np.float32), H).to(dev)
+        ts = pcn_mod.default_model_tensors(m)
+        N, ld = 64, S + d + (A if cont else 1)
+        store = rn(N, ld)
+        if not cont:
+            store[:, S + d] = th.randint(0, A, (N,), device=dev, generator=g).int().view(th.float32)
+        rows, hor = th.randint(0, N, (B,), device=dev, generator=g).int(), th.randint(1, 50, (B,), device=dev, generator=g).int()
+        stats, pred = th.zeros(2, device=dev), th.zeros(B, A, device=dev)
+        ops.pcn_update(ops.pcn_pointer_table(ts), ops.pcn_pointer_table([th.empty_like(t) for t in ts]), m.scaling_factor, store, S, d, rows, hor,
+                       B, H, A, cont, stats[0:1], stats[1:2], pred, ops.pcn_workspace(S, d, H, A, B, dev))
+        out, am = th.zeros(B, A, device=dev), th.zeros(B, dtype=th.int32, device=dev)
+        ops.pcn_forward(ops.pcn_pointer_table(ts), m.scaling_factor, rn(B, S), rn(B, d), th.ones(B, device=dev), H, not cont, out, am)
+        pin_out = th.zeros(1, A).pin_memory()
+        ops.pcn_forward(ops.pcn_pointer_table(ts), m.scaling_factor, th.ones(1, S).pin_memory(), th.ones(1, d).pin_memory(), th.ones(1).pin_memory(),
+                        H, not cont, pin_out)
+    th.cuda.synchronize()
+    print("pcn ok")
 print("sanitize run ok")
