@@ -17,6 +17,8 @@ from typing import Any, Callable, Hashable, Iterable, List, Optional
 import numpy as np
 import torch as th
 
+from .. import ops
+
 
 @contextlib.contextmanager
 def _gc_paused():
@@ -39,6 +41,7 @@ class GraphedStep:
         self.mutated = mutated
         self.warmup = warmup
         self.graph = None
+        self.launches = None
 
     def _record(self):
         """The work the graph records (the warm-up passes run ``fn``)."""
@@ -55,8 +58,10 @@ class GraphedStep:
                 self.fn()
         th.cuda.current_stream().wait_stream(side)
         g = th.cuda.CUDAGraph()
+        before = ops.launch_count
         with _gc_paused(), th.cuda.graph(g):
             self._record()
+        self.launches = ops.launch_count - before  # the project's kernel launches one replay makes
         with th.no_grad():
             for t, s in zip(tensors, snap):
                 t.copy_(s)

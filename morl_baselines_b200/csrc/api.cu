@@ -1,5 +1,4 @@
 // api.cu -- version / error plumbing of the C-ABI (include/morl_b200.h).
-#include <stdlib.h>
 #include <stdarg.h>
 #include <string.h>
 
@@ -24,20 +23,6 @@ int check_launch(const char* what) {
         return static_cast<int>(e);
     }
     return MORL_OK;
-}
-
-bool pdl_enabled() {
-    // opt-in: with the attribute on EVERY kernel of the step the early-resident CTAs of the small kernels take issue slots and shared memory
-    // from the draining grid (not measured on H100).  The GEMM chain keeps its own switch (MORL_GEMM_PDL, default on), where the prologue
-    // that overlaps (barrier initialisation, tensor-map prefetch) is longer.
-    static const bool on = [] { const char* e = getenv("MORL_PDL"); return e && e[0] == '1'; }();
-    return on;
-}
-
-bool gemm_pdl_enabled() {
-    // programmatic dependent launch between the consecutive tensor-core GEMMs of the update (MORL_GEMM_PDL=0 disables it)
-    static const bool on = [] { const char* e = getenv("MORL_GEMM_PDL"); return !(e && e[0] == '0'); }();
-    return on;
 }
 
 }  // namespace morl

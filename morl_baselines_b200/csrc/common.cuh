@@ -25,21 +25,20 @@ int check_launch(const char* what);
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // ---- programmatic dependent launch (PDL) -----------------------------------------------------------
-// Every kernel of the captured Envelope update is launched through launch_k() and starts with pdl_enter(): the grid may become resident
+// Every kernel of the captured Envelope update starts with pdl_enter().  A kernel launched with the PDL attribute may become resident
 // while its predecessor in the stream is still draining (the launch latency and the block scheduling of kernel n+1 overlap the tail of
 // kernel n; in a CUDA graph the edge is captured as a programmatic dependency), and `griddepcontrol.wait` then blocks until the
 // predecessor has COMPLETED and its writes are visible.  Rules that keep this equivalent to plain stream order:
 //   * pdl_enter() is the first statement of the kernel, executed by every thread, before any global-memory access;
 //   * a kernel launched with the attribute always executes the wait (the chain kernel n-1 -> n -> n+1 stays transitively ordered).
-// Without the launch attribute both instructions are no-ops.  The attribute is OPT-IN (MORL_PDL=1): on every kernel of the update it
-// measured 4.5 % slower than plain stream order (api.cu: pdl_enabled); the GEMM chain has its own switch (MORL_GEMM_PDL, default on).
+// Without the launch attribute both instructions are no-ops.  The tensor-core GEMM, chain and fused-head (qhead_envelope) launches set it
+// (launch_k_pdl(true, ...)), where the prologue that overlaps (barrier initialisation, tensor-map prefetch) is long.  Every other kernel
+// is launched in plain stream order (launch_k): with the attribute on every kernel of the update, the update measured 4.5 % slower than
+// plain stream order (the early-resident CTAs of the small kernels take issue slots and shared memory from the draining grid).
 __device__ __forceinline__ void pdl_enter() {
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     asm volatile("griddepcontrol.wait;" ::: "memory");
 }
-
-bool pdl_enabled();       // api.cu: MORL_PDL=1
-bool gemm_pdl_enabled();  // api.cu: MORL_GEMM_PDL, default on (the tensor-core GEMM and qhead launches)
 
 // Launch with the PDL attribute iff `pdl`.
 template <typename... KArgs, typename... Args>
@@ -60,7 +59,7 @@ static inline void launch_k_pdl(bool pdl, void (*kernel)(KArgs...), dim3 grid, d
 
 template <typename... KArgs, typename... Args>
 static inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
-    launch_k_pdl(pdl_enabled(), kernel, grid, block, smem, stream, static_cast<Args&&>(args)...);
+    launch_k_pdl(false, kernel, grid, block, smem, stream, static_cast<Args&&>(args)...);
 }
 
 // Raises the dynamic-shared-memory limit of kernel K to `bytes` once per process (the first call of each instantiation).

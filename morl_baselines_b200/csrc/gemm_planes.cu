@@ -2086,7 +2086,7 @@ static int launch_gemm_planes(const CUtensorMap& tmA, const CUtensorMap& tmB, co
     set_smem_limit_once<gemm_planes_kernel<FMT, SPLIT, EPI>>(smem);
     constexpr int kUnitN = SPLIT ? 128 : 256;  // column units per tile: as gemm_planes_kernel
     const int n_work = (g.M + kGemmBM - 1) / kGemmBM * ((g.N_pad + kUnitN - 1) / kUnitN);
-    launch_k_pdl(gemm_pdl_enabled(), gemm_planes_kernel<FMT, SPLIT, EPI>, dim3(n_work < sms ? n_work : sms), dim3(kGemmThreads), smem, st, tmA, tmB, tmC, g);
+    launch_k_pdl(true, gemm_planes_kernel<FMT, SPLIT, EPI>, dim3(n_work < sms ? n_work : sms), dim3(kGemmThreads), smem, st, tmA, tmB, tmC, g);
     return check_launch(EPI == kEpiLn ? "morl_gemm_planes_ln_f32" : "morl_gemm_planes_f32");
 }
 
@@ -2274,7 +2274,7 @@ static int launch_chain_resident(ResChainArgs& g, int n_chains, int n_layers, co
     const int n_tiles = (M + kGemmBM - 1) / kGemmBM;
     constexpr size_t smem = ResPlan::kBytes;
     set_smem_limit_once<gemm_chain_resident_kernel>(smem);
-    launch_k_pdl(gemm_pdl_enabled(), gemm_chain_resident_kernel, dim3(n_tiles < sms ? n_tiles : sms), dim3(kGemmThreads), smem,
+    launch_k_pdl(true, gemm_chain_resident_kernel, dim3(n_tiles < sms ? n_tiles : sms), dim3(kGemmThreads), smem,
                  static_cast<cudaStream_t>(stream), maps, g);
     return check_launch(name);
 }
@@ -2345,7 +2345,7 @@ extern "C" int morl_gemm_chain_f32(int fmt, int n_chains, int n_layers, const vo
         constexpr size_t smem = KPlan<kFmt>::kBytes;
         g.n_stages = KPlan<kFmt>::kStages;
         set_smem_limit_once<gemm_chain_kernel<kFmt>>(smem);
-        launch_k_pdl(gemm_pdl_enabled(), gemm_chain_kernel<kFmt>, dim3(n_tiles < sms ? n_tiles : sms), dim3(kGemmThreads), smem,
+        launch_k_pdl(true, gemm_chain_kernel<kFmt>, dim3(n_tiles < sms ? n_tiles : sms), dim3(kGemmThreads), smem,
                      static_cast<cudaStream_t>(stream), maps, g);
     });
     return check_launch("morl_gemm_chain_f32");

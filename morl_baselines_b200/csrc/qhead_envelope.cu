@@ -254,7 +254,7 @@ template <int FMT, int D, int MODE>
 static int launch_qhead(const CUtensorMap& tmA_on, const CUtensorMap& tmA_tg, const CUtensorMap& tmB_on, const CUtensorMap& tmB_tg, const QHeadArgs& g,
                         size_t smem, int grid, cudaStream_t st) {
     set_smem_limit_once<qhead_envelope_kernel<FMT, D, MODE>>(227 * 1024);
-    launch_k_pdl(gemm_pdl_enabled(), qhead_envelope_kernel<FMT, D, MODE>, dim3((unsigned)grid), dim3(kQhThreads), smem, st, tmA_on, tmA_tg, tmB_on, tmB_tg, g);
+    launch_k_pdl(true, qhead_envelope_kernel<FMT, D, MODE>, dim3((unsigned)grid), dim3(kQhThreads), smem, st, tmA_on, tmA_tg, tmB_on, tmB_tg, g);
     return check_launch("morl_qhead_envelope_td_f32");
 }
 

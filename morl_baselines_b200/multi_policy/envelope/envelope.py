@@ -23,6 +23,7 @@ network shapes the tensor-core path does not cover raise instead of silently tak
 from __future__ import annotations
 
 import os
+from functools import partial
 from typing import List, Optional, Union
 
 import numpy as np
@@ -34,6 +35,7 @@ from ... import ops
 from ...tc_mlp import TCPairMlp, TCPairMlpFn
 from ...common.buffer import ReplayBuffer
 from ...common.fused_adam import FusedClipAdam
+from ...common.graphed import GraphCache, GraphedStep, optimizer_tensors
 from ...common.morl_algorithm import MOAgent, MOPolicy
 from ...common.networks import NatureCNN, get_grad_norm, layer_init, mlp, polyak_update
 from ...common.prioritized_buffer import PrioritizedReplayBuffer
@@ -43,15 +45,6 @@ from ...common.weights import equally_spaced_weights, random_weights
 # output layers + envelope operator + Bellman line as one kernel (csrc/qhead_envelope.cu; bit-identical to the
 # three-launch chain, tests/test_qhead_envelope_gpu.py); MORL_FUSED_HEAD=0 keeps the three-launch chain (A/B runs)
 _FUSED_HEAD = os.environ.get("MORL_FUSED_HEAD", "1") != "0"
-_PRE_REFRESH = os.environ.get("MORL_PRE_REFRESH", "1") == "1"  # weight-plane refresh on a side branch, under the tree walk + gather (+1.4 %)
-_HEAD_REVERSE = os.environ.get("MORL_HEAD_REVERSE", "1") == "1"  # the fused head walks the tiles from the last one after a chained pass (L2; +1.2 %)
-# device PER: fork the priority / sum-tree branch after the backward GEMMs instead of right after the loss (MORL_DEFER_TREE=0: the earlier order)
-_DEFER_TREE = os.environ.get("MORL_DEFER_TREE", "1") != "0"
-# the online-net and target-net no-grad chains as two branches of the captured graph: one chain's kernels fill the launch gaps and tile
-# tails of the other's (+2 % on the update; MORL_TWO_STREAMS=0: one stream; needs the fused head)
-_TWO_STREAMS = os.environ.get("MORL_TWO_STREAMS", "1") == "1"
-# ... and the training pass's forward as a third branch (+1 %; MORL_THREE_STREAMS=0 disables it)
-_THREE_STREAMS = os.environ.get("MORL_THREE_STREAMS", "1") == "1"
 
 
 class QNet(nn.Module):
@@ -239,7 +232,7 @@ class Envelope(MOPolicy, MOAgent):
         self._dq = self._grad_bufs = None
         self._last_lazy, self._last_inds_v, self._last_priority_v, self._updates_done = False, None, None, 0
         self._side_pending = False
-        self._graphs = {}
+        self._graphs = GraphCache()  # one captured step per mode ("device_per", "device", "host")
         self._static = None
         self._last_loss = None
         self.log = log
@@ -294,13 +287,13 @@ class Envelope(MOPolicy, MOAgent):
             self.replay_buffer = params["replay_buffer"]
             if hasattr(self.replay_buffer, "to"):
                 self.replay_buffer.to(self.device)
-            self._graphs = {}  # a captured step gathers from the PREVIOUS buffer's device stores: re-capture against the new mirror
+            self._graphs.clear()  # a captured step gathers from the PREVIOUS buffer's device stores: re-capture against the new mirror
 
     def _load_optimizer_inplace(self, sd):
         cur = self.q_optim.state_dict()
         if len(cur["state"]) == 0 or not self._graphs:
             self.q_optim.load_state_dict(sd)
-            self._graphs = {}  # state tensors were re-created: re-capture lazily
+            self._graphs.clear()  # state tensors were re-created: re-capture lazily
             return
         for gi, g in enumerate(sd["param_groups"]):
             for k, v in g.items():
@@ -391,152 +384,153 @@ class Envelope(MOPolicy, MOAgent):
         # recorded INSIDE the captured step right after its first node: the staging buffer may be overwritten by the next step's copy
         s["consumed"] = th.cuda.Event(external=True)
         self._static = s
+        self._ensure_plans()
         return s
 
-    def _gradient_step(self, obs, act, rew, nobs, done, wset, device_per: bool = False):
-        """One gradient update on device tensors (everything between sampling and the priority write-back)."""
-        s = self._static
-        B, W, A, D = obs.shape[0], wset.shape[0], self.action_dim, self.reward_dim
-        with th.no_grad():
-            if self.use_tensor_cores and B == self.batch_size and W == self.num_sample_w:
-                if self._tc_on is None:
-                    split = self.tensor_core_accumulators == "split"
-                    self._tc_on = TCPairMlp(self.q_net.net, self.q_net.feat_dim, B, W, fmt=self._tc_fmt, split_acc=split)
-                    self._tc_tg = TCPairMlp(self.target_q_net.net, self.target_q_net.feat_dim, B, W, fmt=self._tc_fmt, split_acc=split)
-                    if TCPairMlp.trainable_supported(self.q_net.net, W, self._tc_fmt):
-                        self._tc_train = TCPairMlp(self.q_net.net, self.q_net.feat_dim, B, W if self._dp is None else self._dp["w_loc"],
-                                                   share_weights_with=self._tc_on, trainable=True, split_acc=split)
-                # every weight plane this step needs (online, target, transposed-for-backward) in one launch (unless _step already did it on a
-                # side branch)
-                if getattr(self, "_planes_fresh", False):
-                    self._planes_fresh = False
-                else:
-                    TCPairMlp.refresh_many([self._tc_on, self._tc_tg], transposed_of=[self._tc_train] if self._tc_train is not None else [])
-                early_q = None
-                if _THREE_STREAMS and self._tc_train is not None:
-                    # the training pass's forward (online net on s) does not depend on the targets: a third branch of the captured graph
-                    main, side3 = th.cuda.current_stream(), s["side_stream3"]
-                    side3.wait_stream(main)
-                    with th.cuda.stream(side3):
-                        dp_ = self._dp
-                        ws_ = wset if dp_ is None else wset[dp_["rank"] * dp_["w_loc"] : (dp_["rank"] + 1) * dp_["w_loc"]]
-                        early_q = self._tc_train.forward_pairs(obs, ws_)
-                fused_head = self.envelope and _FUSED_HEAD and self.tensor_core_accumulators != "split" and self._tc_on.head_operands() is not None \
-                    and ops.qhead_envelope_supported(self._tc_fmt, B, W, A, D, self._tc_on.lin[-1].in_features)
-                self.fused_head_active = bool(fused_head)
-                head_reverse = False
-                if fused_head:
-                    # output layers of both nets + envelope operator + Bellman line in ONE kernel: Q_on / Q_tg (envelope.py:420, :429) exist
-                    # in tensor / shared memory only (csrc/qhead_envelope.cu; bit-identical to the three-launch chain below)
-                    if self._tc_on.pair_chain_supported() and self._tc_tg.pair_chain_supported():
-                        # layers 1.. of BOTH nets in one persistent launch from the first layer's (u, v): a CTA keeps each of its row
-                        # tiles in shared memory through all layers of a net, and only the last hidden activation of each net is
-                        # written (csrc/gemm_planes.cu: gemm_chain_resident_kernel)
-                        if self._nograd_chain is None:
-                            self._nograd_chain = TCPairMlp.make_pair_chain([self._tc_on, self._tc_tg])
-                        u_on, v_on = self._tc_on.layer1_uv(nobs, wset)
-                        u_tg, v_tg = self._tc_tg.layer1_uv(nobs, wset)
-                        self._nograd_chain([u_on, u_tg], [v_on, v_tg])
-                        h_on, h_tg = self._tc_on.h[-1], self._tc_tg.h[-1]
-                        head_reverse = _HEAD_REVERSE  # the chain wrote its highest tiles last: start the head on them (still in L2)
-                    elif self._tc_on.chain_supported() and self._tc_tg.chain_supported():
-                        # hidden layers 2.. of BOTH nets in one persistent launch (bf16x3: csrc/gemm_planes.cu: gemm_chain_kernel)
-                        if self._nograd_chain is None:
-                            self._nograd_chain = TCPairMlp.make_chain([self._tc_on, self._tc_tg])
-                        self._tc_on.layer1(nobs, wset)
-                        self._tc_tg.layer1(nobs, wset)
-                        self._nograd_chain()
-                        h_on, h_tg = self._tc_on.h[-1], self._tc_tg.h[-1]
-                        head_reverse = _HEAD_REVERSE  # the chain wrote its highest tiles last: start the head on them (still in L2)
-                    elif _TWO_STREAMS:
-                        # the two no-grad chains are independent: fork the target-net chain onto a side stream (a parallel branch of the
-                        # captured graph) so that its kernels fill the launch gaps and tile tails of the online-net chain
-                        main, side = th.cuda.current_stream(), s["side_stream2"]
-                        side.wait_stream(main)
-                        with th.cuda.stream(side):
-                            h_tg = self._tc_tg.forward_hidden(nobs, wset)
-                        h_on = self._tc_on.forward_hidden(nobs, wset)
-                        main.wait_stream(side)
-                    else:
-                        h_on = self._tc_on.forward_hidden(nobs, wset)
-                        h_tg = self._tc_tg.forward_hidden(nobs, wset)
-                    (w_on, sw_on, b_on), (w_tg, sw_tg, b_tg) = self._tc_on.head_operands(), self._tc_tg.head_operands()
-                    target_q, _, _ = ops.qhead_envelope_td(h_on, h_tg, w_on, w_tg, b_on.detach(), b_tg.detach(), wset, rew, done.reshape(-1), self.gamma,
-                                                           B, W, A, D, self.dot_mode, ops.ROWS_BMAJOR, a_scale_on=self._tc_on.s_act,
-                                                           a_scale_tg=self._tc_tg.s_act, w_scale_on=sw_on, w_scale_tg=sw_tg, reverse_tiles=head_reverse)
-                    q_on = q_tg = None
-                else:
-                    q_on = self._tc_on.forward_pairs(nobs, wset).view(B, W, A, D)  # online net selects   (envelope.py:420)
-                    q_tg = self._tc_tg.forward_pairs(nobs, wset).view(B, W, A, D)  # target net evaluates (envelope.py:429)
-            else:
-                fused_head, early_q = False, None
-                q_on = self.q_net.forward_pairs(nobs, wset)
-                q_tg = self.target_q_net.forward_pairs(nobs, wset)
-            done1 = done.reshape(-1)
-            if fused_head:
-                pass
-            elif self.envelope:
-                target_q, _, _ = ops.envelope_td(q_on, q_tg, wset, rew, done1, self.gamma, self.dot_mode, ops.ROWS_BMAJOR, want_indices=False)
-            else:
-                target_q, _ = ops.greedy_td(q_on.view(B * W, A, D), q_tg.view(B * W, A, D), wset, rew, done1, self.gamma, self.dot_mode,
-                                            ops.MAP_TILE, ops.MAP_BLOCK)
-        dp = self._dp
-        if self._tc_train is not None and B == self.batch_size and W == self.num_sample_w:
-            # training pass on the tensor cores, without autograd: forward, fused loss (emits d loss / d Q, the loss and the priorities),
-            # hand-written backward straight into the persistent .grad buffers; weight planes were refreshed above
-            with th.no_grad():
-                Wt, wset_t = W, wset
-                if dp is not None:
-                    # DP-Envelope: this rank's loss rows are those of its own scalarising weights i in [lo, hi) (all transitions); the targets
-                    # above were formed for every i because the envelope maximum runs over all preference rows j
-                    Wt, lo = dp["w_loc"], dp["rank"] * dp["w_loc"]
-                    wset_t = wset[lo : lo + Wt]
-                    target_q = target_q.view(B, W, D)[:, lo : lo + Wt].reshape(B * Wt, D)
-                if early_q is not None:
-                    th.cuda.current_stream().wait_stream(s["side_stream3"])
-                    q_values = early_q.view(B * Wt, A, D)
-                else:
-                    q_values = self._tc_train.forward_pairs(obs, wset_t).view(B * Wt, A, D)
-                if self._dq is None:
-                    self._dq = th.empty_like(q_values)
-                    self._grad_bufs = []
-                    if dp is not None:
-                        from ...parallel import DPFlat
+    def _ensure_plans(self):
+        """The tensor-core plans of the update, made once before the first step: the no-grad passes of the online and the target net, the
+        training pass (it shares the online net's weight planes), and the launch that chains the hidden layers of both no-grad passes."""
+        self.fused_head_active = False
+        if not self.use_tensor_cores:
+            return
+        B, W, A, D = self.batch_size, self.num_sample_w, self.action_dim, self.reward_dim
+        split = self.tensor_core_accumulators == "split"
+        self._tc_on = TCPairMlp(self.q_net.net, self.q_net.feat_dim, B, W, fmt=self._tc_fmt, split_acc=split)
+        self._tc_tg = TCPairMlp(self.target_q_net.net, self.target_q_net.feat_dim, B, W, fmt=self._tc_fmt, split_acc=split)
+        self._tc_train = TCPairMlp(self.q_net.net, self.q_net.feat_dim, B, W if self._dp is None else self._dp["w_loc"],
+                                   share_weights_with=self._tc_on, trainable=True, split_acc=split)
+        # output layers of both nets + envelope operator + Bellman line in ONE kernel: Q_on / Q_tg (envelope.py:420, :429) exist in tensor /
+        # shared memory only (csrc/qhead_envelope.cu; bit-identical to the three-launch chain)
+        self.fused_head_active = bool(self.envelope and _FUSED_HEAD and not split and self._tc_on.head_operands() is not None
+                                      and ops.qhead_envelope_supported(self._tc_fmt, B, W, A, D, self._tc_on.lin[-1].in_features))
+        if not self.fused_head_active:
+            return
+        if self._tc_on.pair_chain_supported() and self._tc_tg.pair_chain_supported():
+            # layers 1.. of BOTH nets in one persistent launch from the first layer's (u, v): a CTA keeps each of its row tiles in shared
+            # memory through all layers of a net, and only the last hidden activation of each net is written (csrc/gemm_planes.cu:
+            # gemm_chain_resident_kernel)
+            self._nograd_chain = TCPairMlp.make_pair_chain([self._tc_on, self._tc_tg])
+        elif self._tc_on.chain_supported() and self._tc_tg.chain_supported():
+            # hidden layers 2.. of BOTH nets in one persistent launch (bf16x3: csrc/gemm_planes.cu: gemm_chain_kernel)
+            self._nograd_chain = TCPairMlp.make_chain([self._tc_on, self._tc_tg])
 
-                        dp["flat"] = DPFlat([p for l in self._tc_train.lin for p in (l.weight, l.bias)], B, dp["group"])
-                        self._grad_bufs = list(dp["flat"].grads)
-                        for prm, gbuf in zip([p for l in self._tc_train.lin for p in (l.weight, l.bias)], self._grad_bufs):
-                            prm.grad = gbuf
-                    else:
-                        for l in self._tc_train.lin:
-                            for p in (l.weight, l.bias):
-                                p.grad = th.zeros_like(p)
-                                self._grad_bufs.append(p.grad)
-                raw = (s["raw_prio"] if device_per else s["prio"]) if self.per else None
-                ops.td_mse_priority(q_values, act.reshape(-1), target_q, wset_t, 0.0, B, Wt, ops.ROWS_BMAJOR, want_grad=True, want_prio=self.per,
-                                    workspace=s["ws"], loss_out=s["loss1"], grad_out=self._dq, prio_out=raw, lambda_dev=s["lam"])
-                # device-resident PER: the priority / sum-tree branch (a single-block kernel with 45 KB of shared memory) is forked only
-                # AFTER the last persistent GEMM of the backward pass -- forked right here it keeps one SM, hence one persistent CTA of every GEMM
-                # that overlaps it, waiting; the host-tree modes keep the early hand-off
-                defer_ship = dp is None and device_per and _DEFER_TREE
-                if dp is None and not defer_ship:
-                    self._ship_results(raw, device_per)
-                for l, (gw, gb) in zip(self._tc_train.lin, zip(self._grad_bufs[0::2], self._grad_bufs[1::2])):
-                    if l.weight.grad is not gw or l.bias.grad is not gb:  # (someone called zero_grad(set_to_none=True) in between)
-                        l.weight.grad, l.bias.grad = gw, gb
-                self._tc_train.backward(obs, wset_t, self._dq.view(B * Wt, A * D), grads_out=self._grad_bufs,
-                                        after_gemms=(lambda: self._ship_results(raw, device_per)) if defer_ship else None)
-            if dp is not None:
+    def _gradient_step(self, obs, act, rew, nobs, done, wset, device_per: bool):
+        """One gradient update on the static device tensors (everything between sampling and the priority write-back)."""
+        s = self._static
+        raw = (s["raw_prio"] if device_per else s["prio"]) if self.per else None  # where the loss kernel leaves |w . td|
+        if self.use_tensor_cores:
+            self._tc_step(obs, act, rew, nobs, done, wset, raw, device_per)
+            if self._dp is not None:
                 return  # the collective and the optimiser step follow the captured half (_dp_finish)
         else:
-            # explicit validation path (use_tensor_cores=False): torch autograd + library GEMMs around the same fused operators
-            q_values = self.q_net.forward_pairs(obs, wset).view(B * W, A, D)
-            raw = (s["raw_prio"] if device_per else s["prio"]) if self.per else None
-            loss = _FusedTDLoss.apply(q_values, act.reshape(-1), target_q, wset, s["lam"], B, W, s["ws"], raw, s["loss1"])
-            self._ship_results(raw, device_per)
-            self.q_optim.zero_grad(set_to_none=True)
-            loss.backward()
+            self._autograd_step(obs, act, rew, nobs, done, wset, raw, device_per)
         self.q_optim.step_fused(self.max_grad_norm)  # clip_grad_norm_ + Adam.step (envelope.py:324-326) in two launches
+
+    @th.no_grad()
+    def _target(self, rew, nobs, done, wset):
+        """The envelope (or double-DQN) target of every (transition b, weight j) row b*W + j, [B * W, D], from the no-grad passes of both nets
+        on (s'_b, w_j)."""
+        B, W, A, D = self.batch_size, self.num_sample_w, self.action_dim, self.reward_dim
+        done1 = done.reshape(-1)
+        if self.fused_head_active:
+            on, tg, chain = self._tc_on, self._tc_tg, self._nograd_chain
+            if isinstance(chain, ops.GemmChainPairs):
+                u_on, v_on = on.layer1_uv(nobs, wset)
+                u_tg, v_tg = tg.layer1_uv(nobs, wset)
+                chain([u_on, u_tg], [v_on, v_tg])
+                h_on, h_tg = on.h[-1], tg.h[-1]
+            elif chain is not None:
+                on.layer1(nobs, wset)
+                tg.layer1(nobs, wset)
+                chain()
+                h_on, h_tg = on.h[-1], tg.h[-1]
+            else:
+                # the two no-grad passes are independent: fork the target net's onto a side stream (a parallel branch of the captured graph)
+                # so that its kernels fill the launch gaps and tile tails of the online net's
+                main, side = th.cuda.current_stream(), self._static["side_stream2"]
+                side.wait_stream(main)
+                with th.cuda.stream(side):
+                    h_tg = tg.forward_hidden(nobs, wset)
+                h_on = on.forward_hidden(nobs, wset)
+                main.wait_stream(side)
+            (w_on, sw_on, b_on), (w_tg, sw_tg, b_tg) = on.head_operands(), tg.head_operands()
+            # after a chained pass the head starts on the tiles the chain wrote last (still in L2)
+            target_q, _, _ = ops.qhead_envelope_td(h_on, h_tg, w_on, w_tg, b_on.detach(), b_tg.detach(), wset, rew, done1, self.gamma, B, W, A, D,
+                                                   self.dot_mode, ops.ROWS_BMAJOR, a_scale_on=on.s_act, a_scale_tg=tg.s_act, w_scale_on=sw_on,
+                                                   w_scale_tg=sw_tg, reverse_tiles=chain is not None)
+            return target_q
+        if self.use_tensor_cores:
+            q_on = self._tc_on.forward_pairs(nobs, wset).view(B, W, A, D)  # online net selects   (envelope.py:420)
+            q_tg = self._tc_tg.forward_pairs(nobs, wset).view(B, W, A, D)  # target net evaluates (envelope.py:429)
+        else:
+            q_on = self.q_net.forward_pairs(nobs, wset)
+            q_tg = self.target_q_net.forward_pairs(nobs, wset)
+        if self.envelope:
+            target_q, _, _ = ops.envelope_td(q_on, q_tg, wset, rew, done1, self.gamma, self.dot_mode, ops.ROWS_BMAJOR, want_indices=False)
+        else:
+            target_q, _ = ops.greedy_td(q_on.view(B * W, A, D), q_tg.view(B * W, A, D), wset, rew, done1, self.gamma, self.dot_mode,
+                                        ops.MAP_TILE, ops.MAP_BLOCK)
+        return target_q
+
+    @th.no_grad()
+    def _tc_step(self, obs, act, rew, nobs, done, wset, raw, device_per: bool):
+        """The update on the tensor cores, without autograd: the training pass's forward, the target, the fused loss (emits d loss / d Q, the
+        loss and the priorities) and the hand-written backward straight into the persistent .grad buffers.  _step has refreshed the weight
+        planes."""
+        s, dp = self._static, self._dp
+        B, W, A, D = self.batch_size, self.num_sample_w, self.action_dim, self.reward_dim
+        # DP-Envelope: this rank's loss rows are those of its own scalarising weights i in [lo, lo + Wt) (all transitions); the targets are
+        # formed for every i because the envelope maximum runs over all preference rows j
+        Wt, lo = (W, 0) if dp is None else (dp["w_loc"], dp["rank"] * dp["w_loc"])
+        wset_t = wset if dp is None else wset[lo : lo + Wt]
+        # the training pass's forward (online net on s) does not depend on the targets: a third branch of the captured graph
+        main, side3 = th.cuda.current_stream(), s["side_stream3"]
+        side3.wait_stream(main)
+        with th.cuda.stream(side3):
+            q_values = self._tc_train.forward_pairs(obs, wset_t).view(B * Wt, A, D)
+        target_q = self._target(rew, nobs, done, wset)
+        if dp is not None:
+            target_q = target_q.view(B, W, D)[:, lo : lo + Wt].reshape(B * Wt, D)
+        main.wait_stream(side3)
+        if self._dq is None:
+            self._dq = th.empty_like(q_values)
+            self._grad_bufs = []
+            if dp is not None:
+                from ...parallel import DPFlat
+
+                dp["flat"] = DPFlat([p for l in self._tc_train.lin for p in (l.weight, l.bias)], B, dp["group"])
+                self._grad_bufs = list(dp["flat"].grads)
+                for prm, gbuf in zip([p for l in self._tc_train.lin for p in (l.weight, l.bias)], self._grad_bufs):
+                    prm.grad = gbuf
+            else:
+                for l in self._tc_train.lin:
+                    for p in (l.weight, l.bias):
+                        p.grad = th.zeros_like(p)
+                        self._grad_bufs.append(p.grad)
+        ops.td_mse_priority(q_values, act.reshape(-1), target_q, wset_t, 0.0, B, Wt, ops.ROWS_BMAJOR, want_grad=True, want_prio=self.per,
+                            workspace=s["ws"], loss_out=s["loss1"], grad_out=self._dq, prio_out=raw, lambda_dev=s["lam"])
+        # device-resident PER: the priority / sum-tree branch (a single-block kernel with 45 KB of shared memory) is forked only AFTER the last
+        # persistent GEMM of the backward pass -- forked right here it keeps one SM, hence one persistent CTA of every GEMM that overlaps it,
+        # waiting; the host-tree modes keep the early hand-off, and DP-Envelope ships after its all-reduce (_dp_finish)
+        ship_after_gemms = dp is None and device_per
+        if dp is None and not device_per:
+            self._ship_results(raw, device_per)
+        for l, (gw, gb) in zip(self._tc_train.lin, zip(self._grad_bufs[0::2], self._grad_bufs[1::2])):
+            if l.weight.grad is not gw or l.bias.grad is not gb:  # (someone called zero_grad(set_to_none=True) in between)
+                l.weight.grad, l.bias.grad = gw, gb
+        self._tc_train.backward(obs, wset_t, self._dq.view(B * Wt, A * D), grads_out=self._grad_bufs,
+                                after_gemms=(lambda: self._ship_results(raw, device_per)) if ship_after_gemms else None)
+
+    def _autograd_step(self, obs, act, rew, nobs, done, wset, raw, device_per: bool):
+        """Explicit validation path (use_tensor_cores=False): torch autograd + library GEMMs around the same fused operators."""
+        s = self._static
+        B, W, A, D = self.batch_size, self.num_sample_w, self.action_dim, self.reward_dim
+        target_q = self._target(rew, nobs, done, wset)
+        q_values = self.q_net.forward_pairs(obs, wset).view(B * W, A, D)
+        loss = _FusedTDLoss.apply(q_values, act.reshape(-1), target_q, wset, s["lam"], B, W, s["ws"], raw, s["loss1"])
+        self._ship_results(raw, device_per)
+        self.q_optim.zero_grad(set_to_none=True)
+        loss.backward()
 
     def _dp_finish(self):
         """Second half of a DP-Envelope update, after the (captured) forward / backward half: ONE all-reduce -- mean gradients into the
@@ -579,15 +573,13 @@ class Envelope(MOPolicy, MOAgent):
         src = s["copy_" + ("device" if mode == "device_per" else mode)][0]  # the segment of the staging buffer this mode's host->device copy fills
         s["work"][src.storage_offset() : src.storage_offset() + src.numel()].copy_(src)
         s["consumed"].record()  # the staging buffer may now be refilled for the next step
-        pre = _PRE_REFRESH and self._tc_on is not None and self.use_tensor_cores
-        if pre:
-            # the weight planes of this step (online, target, transposed) depend only on the parameters: split them on a side branch while the
-            # main branch walks the tree and gathers the minibatch
+        if self.use_tensor_cores:
+            # every weight plane of this step (online, target, transposed for the backward) in one launch: they depend only on the parameters,
+            # so they are split on a side branch while the main branch walks the tree and gathers the minibatch
             main, side = th.cuda.current_stream(), s["side_stream2"]
             side.wait_stream(main)
             with th.cuda.stream(side):
-                TCPairMlp.refresh_many([self._tc_on, self._tc_tg], transposed_of=[self._tc_train] if self._tc_train is not None else [])
-            self._planes_fresh = True
+                TCPairMlp.refresh_many([self._tc_on, self._tc_tg], transposed_of=[self._tc_train])
         if mode == "device_per":
             # SumTree.sample on the device (prioritized_buffer.py:30-54): the host only supplied B uniform doubles from the numpy stream
             self.replay_buffer.tree.walk_into(s["u"], s["idx_out"], scale_by_root=True)
@@ -600,57 +592,21 @@ class Envelope(MOPolicy, MOAgent):
         else:
             st = s["stage"]
             obs, act, rew, nobs, done = st["obs"], st["act"], st["rew"], st["nobs"], st["done"]
-        if pre:
+        if self.use_tensor_cores:
             th.cuda.current_stream().wait_stream(s["side_stream2"])
         self._gradient_step(obs, act, rew, nobs, done, s["wset"], device_per=(mode == "device_per"))
         if self._side_pending:  # join the priority / tree branch
             th.cuda.current_stream().wait_stream(s["side_stream"])
             self._side_pending = False
 
-    def _snapshot(self):
-        snap = {"p": [p.detach().clone() for p in self.q_net.parameters()], "o": []}
-        for p in self.q_net.parameters():
-            st = self.q_optim.state.get(p, None)
-            snap["o"].append(None if not st else {k: (v.clone() if th.is_tensor(v) else v) for k, v in st.items()})
+    def _mutated_tensors(self):
+        """What a step writes that capture must leave as it found it: parameters, optimiser state and, with the sum tree in HBM, the tree
+        and min_priority."""
+        ts = list(self.q_net.parameters()) + optimizer_tensors(self.q_optim)
         rb = self.replay_buffer
-        if getattr(rb, "tree_on_device", False):  # the captured step also writes the device sum tree and min_priority
-            snap["tree"] = (rb.tree.flat.clone(), rb._min_p_dev.clone())
-        return snap
-
-    def _restore(self, snap):
-        with th.no_grad():
-            for p, saved, st_saved in zip(self.q_net.parameters(), snap["p"], snap["o"]):
-                p.copy_(saved)
-                st = self.q_optim.state.get(p, None)
-                if st:
-                    for k, v in st.items():
-                        if th.is_tensor(v):
-                            v.copy_(st_saved[k]) if st_saved is not None else v.zero_()
-            if "tree" in snap:
-                self.replay_buffer.tree.flat.copy_(snap["tree"][0])
-                self.replay_buffer._min_p_dev.copy_(snap["tree"][1])
-
-    def _capture(self, mode: str):
-        """Warm up on a side stream, capture one step into a CUDA graph, then restore parameters and optimiser state IN
-        PLACE so the warm-up iterations leave no trace (parity with the reference's update count)."""
-        self._ensure_static()
-        if mode == "device":
-            self.replay_buffer.flush()
-        snap = self._snapshot()
-        side = th.cuda.Stream()
-        side.wait_stream(th.cuda.current_stream())
-        with th.cuda.stream(side):
-            for _ in range(3):
-                self._step(mode)
-        th.cuda.current_stream().wait_stream(side)
-        g = th.cuda.CUDAGraph()
-        before = ops.launch_count
-        with th.cuda.graph(g):
-            self._step(mode)
-        self.launches_per_step = ops.launch_count - before
-        self._restore(snap)
-        self._graphs[mode] = g
-        return g
+        if getattr(rb, "tree_on_device", False):
+            ts += [rb.tree.flat, rb._min_p_dev]
+        return ts
 
     def __sample_indices(self):
         if self.per:
@@ -702,10 +658,11 @@ class Envelope(MOPolicy, MOAgent):
                 th.cuda.current_stream().wait_stream(s["side_stream"])
                 self._side_pending = False
             if self.use_cuda_graph:
-                g = self._graphs.get(mode) or self._capture(mode)
                 if has_mirror:
-                    rb.flush()
-                g.replay()
+                    rb.flush()  # new transitions into the HBM mirror: a replay does not run the host-side flush of device_stores()
+                g = self._graphs.get_or_build(mode, lambda: GraphedStep(partial(self._step, mode), self._mutated_tensors))
+                g()
+                self.launches_per_step = g.launches
             else:
                 self._step(mode)
             if self._dp is not None:

@@ -15,7 +15,7 @@ from oracle.ref_harness import FakeEnv
 pytestmark = pytest.mark.gpu
 
 
-def _run(cuda, per, tc, graph, lam=0.0, envelope=True, steps=3, W=8, net=(64, 64, 64), param_atol=2e-6):
+def _run(cuda, per, tc, graph, lam=0.0, envelope=True, steps=3, W=8, net=(64, 64, 64), param_atol=2e-6, replay_on_device=True):
     from morl_baselines_b200.common.weights import random_weights
     from morl_baselines_b200.multi_policy.envelope.envelope import Envelope
 
@@ -23,7 +23,8 @@ def _run(cuda, per, tc, graph, lam=0.0, envelope=True, steps=3, W=8, net=(64, 64
     net = list(net)
     th.manual_seed(0)
     agent = Envelope(FakeEnv(obs_dim=OBS, n_actions=A, reward_dim=D), batch_size=B, num_sample_w=W, per=per, buffer_size=N, net_arch=net,
-                     log=False, seed=3, device=cuda, use_cuda_graph=graph, use_tensor_cores=tc, initial_homotopy_lambda=lam, envelope=envelope)
+                     log=False, seed=3, device=cuda, use_cuda_graph=graph, use_tensor_cores=tc, initial_homotopy_lambda=lam, envelope=envelope,
+                     replay_on_device=replay_on_device)
     assert agent.use_tensor_cores == tc
     store = synthetic_store(N, OBS, A, D, seed=1)
     rb = agent.replay_buffer
@@ -82,12 +83,26 @@ def test_envelope_update_homotopy_and_ddqn(cuda):
     assert all(np.isfinite(losses))
 
 
-def test_graph_and_eager_paths_agree_bitwise(cuda):
-    l_graph, a_g = _run(cuda, per=True, tc=True, graph=True)
-    l_eager, a_e = _run(cuda, per=True, tc=True, graph=False)
+# the graph's mode: sum tree in HBM ("device_per"), HBM replay mirror without PER ("device"), host-resident buffer with PER ("host")
+MODES = {"device_per": dict(per=True), "device": dict(per=False), "host": dict(per=True, replay_on_device=False)}
+
+
+def _graph_equals_eager(cuda, mode):
+    l_graph, a_g = _run(cuda, tc=True, graph=True, **MODES[mode])
+    assert list(a_g._graphs) == [mode]
+    l_eager, a_e = _run(cuda, tc=True, graph=False, **MODES[mode])
     assert l_graph == l_eager
     for v, v2 in zip(a_g.q_net.state_dict().values(), a_e.q_net.state_dict().values()):
         assert th.equal(v, v2)
+
+
+def test_graph_and_eager_paths_agree_bitwise(cuda):
+    _graph_equals_eager(cuda, "device_per")
+
+
+@pytest.mark.parametrize("mode", ["device", "host"])
+def test_graph_and_eager_paths_agree_bitwise_in_other_modes(cuda, mode):
+    _graph_equals_eager(cuda, mode)
 
 
 def test_envelope_api_surface(cuda):

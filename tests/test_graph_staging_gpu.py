@@ -1,11 +1,11 @@
-"""The graph inputs of every graphed learner update are staged through pinned memory (common/graphed.Staging).  When the host runs
-ahead of the device, a pinned input must not be rewritten while the asynchronous copy that reads it is still queued; otherwise an
-update trains on a later update's minibatch.
+"""The graph inputs of every graphed learner update are staged through pinned memory (common/graphed.Staging; Envelope: its one
+pinned per-step pack).  When the host runs ahead of the device, a pinned input must not be rewritten while the asynchronous copy that
+reads it is still queued; otherwise an update trains on a later update's minibatch.
 
 Each case runs the same updates on two identically seeded agents with no injected noise.  Agent A captures its graphs, then holds the
 stream with one bounded device spin and queues all updates without a synchronise, so the host is certainly ahead of the device.  Agent
 B synchronises after every update.  Every parameter, optimiser moment and step counter, and every other tensor the learner keeps
-(``log_alpha``, the temperature, the last losses) must be equal bit for bit."""
+(``log_alpha``, the temperature, the last losses, Envelope's sum tree) must be equal bit for bit."""
 
 import random
 
@@ -163,8 +163,46 @@ def _morld_mosac(cuda):
     return algo, [update], [update] * K, lambda: [x for p in algo.population for x in _tensors(p.wrapped, f"population[{p.id}].")]
 
 
+def _envelope(mode):
+    """Envelope in one graph mode: sum tree in HBM ("device_per"), HBM replay mirror without PER ("device"), host-resident buffer ("host")."""
+
+    def case(cuda):
+        from morl_baselines_b200.multi_policy.envelope.envelope import Envelope
+
+        OBS, A, D = 12, 4, 3
+        per = mode != "device"
+        agent = Envelope(FakeEnv(obs_dim=OBS, n_actions=A, reward_dim=D), batch_size=32, num_sample_w=8, per=per, buffer_size=256,
+                         net_arch=[64, 64, 64], gradient_updates=4, target_net_update_freq=2, log=False, seed=3, device=cuda,
+                         replay_on_device=mode != "host")
+        rb = agent.replay_buffer
+        _fill(rb, np.random.default_rng(5), 256, OBS, 1, D, act_dtype=np.uint8, discrete=A)
+        if per:
+            rb.tree.batch_set(np.arange(256), np.random.default_rng(6).random(256) + 0.01)
+        agent.global_step = 1
+
+        def update():
+            agent.update()
+            agent.global_step += 1
+
+        def state():
+            out = _tensors(agent)
+            if per:
+                out += [("replay_buffer.tree", th.from_numpy(np.concatenate(rb.tree.nodes))),
+                        ("replay_buffer.min_priority", th.tensor(rb.min_priority, dtype=th.float64))]
+            return out
+
+        def warmup():
+            update()
+            assert list(agent._graphs) == [mode]
+
+        return agent, [warmup], [update] * K, state
+
+    return case
+
+
 CASES = {"mosac": _mosac, "mosac_discrete": _mosac_discrete, "capql": _capql, "gpils": _gpils, "gpils_continuous": _gpils_continuous,
-         "mo_ppo": _mo_ppo, "morld_mosac": _morld_mosac}
+         "mo_ppo": _mo_ppo, "morld_mosac": _morld_mosac, "envelope_device_per": _envelope("device_per"), "envelope_device": _envelope("device"),
+         "envelope_host": _envelope("host")}
 
 
 def _run(case, cuda, held: bool):
