@@ -603,6 +603,35 @@ MORL_API int morl_pcn_update_f32(const float* const* params, float* const* grads
 MORL_API int morl_pcn_forward_f32(const float* const* params, const float* scaling, const float* obs, const float* ret, const float* hor, int N,
                                   int obs_dim, int d, int hidden, int n_out, int log_softmax, float* out, int32_t* argmax_out, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * EUPG (reference single_policy/esr/eupg.py), csrc/eupg.cu.
+ *
+ * The policy network (eupg.py:22-75): x = [obs (S) || accrued reward (d)], hidden layers a = tanh(W a + b) of widths hidden[0..n_hidden-1],
+ *   logits z = W_L a + b_L [A], p = sigmoid(z) / sum_a sigmoid(z_a) per row, log p_a = log(clamp(p_a, 2^-23, 1 - 2^-23)) (no gradient
+ *   where the clamp acts).  params / grads: HOST arrays of 2 (n_hidden + 1) device pointers in state-dict order: W_0 [h_0, S + d], b_0,
+ *   ..., W_L [A, h_last], b_L [A].  hidden: HOST int array [n_hidden].
+ * Supported range (morl_eupg_supported, no device needed): 1 <= S, 1 <= d <= MORL_MAX_D, S + d <= 256, 1 <= n_hidden <= 4, every width in
+ *   [1, 256], 1 <= A <= 32; anything else returns MORL_ERR_UNSUPPORTED.
+ *
+ * morl_eupg_returns_f32 (eupg.py:263-270): out [T, d] = discounted forward returns of rewards [T, d] (row stride ld floats), c = gamma * c + r_t
+ *   from t = T - 1 down to 0, product and sum rounded separately in float32: bit-identical to the reference's loop.  Any d >= 1 (it is not
+ *   limited to MORL_MAX_D: objectives are independent).  out: contiguous [T, d].  One launch.
+ * morl_eupg_update_f32 (eupg.py:226-251): one episode of T rows, row t reading obs int32 [S] at obs + t * ld, the accrued reward f32 [d] at
+ *   acc + t * ld and the action int32 (in [0, A)) at actions + t * ld (one interleaved staging block), and v[t * v_stride] (v_stride >= 0;
+ *   0 broadcasts one value).  loss_out[0] = -mean_t(log p_{action_t} * v_t); grads[t] are OVERWRITTEN with d loss / d params[t].
+ *   Deterministic: a fixed number of CTAs folds contiguous ranges of 16-row tiles in order, then a fixed-order sum over the CTAs (no float
+ *   atomics); results depend on neither the SM count nor the run.  Two launches.  workspace: morl_eupg_workspace_bytes(...) bytes, which do
+ *   not depend on T.
+ * morl_eupg_probs_f32 (eupg.py:46-61): p [N, A] of rows x [N, S + d]; x and out may be pinned host memory.  One launch. */
+MORL_API int morl_eupg_supported(int obs_dim, int d, const int* hidden, int n_hidden, int n_out);
+MORL_API size_t morl_eupg_workspace_bytes(int obs_dim, int d, const int* hidden, int n_hidden, int n_out);
+MORL_API int morl_eupg_returns_f32(const float* rewards, int ld, int T, int d, float gamma, float* out, void* stream);
+MORL_API int morl_eupg_update_f32(const float* const* params, float* const* grads, const int32_t* obs, const float* acc, const int32_t* actions,
+                                  int ld, const float* v, int v_stride, int T, int obs_dim, int d, const int* hidden, int n_hidden, int n_out,
+                                  float* loss_out, void* workspace, void* stream);
+MORL_API int morl_eupg_probs_f32(const float* const* params, const float* x, int N, int obs_dim, int d, const int* hidden, int n_hidden,
+                                 int n_out, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -96,6 +96,11 @@ SIGNATURES = {
     "morl_pcn_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
     "morl_pcn_update_f32": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "morl_pcn_forward_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "morl_eupg_supported": (_i, [_i, _i, _vp, _i, _i]),
+    "morl_eupg_workspace_bytes": (_sz, [_i, _i, _vp, _i, _i]),
+    "morl_eupg_returns_f32": (_i, [_vp, _i, _i, _i, _f, _vp, _vp]),
+    "morl_eupg_update_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp]),
+    "morl_eupg_probs_f32": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _i, _vp, _vp]),
 }
 
 SPLIT_MAX_JOBS = 16

@@ -1133,3 +1133,139 @@ def pcn_forward(params, scaling: th.Tensor, obs: th.Tensor, ret: th.Tensor, hor:
                                           int(out.shape[1]), int(bool(log_softmax)), _ptr(out), _ptr(argmax_out), _stream())
     _lib.check(rc, "morl_pcn_forward_f32")
     _count()
+
+
+# ---- EUPG (csrc/eupg.cu) -------------------------------------------------------------------------------------------------------------
+def _int_array(values):
+    import ctypes
+
+    vals = [int(x) for x in values]
+    return (ctypes.c_int * max(1, len(vals)))(*vals), len(vals)
+
+
+def eupg_supported(obs_dim: int, d: int, hidden, n_out: int) -> bool:
+    """Whether the fused EUPG kernels cover this policy network: 1 <= obs_dim, 1 <= d <= 8, obs_dim + d <= 256, 1 to 4 hidden layers of
+    widths 1 to 256, 1 <= n_out <= 32 (include/morl_b200.h).  Needs no device."""
+    arr, n = _int_array(hidden)
+    return bool(_lib.load().morl_eupg_supported(int(obs_dim), int(d), arr, n, int(n_out)))
+
+
+class EupgNet:
+    """What the EUPG kernels need about one network: its shape and the host pointer tables of its parameters and gradients.  Build it
+    once per set of storages (the tables hold raw device pointers)."""
+
+    def __init__(self, obs_dim: int, d: int, hidden, n_out: int, params, grads=None):
+        self.obs_dim, self.d, self.n_out = int(obs_dim), int(d), int(n_out)
+        self.hidden, self.n_hidden = _int_array(hidden)
+        if not _lib.load().morl_eupg_supported(self.obs_dim, self.d, self.hidden, self.n_hidden, self.n_out):
+            raise _lib.MorlB200Error(f"EupgNet: unsupported configuration obs_dim={obs_dim} d={d} hidden={list(hidden)} n_out={n_out}")
+        self.params = self._table(params, "param")
+        self.grads = None if grads is None else self._table(grads, "grad")
+
+    def _table(self, tensors, what):
+        import ctypes
+
+        ts = list(tensors)
+        if len(ts) != 2 * (self.n_hidden + 1):
+            raise _lib.MorlB200Error(f"EUPG kernels take {2 * (self.n_hidden + 1)} {what} tensors, got {len(ts)}")
+        for i, t in enumerate(ts):
+            _dev_view(t, f"eupg {what} {i}")
+            if not t.is_contiguous():
+                raise _lib.MorlB200Error(f"eupg {what} {i} must be contiguous")
+        return (ctypes.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+
+    @property
+    def workspace_bytes(self) -> int:
+        return int(_lib.load().morl_eupg_workspace_bytes(self.obs_dim, self.d, self.hidden, self.n_hidden, self.n_out))
+
+    def workspace(self, device) -> th.Tensor:
+        return th.empty((self.workspace_bytes + 7) // 8, device=device, dtype=th.float64)
+
+
+def eupg_workspace_bytes(obs_dim: int, d: int, hidden, n_out: int) -> int:
+    arr, n = _int_array(hidden)
+    return int(_lib.load().morl_eupg_workspace_bytes(int(obs_dim), int(d), arr, n, int(n_out)))
+
+
+def _dev_view(t: th.Tensor, name: str, dtype=th.float32) -> th.Tensor:
+    """A CUDA tensor of ``dtype``, checked without copying: the EUPG kernels read strided views of one staging block in place."""
+    if not isinstance(t, th.Tensor) or not t.is_cuda:
+        raise _lib.MorlB200Error(f"{name} must be a CUDA tensor (morl_baselines_b200 has no CPU fallback)")
+    if t.dtype != dtype:
+        raise _lib.MorlB200Error(f"{name} must have dtype {dtype}, got {t.dtype}")
+    return t
+
+
+def _eupg_rows(t: th.Tensor, name: str, cols: int, dtype=th.float32) -> th.Tensor:
+    """[T, cols] with contiguous columns and a non-negative row stride."""
+    _dev_view(t, name, dtype)
+    if t.dim() != 2 or t.shape[1] != cols or (cols > 1 and t.stride(1) != 1) or t.stride(0) < 0:
+        raise _lib.MorlB200Error(f"{name} must be [T, {cols}] with contiguous columns, got shape {tuple(t.shape)} strides {t.stride()}")
+    return t
+
+
+def eupg_returns(rewards: th.Tensor, gamma: float, out: Optional[th.Tensor] = None) -> th.Tensor:
+    """Discounted forward returns of an episode's rewards [T, d] (rows may be strided, columns contiguous), bit-identical to the
+    reference's float32 loop ``c = gamma * c + r_t`` run backward (eupg.py:263-270), for any number of objectives.  ``out``: a
+    contiguous float32 [T, d] CUDA tensor, allocated when not given."""
+    if not isinstance(rewards, th.Tensor) or rewards.dim() != 2:
+        raise _lib.MorlB200Error("eupg_returns: rewards must be a [T, d] tensor")
+    T, d = rewards.shape
+    _eupg_rows(rewards, "rewards", d)
+    if out is None:
+        out = th.empty((T, d), device=rewards.device, dtype=th.float32)
+    elif not (isinstance(out, th.Tensor) and out.is_cuda and out.dtype == th.float32 and tuple(out.shape) == (T, d) and out.is_contiguous()):
+        raise _lib.MorlB200Error(f"eupg_returns: out must be a contiguous float32 CUDA tensor of shape {(T, d)}")
+    rc = _lib.load().morl_eupg_returns_f32(_ptr(rewards), int(rewards.stride(0)), int(T), int(d), float(gamma), _ptr(out), _stream())
+    _lib.check(rc, "morl_eupg_returns_f32")
+    _count()
+    return out
+
+
+def eupg_update(net: EupgNet, obs: th.Tensor, acc: th.Tensor, actions: th.Tensor, v: th.Tensor, loss_out: th.Tensor, workspace: th.Tensor):
+    """One EUPG episode update (reference eupg.py:236-251): rows ``obs`` int32 [T, S], ``acc`` f32 [T, d] and ``actions`` int32 [T] are
+    views with one common row stride (columns of one staging block), read in place; ``v`` f32 [T] or one element (broadcast).  Writes
+    the loss into ``loss_out`` [>= 1] and overwrites the gradients of ``net.grads``."""
+    if net.grads is None:
+        raise _lib.MorlB200Error("eupg_update: the EupgNet was built without gradient tensors")
+    _eupg_rows(obs, "obs", net.obs_dim, th.int32)
+    _eupg_rows(acc, "acc", net.d)
+    _dev_view(actions, "actions", th.int32)
+    _dev_view(v, "v")
+    _dev_view(loss_out, "loss_out")
+    _dev_view(workspace, "workspace", workspace.dtype)
+    T = obs.shape[0]
+    ld = obs.stride(0)
+    if actions.dim() != 1 or acc.stride(0) != ld or actions.stride(0) != ld or acc.shape[0] != T or actions.shape[0] != T:
+        raise _lib.MorlB200Error("eupg_update: obs, acc and actions must be rows of one block with a common row stride")
+    if loss_out.numel() < 1 or not loss_out.is_contiguous():
+        raise _lib.MorlB200Error("eupg_update: loss_out must be a contiguous float32 CUDA tensor with at least one element")
+    if not workspace.is_contiguous() or workspace.numel() * workspace.element_size() < net.workspace_bytes:
+        raise _lib.MorlB200Error(f"eupg_update: workspace must be contiguous and hold {net.workspace_bytes} bytes")
+    if v.numel() == 1:
+        v_stride = 0
+    elif v.dim() == 1 and v.shape[0] == T and v.stride(0) >= 0:
+        v_stride = int(v.stride(0))
+    else:
+        raise _lib.MorlB200Error(f"eupg_update: v must have T={T} elements or one, got shape {tuple(v.shape)}")
+    rc = _lib.load().morl_eupg_update_f32(net.params, net.grads, _ptr(obs), _ptr(acc), _ptr(actions), int(ld), _ptr(v), v_stride, int(T),
+                                          net.obs_dim, net.d, net.hidden, net.n_hidden, net.n_out, _ptr(loss_out), _ptr(workspace), _stream())
+    _lib.check(rc, "morl_eupg_update_f32")
+    _count(2)
+
+
+def eupg_probs(net: EupgNet, x: th.Tensor, out: th.Tensor):
+    """Action probabilities [N, A] of rows ``x`` [N, S + d] (reference eupg.py:46-61 after Categorical's renormalisation).  ``x`` and
+    ``out`` may be contiguous CUDA tensors or pinned host tensors; with a pinned output the caller synchronises the stream before reading
+    it."""
+    _dev_or_pinned(x, "x")
+    _dev_or_pinned(out, "out")
+    N = x.shape[0] if x.dim() == 2 else 0
+    if x.dim() != 2 or N < 1 or x.shape[1] != net.obs_dim + net.d:
+        raise _lib.MorlB200Error(f"eupg_probs: x must be [N, {net.obs_dim + net.d}], got {tuple(x.shape)}")
+    if tuple(out.shape) != (N, net.n_out):
+        raise _lib.MorlB200Error(f"eupg_probs: out must be {(N, net.n_out)}, got {tuple(out.shape)}")
+    rc = _lib.load().morl_eupg_probs_f32(net.params, _ptr(x), int(N), net.obs_dim, net.d, net.hidden, net.n_hidden, net.n_out, _ptr(out),
+                                         _stream())
+    _lib.check(rc, "morl_eupg_probs_f32")
+    _count()

@@ -2,10 +2,11 @@
 
     compute-sanitizer --tool memcheck|racecheck|synccheck|initcheck python scripts/sanitize_all.py [group ...]
 
-groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners ppo pcn (default: all; dyna includes the fused Dyna commit).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
+groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners ppo pcn eupg (default: all; dyna includes the fused Dyna commit).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
 every code path: all envelope kernel families, both GEMM operand formats x CTA modes x accumulator modes, MN split-K GEMM with the fused
 column sums, every split / reduction helper, the loss kernels (discrete SAC's included), Adam, polyak, Pareto + front records, replay gather,
-the corner-weight enumeration, MO-PPO's vector GAE and loss (racecheck: the loss kernel's CTA reductions), PCN's update and forward."""
+the corner-weight enumeration, MO-PPO's vector GAE and loss (racecheck: the loss kernel's CTA reductions), PCN's update and forward,
+EUPG's returns, update and probabilities."""
 import os
 import sys
 
@@ -23,7 +24,7 @@ if os.environ.get("SAN_ZERO_PLANES") == "1":
     # from a genuine read of memory nobody wrote.
     _empty = ops.empty_planes
     ops.empty_planes = lambda *a, **k: _empty(*a, **k).zero_()
-groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain", "corners", "ppo", "pcn"}
+groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain", "corners", "ppo", "pcn", "eupg"}
 
 
 def rn(*s, scale=1.0):
@@ -253,4 +254,27 @@ if "pcn" in groups:
                         H, not cont, pin_out)
     th.cuda.synchronize()
     print("pcn ok")
+if "eupg" in groups:
+    # EUPG (csrc/eupg.cu): a ragged last tile, T = 1, a T that gives each CTA several tiles (> 128 * 16 rows), width 50 and 256, one
+    # action, a scalar v; the returns kernel over several chunks; the probabilities on device and pinned rows
+    from morl_baselines_b200.single_policy.esr.eupg import PolicyNet, policy_tensors
+
+    for arch, S, d, A, T in [([50], 1, 2, 2, 37), ([50], 3, 2, 4, 1), ([256], 8, 3, 32, 5000), ([17, 5], 2, 2, 1, 20), ([256, 50, 3, 7], 4, 8, 5, 70)]:
+        net = PolicyNet((S,), A, d, arch).to(dev)
+        ts = policy_tensors(net)
+        knet = ops.EupgNet(S, d, arch, A, ts, [th.empty_like(t) for t in ts])
+        ld = S + 2 * d + 1
+        block = rn(T, ld)
+        block[:, :S] = th.randint(-3, 4, (T, S), device=dev, generator=g).int().view(th.float32)
+        block[:, S + d] = th.randint(0, A, (T,), device=dev, generator=g).int().view(th.float32)
+        fwd = ops.eupg_returns(block[:, S + d + 1:], 0.99)
+        v = fwd.sum(1) if T > 1 else fwd.sum().reshape(())
+        ops.eupg_update(knet, block[:, :S].view(th.int32), block[:, S:S + d], block[:, S + d].view(th.int32), v, th.zeros(1, device=dev),
+                        knet.workspace(dev))
+        out = th.zeros(7, A, device=dev)
+        ops.eupg_probs(knet, rn(7, S + d), out)
+        pin_out = th.zeros(1, A).pin_memory()
+        ops.eupg_probs(knet, th.ones(1, S + d).pin_memory(), pin_out)
+    th.cuda.synchronize()
+    print("eupg ok")
 print("sanitize run ok")
