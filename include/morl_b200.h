@@ -501,11 +501,13 @@ MORL_API size_t morl_gemm_mn_workspace_bytes(int M, int a_cols, int b_cols);
 MORL_API int morl_gemm_planes_mn_f32(int fmt, const void* g_planes, long long g_plane_stride, int ldg, int g_cols, const float* g_scale,
                                      const void* h_planes, long long h_plane_stride, int ldh, int h_cols, const float* h_scale, int M,
                                      int transpose_out, float* out, int ld_out, float* colsum_out, void* workspace, void* stream);
-/* out[n] = (1 / *scale) sum_m sum_p planes[p][m][n]  (bias gradients); workspace: 296 * N floats */
+/* out[n] = (1 / *scale) sum_m sum_p planes[p][m][n]  (bias gradients); workspace: morl_colsum_workspace_bytes(N) bytes */
+MORL_API size_t morl_colsum_workspace_bytes(int N);
 MORL_API int morl_colsum_planes(int fmt, const void* planes, long long plane_stride, const float* scale, int M, int ld, int N, float* out,
                                 void* workspace, void* stream);
 /* gradients of the separable first layer: dU[b,:] = sum_j G[b*W+j,:], dV[j,:] = sum_b G[b*W+j,:]  (G planes [P][B*W][H] scaled by
- * *scale, W <= 64 for the one-pass kernel); workspace: 296 * W * H floats */
+ * *scale, W <= 64 for the one-pass kernel); workspace: morl_pairs_grad_reduce_workspace_bytes(B, W, H) bytes */
+MORL_API size_t morl_pairs_grad_reduce_workspace_bytes(int B, int W, int H);
 MORL_API int morl_pairs_grad_reduce_planes(int fmt, const void* planes, long long plane_stride, const float* scale, int B, int W, int H,
                                            float* dU, float* dV, void* workspace, void* stream);
 

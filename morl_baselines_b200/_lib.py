@@ -81,7 +81,9 @@ SIGNATURES = {
     "morl_pairs_product_split_planes": (_i, [_i, _vp, _vp, _i, _i, _i, _vp, C.c_longlong, _vp, _vp]),
     "morl_gemm_mn_workspace_bytes": (_sz, [_i, _i, _i]),
     "morl_gemm_planes_mn_f32": (_i, [_i, _vp, C.c_longlong, _i, _i, _vp, _vp, C.c_longlong, _i, _i, _vp, _i, _i, _vp, _i, _vp, _vp, _vp]),
+    "morl_colsum_workspace_bytes": (_sz, [_i]),
     "morl_colsum_planes": (_i, [_i, _vp, C.c_longlong, _vp, _i, _i, _i, _vp, _vp, _vp]),
+    "morl_pairs_grad_reduce_workspace_bytes": (_sz, [_i, _i, _i]),
     "morl_pairs_grad_reduce_planes": (_i, [_i, _vp, C.c_longlong, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "morl_pair_layer1_uv_f32": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "morl_product_layer1_uv_f32": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),

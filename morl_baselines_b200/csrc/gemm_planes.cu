@@ -1901,13 +1901,34 @@ extern "C" int morl_gemm_planes_mn_f32(int fmt, const void* g_planes, long long 
     return check_launch("morl_gemm_planes_mn_f32(reduce)");
 }
 
+// Row chunks of the split column sums: each chunk writes one row of partials to the workspace, reduced in a fixed order afterwards.
+constexpr int kColsumChunks = 296;     // morl_colsum_planes
+constexpr int kPgrFusedChunks = 296;   // morl_pairs_grad_reduce_planes, one-pass form
+constexpr int kPgrTwoPassChunks = 74;  // morl_pairs_grad_reduce_planes, two-pass form
+
+// Transitions per chunk of the one-pass pairs_grad_reduce (at most kPgrMaxB, at most kPgrFusedChunks chunks), or 0 when the two-pass
+// form runs instead.
+static int pgr_fused_rows_per_chunk(int B, int W) {
+    if (W > 64) return 0;
+    int bpc = (B + kPgrFusedChunks - 1) / kPgrFusedChunks;
+    if (bpc > morl::kPgrMaxB) bpc = morl::kPgrMaxB;
+    return (B + bpc - 1) / bpc <= kPgrFusedChunks ? bpc : 0;
+}
+
+extern "C" size_t morl_colsum_workspace_bytes(int N) { return N > 0 ? (size_t)kColsumChunks * N * sizeof(float) : 0; }
+
+extern "C" size_t morl_pairs_grad_reduce_workspace_bytes(int B, int W, int H) {
+    if (B <= 0 || W <= 0 || H <= 0) return 0;
+    return (size_t)(pgr_fused_rows_per_chunk(B, W) ? kPgrFusedChunks : kPgrTwoPassChunks) * W * H * sizeof(float);
+}
+
 extern "C" int morl_colsum_planes(int fmt, const void* planes, long long plane_stride, const float* scale, int M, int ld, int N, float* out,
                                   void* workspace, void* stream) {
     using namespace morl;
     MORL_REQUIRE(fmt_ok(fmt), MORL_ERR_UNSUPPORTED, "morl_colsum_planes: unknown plane format %d", fmt);
     MORL_REQUIRE(planes && out && workspace, MORL_ERR_NULL, "morl_colsum_planes: NULL pointer argument");
     MORL_REQUIRE(M > 0 && N > 0 && ld >= N && ld % 8 == 0 && plane_stride % 8 == 0, MORL_ERR_SHAPE, "morl_colsum_planes: bad shape M=%d N=%d ld=%d", M, N, ld);
-    const int chunks = 296;
+    const int chunks = kColsumChunks;
     const int rpc = (M + chunks - 1) / chunks;
     const int nch = (M + rpc - 1) / rpc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1928,25 +1949,21 @@ extern "C" int morl_pairs_grad_reduce_planes(int fmt, const void* planes, long l
     MORL_REQUIRE(B > 0 && W > 0 && H > 0 && H % 8 == 0 && plane_stride % 8 == 0, MORL_ERR_SHAPE, "morl_pairs_grad_reduce_planes: bad shape B=%d W=%d H=%d", B, W, H);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const uint16_t* pl = static_cast<const uint16_t*>(planes);
-    if (W <= 64) {
+    if (const int bpc = pgr_fused_rows_per_chunk(B, W)) {
         // one pass: dU directly, dV as per-chunk partials [chunks][W*H] reduced in a fixed order
-        int bpc = (B + 295) / 296;  // <= 296 chunks (the documented workspace size), at most kPgrMaxB transitions per chunk
-        if (bpc > kPgrMaxB) bpc = kPgrMaxB;
         const int nchf = (B + bpc - 1) / bpc;
-        if (nchf <= 296) {
-            const int Nf = W * H;
-            float* partf = static_cast<float*>(workspace);
-            const size_t smemf = (size_t)kPgrMaxB * 8 * 32 * 9 * sizeof(float);  // 73,728 B
-            MORL_DISPATCH_FMT(fmt, {
-                set_smem_limit_once<pairs_grad_reduce_fused_kernel<kFmt>>(smemf);
-                launch_k(pairs_grad_reduce_fused_kernel<kFmt>, dim3(dim3((unsigned)nchf, (unsigned)((H + 255) / 256))), dim3(dim3(32, 8)), smemf, st, pl, plane_stride, B, W,
-                                                                                                                                     H, bpc, dU, partf, scale);
-            });
-            int rcf = check_launch("morl_pairs_grad_reduce_planes(fused)");
-            if (rcf) return rcf;
-            launch_k(reduce_partials_kernel, dim3((Nf + 31) / 32), dim3(dim3(32, 8)), 0, st, partf, nchf, 1, Nf, 1, Nf, 0, dV, Nf, 1 << 30, nullptr, nullptr, scale, nullptr);
-            return check_launch("morl_pairs_grad_reduce_planes(reduce)");
-        }
+        const int Nf = W * H;
+        float* partf = static_cast<float*>(workspace);
+        const size_t smemf = (size_t)kPgrMaxB * 8 * 32 * 9 * sizeof(float);  // 73,728 B
+        MORL_DISPATCH_FMT(fmt, {
+            set_smem_limit_once<pairs_grad_reduce_fused_kernel<kFmt>>(smemf);
+            launch_k(pairs_grad_reduce_fused_kernel<kFmt>, dim3(dim3((unsigned)nchf, (unsigned)((H + 255) / 256))), dim3(dim3(32, 8)), smemf, st, pl, plane_stride, B, W,
+                                                                                                                                 H, bpc, dU, partf, scale);
+        });
+        int rcf = check_launch("morl_pairs_grad_reduce_planes(fused)");
+        if (rcf) return rcf;
+        launch_k(reduce_partials_kernel, dim3((Nf + 31) / 32), dim3(dim3(32, 8)), 0, st, partf, nchf, 1, Nf, 1, Nf, 0, dV, Nf, 1 << 30, nullptr, nullptr, scale, nullptr);
+        return check_launch("morl_pairs_grad_reduce_planes(reduce)");
     }
     // dU[b] = sum over the W rows of transition b
     MORL_DISPATCH_FMT(fmt, (pairs_rowblock_sum_kernel<kFmt><<<dim3((unsigned)B, (unsigned)((H + 255) / 256)), dim3(32, 8), 0, st>>>(pl, plane_stride, W, H,
@@ -1955,7 +1972,7 @@ extern "C" int morl_pairs_grad_reduce_planes(int fmt, const void* planes, long l
     if (rc) return rc;
     // dV[j] = sum over b: column sums of the [B, W*H] view
     const int N = W * H;
-    const int chunks = 74;
+    const int chunks = kPgrTwoPassChunks;
     const int rpc = (B + chunks - 1) / chunks;
     const int nch = (B + rpc - 1) / rpc;
     float* part = static_cast<float*>(workspace);

@@ -134,8 +134,7 @@ class TCPairMlp:
             # the largest split-K workspace of the weight-gradient products dW_l = G_l^T H_{l-1} of layers 2..
             self.ws_mn = th.empty(max(ops.gemm_mn_workspace_bytes(M, l.out_features, l.in_features) for l in self.lin[1:]) // 4 + 1,
                                   device=dev, dtype=th.float32)
-            # pairs_grad_reduce: per-chunk dV partials, <= 296 chunks in the one-pass form (|W| <= 64), <= 74 in the two-pass form
-            self.ws_red = th.empty((296 if n_w <= 64 else 74) * max(n_w * hid, 256), device=dev, dtype=th.float32)
+            self.ws_red = ops.pairs_grad_reduce_workspace(n_obs, n_w, hid, dev)  # the G planes are hid wide
             first = self.lin[0]
             self.ws_l1 = ops.pair_layer1_grad_workspace(feat_dim, first.in_features - feat_dim, first.out_features, dev)
             self.dU = th.empty((n_obs, first.out_features), device=dev, dtype=th.float32)

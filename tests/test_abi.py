@@ -103,3 +103,15 @@ def test_fusion_coverage_predicates_need_no_device():
     rc = lib.morl_qhead_envelope_td_f32(F16, 16, 16, 0, None, None, 16, 16, 0, None, None, None, None, 256, 16, 16, 16, 0.99, 1024, 48, 8, 3, 0, 0, 0, 16, None, None, None,
                                         None, None)
     assert rc == -4 and b"unsupported configuration" in lib.morl_last_error()
+
+
+def test_reduction_workspaces_cover_the_chunk_partials():
+    """The column-sum reductions write one row of partials per row chunk: up to 296 chunks for morl_colsum_planes and the one-pass
+    pairs_grad_reduce (|W| <= 64, at most 8 transitions per chunk), up to 74 for the two-pass form (|W| > 64, or a batch too large for
+    296 chunks of 8).  The library's byte counts cover them, so no caller needs to know the chunk arithmetic."""
+    from morl_baselines_b200 import _lib
+
+    lib = _lib.load()
+    assert lib.morl_colsum_workspace_bytes(24) >= 296 * 24 * 4
+    for B, W, H, chunks in ((1024, 64, 256, 296), (6, 5, 64, 296), (3, 70, 64, 74), (256, 128, 256, 74), (4096, 8, 64, 74)):
+        assert lib.morl_pairs_grad_reduce_workspace_bytes(B, W, H) >= chunks * W * H * 4, (B, W, H)
