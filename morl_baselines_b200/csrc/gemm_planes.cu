@@ -28,9 +28,9 @@
 //              64-byte swizzle, 2 x 72 KB), mbarrier ring; it keeps loading the next tile while the consumers are in their epilogue.
 // Operands: A [P][M][K] (K-major), B [P][N_pad][K] (K-major), K % BK == 0, N_pad % 32 == 0, N_pad <= 512.  An output wider than 256
 // columns runs as two column units [0, 256) and [256, N_pad) of the same tile, each with the shared-memory plan of N_pad = 256.
-// The chained hidden layers (gemm_chain_kernel) run the same pipeline -- carve_kplan, the producer's load_unit, the consumer's consume_unit and
-// reload_bias -- on their own schedule of units; f16x2 chains run on gemm_chain_resident_kernel, which keeps a CTA's activation tile in shared
-// memory through all layers and streams only the weights.
+// bf16x3 chains of hidden layers (gemm_chain_kernel) run the same pipeline -- carve_kplan, the producer's load_unit, the consumer's consume_unit
+// and reload_bias -- on their own schedule of units; f16x2 chains run on gemm_chain_resident_kernel, which keeps a CTA's activation tile in
+// shared memory through all layers and streams only the weights.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -298,11 +298,30 @@ __device__ __forceinline__ void epilogue_values(const float (&a)[16], int col0, 
     }
 }
 
+// A thread's x[2][8] of such a chunk re-split into P planes of [16 rows][64 B] in shared memory, plane p at base + p plane_stride, in the
+// 64-byte swizzle of a TMA box (16-byte chunk q of row r at q ^ ((r >> 1) & 3): bank-conflict free), two columns per word
+template <int FMT>
+__device__ __forceinline__ void stage_chunk_planes(const float (&x)[2][8], uint8_t* base, uint32_t plane_stride, int lane, float& amax) {
+    using F = PlaneFmt<FMT>;
+    const int l4 = lane & 3, lr = lane >> 2;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int rl = lr + 8 * h;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            uint32_t w[F::P];
+            F::split2(x[h][2 * q], x[h][2 * q + 1], w, amax);
+            uint8_t* st = base + rl * 64 + ((q ^ ((rl >> 1) & 3)) << 4) + 4 * l4;
+#pragma unroll
+            for (int p = 0; p < F::P; ++p) *reinterpret_cast<uint32_t*>(st + p * plane_stride) = w[p];
+        }
+    }
+}
+
 template <int FMT, bool PRE = false>
 __device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, int rbase, int lane, const EpiArgs& e, const CUtensorMap* tmC,
                                                uint8_t* my_stage, uint32_t& n_stored, float& amax) {
-    using F = PlaneFmt<FMT>;
-    constexpr int P = F::P;
+    constexpr int P = PlaneFmt<FMT>::P;
     const int l4 = lane & 3, lr = lane >> 2;
     float x[2][8];
     epilogue_values<PRE>(a, col0, rbase, lane, e, x);
@@ -341,27 +360,21 @@ __device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, i
         }
     }
     if (e.planes && col0 < e.ldp) {
-        // stage the warp's [16 rows x 32 cols] x P planes in shared memory (TMA SWIZZLE_64B pattern: 16-byte chunk index XOR ((row >> 1) & 3),
-        // bank-conflict free), then ONE bulk tensor store writes it out coalesced and asynchronously
+        // stage the warp's [16 rows x 32 cols] x P planes in shared memory, then ONE bulk tensor store writes it out coalesced and asynchronously
         uint8_t* tile = my_stage + (n_stored & 1u) * (uint32_t)(P * 1024);
         ++n_stored;
         if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");  // the store before the previous one has read this tile
         __syncwarp();
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int rl = lr + 8 * h;
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
                 const int col = col0 + 8 * q + 2 * l4;
-                // ragged last chunk: columns [N, ldp) are written as zero
-                const float x0 = col < e.N ? x[h][2 * q] * e.c_mul : 0.f, x1 = col + 1 < e.N ? x[h][2 * q + 1] * e.c_mul : 0.f;
-                uint32_t w[P];
-                F::split2(x0, x1, w, amax);  // re-split (c_scale x) into P planes, two columns per word
-                uint8_t* st = tile + rl * 64 + ((q ^ ((rl >> 1) & 3)) << 4) + 4 * l4;
-#pragma unroll
-                for (int p = 0; p < P; ++p) *reinterpret_cast<uint32_t*>(st + p * 1024) = w[p];
+                // (c_scale x); ragged last chunk: columns [N, ldp) are written as zero
+                x[h][2 * q] = col < e.N ? x[h][2 * q] * e.c_mul : 0.f;
+                x[h][2 * q + 1] = col + 1 < e.N ? x[h][2 * q + 1] * e.c_mul : 0.f;
             }
-        }
+        stage_chunk_planes<FMT>(x, tile, 1024, lane, amax);
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncwarp();
         if (lane == 0) {
@@ -611,18 +624,35 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 }
 
 // =================================================================================================================
-// CHAIN kernel: several dense hidden layers of one or two networks in ONE persistent launch (f16x2 / bf16x3 planes, N = 256 wide
-// layers).  A layer's output rows depend only on the same rows of its input, so a CTA can take one of its 128-row tiles through ALL
-// layers: the tile it stores for layer l is the tile it loads for layer l+1 a few units later -- by then still in the 50 MB L2, so only the
-// first layer's input is read from HBM, and the launch prologue / drain is paid once instead of per layer.  Work of a CTA: its tiles in
-// groups of `lanes / n_chains`; per group, for every layer, one unit per LANE (lane = (chain, tile
+// CHAIN kernel: several dense hidden layers of one or two networks in ONE persistent launch (bf16x3 planes, N = 256 wide layers; f16x2
+// chains run on the resident kernel below).  A layer's output rows depend only on the same rows of its input, so a CTA can take one of
+// its 128-row tiles through ALL layers: the tile it stores for layer l is the tile it loads for layer l+1 a few units later -- by then
+// still in the 50 MB L2, so only the first layer's input is read from HBM, and the launch prologue / drain is paid once instead of per
+// layer.  Work of a CTA: its tiles in groups of `lanes / n_chains`; per group, for every layer, one unit per LANE (lane = (chain, tile
 // of the group)): four lanes keep the dependency distance at four units (unit (l, lane) needs the stores of unit (l-1, lane)), so the
 // producer never waits for the epilogue that has just finished.  The shared-memory carve, the producer's load_unit and the consumer's
-// consume_unit are those of gemm_planes_kernel<FMT, 0> (bit-identical outputs: tests/test_gemm_gpu.py); additional barrier stored[lane]: the
-// consumer warps arrive once their bulk stores of the unit have COMPLETED, the producer waits for it before loading the next layer of that lane.
+// consume_unit are those of gemm_planes_kernel<bf16x3, 0> (bit-identical outputs: tests/test_gemm_gpu.py); additional barrier stored[lane]:
+// the consumer warps arrive once their bulk stores of the unit have COMPLETED, the producer waits for it before loading the next layer of
+// that lane.
 // =================================================================================================================
 constexpr int kChainMaxJobs = 8;   // chains x layers
 constexpr int kChainLanes = 4;
+
+// The tiles of both chain kernels on CTA `unit` of n_units: tile t of chain c goes to CTA (t + offset_c) mod n_units with a DIFFERENT rotation
+// per chain: when the tiles do not divide evenly, both chains on the same CTAs would give some CTAs two extra tiles and others none; chain 1
+// rotated by half the grid spreads the remainders (host model: tests/chain_tiles.py).
+struct ChainTiles {
+    int cu0, cu1, mt0, mt1, n_units;
+    __device__ __forceinline__ ChainTiles(int n_tiles, int n_units_, int n_chains, int unit)
+        : cu0(unit), cu1((unit + n_units_ / 2) % n_units_), n_units(n_units_) {
+        mt0 = cu0 < n_tiles ? (n_tiles - cu0 + n_units - 1) / n_units : 0;
+        mt1 = n_chains > 1 && cu1 < n_tiles ? (n_tiles - cu1 + n_units - 1) / n_units : 0;
+    }
+    // number of tiles of chain c on this CTA
+    __device__ __forceinline__ int count(int c) const { return c ? mt1 : mt0; }
+    // first row of tile index ti of chain c on this CTA, or -1
+    __device__ __forceinline__ int row(int ti, int c) const { return ti < count(c) ? ((c ? cu1 : cu0) + ti * n_units) * kGemmBM : -1; }
+};
 
 struct alignas(64) ChainMaps {
     CUtensorMap A[kChainMaxJobs];  // load map of the INPUT of job (chain c, layer l): [P][M][K], box P x 128 x BK
@@ -630,6 +660,7 @@ struct alignas(64) ChainMaps {
     CUtensorMap C[kChainMaxJobs];  // store map of the OUTPUT of the job: [P][M][256], box P x 16 x 32 (64-byte swizzle)
 };
 
+// Arguments of both chain kernels (host: set_chain_args); job (c, l) = layer l of chain c, index c n_layers + l
 struct ChainArgs {
     int M, K;                      // rows, reduction length (= width of the layers: square 256-wide layers, K % BK == 0)
     int k_first;                   // reduction length of layer 0 of every chain (its INPUT may be narrower: the dX product of the output layer), K % BK == 0
@@ -640,12 +671,12 @@ struct ChainArgs {
     const uint32_t* bits_in[kChainMaxJobs];  // ReLU-backward masks applied to the job's output (dX chains), or nullptr
     const float* a_scale;          // activation scale (input AND output of every layer), device scalar or nullptr
     int relu;                      // max(x, 0) on every job's output (forward chains)
-    int n_stages;
+    int n_stages;                  // TMA ring depth of gemm_chain_kernel (KPlan<bf16x3>::kStages; the resident kernel has its own)
 };
 
-template <int FMT>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
+    constexpr int FMT = MORL_FMT_BF16X3;
     using L = KPlan<FMT>;
     constexpr int BN = 256;
     extern __shared__ uint8_t gsmem_raw[];
@@ -654,21 +685,15 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int unit = blockIdx.x, n_units = gridDim.x;
-    const int n_tiles = (g.M + kGemmBM - 1) / kGemmBM;
     const int n_kblk_full = g.K / PlaneFmt<FMT>::BK, n_kblk_first = g.k_first / PlaneFmt<FMT>::BK;
     const int tiles_per_group = kChainLanes / g.n_chains;  // lanes of a group: (tile of the group) x (chain)
-    // Tile t of chain c goes to CTA (t + offset_c) mod n_units with a DIFFERENT rotation per chain: when the tiles do not divide evenly, both
-    // chains on the same CTAs would give some CTAs two extra tiles and others none; rotated by half the grid the remainders spread.
-    const int cu0 = unit, cu1 = (unit + n_units / 2) % n_units;
-    const int mt0 = cu0 < n_tiles ? (n_tiles - cu0 + n_units - 1) / n_units : 0;
-    const int mt1 = g.n_chains > 1 ? (cu1 < n_tiles ? (n_tiles - cu1 + n_units - 1) / n_units : 0) : 0;
-    const int n_groups = ((mt0 > mt1 ? mt0 : mt1) + tiles_per_group - 1) / tiles_per_group;
-    // unit (group gi, layer l, lane ln) -> (job, tile) or tile = -1 (no such tile for this CTA)
-    auto unit_of = [&](int gi, int l, int ln, int& job, int& tile) {
-        const int c = ln % g.n_chains, ti = gi * tiles_per_group + ln / g.n_chains;
+    const ChainTiles tiles((g.M + kGemmBM - 1) / kGemmBM, gridDim.x, g.n_chains, blockIdx.x);
+    const int n_groups = (max(tiles.count(0), tiles.count(1)) + tiles_per_group - 1) / tiles_per_group;
+    // unit (group gi, layer l, lane ln) -> (job, first row of its tile) or row0 = -1 (no such tile for this CTA)
+    auto unit_of = [&](int gi, int l, int ln, int& job, int& row0) {
+        const int c = ln % g.n_chains;
         job = c * g.n_layers + l;
-        tile = ti < (c ? mt1 : mt0) ? (c ? cu1 : cu0) + ti * n_units : -1;
+        row0 = tiles.row(gi * tiles_per_group + ln / g.n_chains, c);
     };
 
     if (threadIdx.x == 0) {
@@ -688,9 +713,9 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
             for (int gi = 0; gi < n_groups; ++gi)
                 for (int l = 0; l < g.n_layers; ++l)
                     for (int ln = 0; ln < kChainLanes; ++ln) {
-                        int job, tile;
-                        unit_of(gi, l, ln, job, tile);
-                        if (tile < 0) continue;
+                        int job, row0;
+                        unit_of(gi, l, ln, job, row0);
+                        if (row0 < 0) continue;
                         if (l > 0) {
                             // the input tile of this unit is the output tile of the lane's previous unit: wait until the stores of
                             // it have completed (completion number done_on_lane[ln] of stored[ln])
@@ -698,7 +723,7 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
                             asm volatile("fence.proxy.async.global;" ::: "memory");
                         }
                         ++done_on_lane[ln];
-                        load_unit<FMT>(s, ring, &maps.A[job], &maps.B[job], tile * kGemmBM, 0, BN, l == 0 ? n_kblk_first : n_kblk_full, false);
+                        load_unit<FMT>(s, ring, &maps.A[job], &maps.B[job], row0, 0, BN, l == 0 ? n_kblk_first : n_kblk_full, false);
                     }
         }
     } else {
@@ -714,9 +739,9 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
         for (int gi = 0; gi < n_groups; ++gi)
             for (int l = 0; l < g.n_layers; ++l)
                 for (int ln = 0; ln < kChainLanes; ++ln) {
-                    int job, tile;
-                    unit_of(gi, l, ln, job, tile);
-                    if (tile < 0) continue;
+                    int job, row0;
+                    unit_of(gi, l, ln, job, row0);
+                    if (row0 < 0) continue;
                     reload_bias(s.bias, g.bias[job], 0, BN, s_act);  // (times the folded output scale)
                     EpiArgs e;
                     e.M = g.M; e.N = BN;
@@ -726,7 +751,7 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
                     e.bias_s = s.bias; e.relu = g.relu; e.bits_in = g.bits_in[job]; e.bits_out = g.bits_out[job]; e.bits_ld = relu_bits_words(BN);
                     e.mask = nullptr; e.ld_mask = 0;
                     e.c_f32 = nullptr; e.ldc = 0; e.planes = 1; e.ldp = BN;
-                    const int rbase = tile * kGemmBM + wg * 64 + (warp & 3) * 16;
+                    const int rbase = row0 + wg * 64 + (warp & 3) * 16;
                     consume_unit<FMT, 0, false>(acc, s, ring, l == 0 ? n_kblk_first : n_kblk_full, 0, BN, rbase, wg, lane, nullptr, [] {}, e,
                                                 &maps.C[job], my_stage, n_stored, amax);
                     // the lane's next layer loads what this unit stored (bit masks included): signal once the bulk stores of this warp have completed
@@ -736,7 +761,6 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
                         g_mbar_arrive(&stored[ln]);
                     }
                 }
-        if (FMT == MORL_FMT_F16X2) note_overflow(amax);
     }
 }
 
@@ -745,10 +769,10 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
 // Layer l's epilogue writes its output chunk c (32 columns) as K-block c of layer l+1's A operand, so no intermediate activation goes
 // through L2 and layer l+1 waits for no global store; the producer streams only weights.  An output leaves by TMA store straight from the
 // tile only when the job's `store` bit is set.  The chain's input is either a TMA load of plane rows (dX chains, GemmChain) or, in pair mode,
-// relu(u[b] + v[j]) s for row b W + j computed by the consumer warps into the tile (the arithmetic of pairs_relu_split_h256_kernel).
+// relu(u[b] + v[j]) s for row b W + j computed by the consumer warps into the tile (pair_split8, as pairs_relu_split_h256_kernel).
 // Schedule of a CTA: its tiles in order, each through every layer of chain 0, then (same tile index, the chain's own rotation) chain 1.
-// Accumulation order = gemm_chain_kernel's: k16 steps in order, products A1B0, A0B1, A0B0 inner (a 32-wide K block issues the same
-// sequence as a 64-wide one), so outputs are bit-identical.
+// Accumulation order = per-layer gemm_planes_kernel<f16x2, 0> launches': k16 steps in order, products A1B0, A0B1, A0B0 inner (a 32-wide
+// K block issues the same sequence as a 64-wide one), so outputs are bit-identical.
 // =================================================================================================================
 struct ResPlan {
     static constexpr int P = 2, BK = 32, kStages = 3;
@@ -770,14 +794,7 @@ struct alignas(64) ResChainMaps {
     CUtensorMap C[kChainMaxJobs];  // stored output of the job [P][M][256], box 1 x 16 x 32 (64-byte swizzle)
 };
 
-struct ResChainArgs {
-    int M, K, k_first, n_chains, n_layers;
-    const float* bias[kChainMaxJobs];
-    const float* b_scale[kChainMaxJobs];
-    uint32_t* bits_out[kChainMaxJobs];
-    const uint32_t* bits_in[kChainMaxJobs];
-    const float* a_scale;
-    int relu;
+struct ResChainArgs : ChainArgs {
     uint32_t store;                // bit job: the job's output is written to global memory
     const float* u[2];             // pair mode (u != nullptr): u[c] [B][256], v[c] [W][256], row r = b W + j
     const float* v[2];
@@ -827,9 +844,30 @@ __device__ __forceinline__ uint8_t* res_chunk(uint8_t* act, int kb, int row, int
     return act + (uint32_t)kb * ResPlan::kKBlock + (uint32_t)row * ResPlan::kRowB + (uint32_t)((q ^ ((row >> 1) & 3)) << 4);
 }
 
+// The pair input of 8 consecutive columns from their pre-activations x (u + v, or the product u v): r = relu(x) (NaN-propagating, like
+// torch.relu) when `relu`, else r = x; o[p][t] = plane p of (r[2 t] s, r[2 t + 1] s).  Returns bit t = (r[t] > 0).
+template <int FMT>
+__device__ __forceinline__ uint32_t pair_split8(const float (&x)[8], bool relu, float s, uint32_t (&o)[PlaneFmt<FMT>::P][4], float& amax) {
+    using F = PlaneFmt<FMT>;
+    uint32_t pos = 0;
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+        float r0 = x[2 * t], r1 = x[2 * t + 1];
+        if (relu) {
+            r0 = r0 < 0.f ? 0.f : r0;
+            r1 = r1 < 0.f ? 0.f : r1;
+        }
+        pos |= (r0 > 0.f ? 1u : 0u) << (2 * t) | (r1 > 0.f ? 1u : 0u) << (2 * t + 1);
+        uint32_t w[F::P];
+        F::split2(r0 * s, r1 * s, w, amax);
+#pragma unroll
+        for (int p = 0; p < F::P; ++p) o[p][t] = w[p];
+    }
+    return pos;
+}
+
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_chain_resident_kernel(const __grid_constant__ ResChainMaps maps, const ResChainArgs g) {
-    using F = PlaneFmt<MORL_FMT_F16X2>;
     using R = ResPlan;
     constexpr int P = R::P, BN = 256;
     extern __shared__ uint8_t gsmem_raw[];
@@ -849,16 +887,9 @@ gemm_chain_resident_kernel(const __grid_constant__ ResChainMaps maps, const ResC
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int unit = blockIdx.x, n_units = gridDim.x;
-    const int n_tiles = (g.M + kGemmBM - 1) / kGemmBM;
     const int n_kblk_full = g.K / R::BK, n_kblk_first = g.k_first / R::BK;
-    // tile t of chain c on CTA (t + offset_c) mod n_units, chain 1 rotated by half the grid (as gemm_chain_kernel: balances ragged tile counts)
-    const int cu0 = unit, cu1 = (unit + n_units / 2) % n_units;
-    const int mt0 = cu0 < n_tiles ? (n_tiles - cu0 + n_units - 1) / n_units : 0;
-    const int mt1 = g.n_chains > 1 ? (cu1 < n_tiles ? (n_tiles - cu1 + n_units - 1) / n_units : 0) : 0;
-    const int n_ti = mt0 > mt1 ? mt0 : mt1;
-    // first row of tile ti of chain c on this CTA, or -1
-    auto tile_row = [&](int ti, int c) { return ti < (c ? mt1 : mt0) ? ((c ? cu1 : cu0) + ti * n_units) * kGemmBM : -1; };
+    const ChainTiles tiles((g.M + kGemmBM - 1) / kGemmBM, gridDim.x, g.n_chains, blockIdx.x);
+    const int n_ti = max(tiles.count(0), tiles.count(1));
 
     if (threadIdx.x == 0) {
         init_ring_barriers(s.full, s.empty, R::kStages);
@@ -878,7 +909,7 @@ gemm_chain_resident_kernel(const __grid_constant__ ResChainMaps maps, const ResC
             uint32_t n_in = 0;  // input tiles loaded
             for (int ti = 0; ti < n_ti; ++ti)
                 for (int c = 0; c < g.n_chains; ++c) {
-                    const int row0 = tile_row(ti, c);
+                    const int row0 = tiles.row(ti, c);
                     if (row0 < 0) continue;
                     for (int l = 0; l < g.n_layers; ++l) {
                         const int job = c * g.n_layers + l;
@@ -925,7 +956,7 @@ gemm_chain_resident_kernel(const __grid_constant__ ResChainMaps maps, const ResC
         uint32_t n_in = 0;
         for (int ti = 0; ti < n_ti; ++ti)
             for (int c = 0; c < g.n_chains; ++c) {
-                const int row0 = tile_row(ti, c);
+                const int row0 = tiles.row(ti, c);
                 if (row0 < 0) continue;
                 if (pairs) {
                     // the input tile: relu(u[b] + v[j]) s split into planes, this warp's 16 rows; lane = (row l / 4 + 8 h, 8 columns l % 4 of
@@ -948,14 +979,7 @@ gemm_chain_resident_kernel(const __grid_constant__ ResChainMaps maps, const ResC
                                 const float4* vp = reinterpret_cast<const float4*>(v + (size_t)j * BN + col);
                                 const float4 u0 = __ldg(up), u1 = __ldg(up + 1), v0 = __ldg(vp), v1 = __ldg(vp + 1);
                                 const float x[8] = {u0.x + v0.x, u0.y + v0.y, u0.z + v0.z, u0.w + v0.w, u1.x + v1.x, u1.y + v1.y, u1.z + v1.z, u1.w + v1.w};
-#pragma unroll
-                                for (int t = 0; t < 4; ++t) {
-                                    uint32_t w[P];
-                                    const float r0 = x[2 * t] < 0.f ? 0.f : x[2 * t], r1 = x[2 * t + 1] < 0.f ? 0.f : x[2 * t + 1];  // NaN-propagating ReLU
-                                    F::split2(r0 * s_act, r1 * s_act, w, amax);
-#pragma unroll
-                                    for (int p = 0; p < P; ++p) o[p][t] = w[p];
-                                }
+                                pair_split8<MORL_FMT_F16X2>(x, true, s_act, o, amax);
                             } else {
 #pragma unroll
                                 for (int t = 0; t < 4; ++t)
@@ -983,7 +1007,7 @@ gemm_chain_resident_kernel(const __grid_constant__ ResChainMaps maps, const ResC
                     const long long c1 = g.stats ? clock64() : 0;
                     EpiArgs e;
                     e.M = g.M; e.N = BN;
-                    e.k_acc = s_act / (s_act * ld_scale(g.b_scale[job]));  // as gemm_chain_kernel's folded epilogue
+                    e.k_acc = s_act / (s_act * ld_scale(g.b_scale[job]));  // as gemm_planes_kernel's folded epilogue
                     e.c_mul = 1.0f;
                     e.bias_s = s.bias; e.relu = g.relu; e.bits_in = g.bits_in[job]; e.bits_out = g.bits_out[job]; e.bits_ld = relu_bits_words(BN);
                     e.mask = nullptr; e.ld_mask = 0; e.c_f32 = nullptr; e.ldc = 0; e.planes = 1; e.ldp = BN;
@@ -1002,19 +1026,9 @@ gemm_chain_resident_kernel(const __grid_constant__ ResChainMaps maps, const ResC
                         float x[2][8];
                         epilogue_values<false>(a, 32 * cc, rbase, lane, e, x);
                         if (to_tile) {
-                            // output chunk cc = K-block cc of the next layer, the swizzled layout of a TMA box [P][128][32]
-#pragma unroll
-                            for (int h = 0; h < 2; ++h) {
-                                const int rl = lr + 8 * h;
-#pragma unroll
-                                for (int q = 0; q < 4; ++q) {
-                                    uint32_t w[P];
-                                    F::split2(x[h][2 * q], x[h][2 * q + 1], w, amax);
-                                    uint8_t* st = res_chunk(act, cc, trow + rl, q) + 4 * l4;
-#pragma unroll
-                                    for (int p = 0; p < P; ++p) *reinterpret_cast<uint32_t*>(st + p * R::kPlaneKB) = w[p];
-                                }
-                            }
+                            // output chunk cc = K-block cc of the next layer, the swizzled layout of a TMA box [P][128][32] (trow % 16 == 0: the
+                            // swizzle of the warp's rows is that of a 16-row staging tile)
+                            stage_chunk_planes<MORL_FMT_F16X2>(x, act + cc * R::kKBlock + trow * R::kRowB, R::kPlaneKB, lane, amax);
                             if (store) {
                                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
                                 __syncwarp();
@@ -1700,20 +1714,7 @@ __global__ void __launch_bounds__(256) pairs_relu_split_kernel(const float* __re
             x[4] = u1.x + v1.x; x[5] = u1.y + v1.y; x[6] = u1.z + v1.z; x[7] = u1.w + v1.w;
         }
         uint32_t o[F::P][4];
-        uint32_t pos = 0;  // bit t = (column 8 h8 + t is positive)
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            uint32_t w[F::P];
-            float r0 = x[2 * q], r1 = x[2 * q + 1];
-            if constexpr (!PRODUCT) {
-                r0 = r0 < 0.f ? 0.f : r0;  // NaN-propagating ReLU
-                r1 = r1 < 0.f ? 0.f : r1;
-            }
-            pos |= (r0 > 0.f ? 1u : 0u) << (2 * q) | (r1 > 0.f ? 1u : 0u) << (2 * q + 1);
-            F::split2(r0 * s, r1 * s, w, amax);
-#pragma unroll
-            for (int p = 0; p < F::P; ++p) o[p][q] = w[p];
-        }
+        const uint32_t pos = pair_split8<FMT>(x, !PRODUCT, s, o, amax);  // bit t = (column 8 h8 + t is positive)
         if (ok) {
             const long long off = row * H + 8 * h8;
 #pragma unroll
@@ -1766,16 +1767,7 @@ __global__ void __launch_bounds__(256) pairs_relu_split_h256_kernel(const float*
             const float x[8] = {uu[0] + va[q].x, uu[1] + va[q].y, uu[2] + va[q].z, uu[3] + va[q].w,
                                 uu[4] + vb[q].x, uu[5] + vb[q].y, uu[6] + vb[q].z, uu[7] + vb[q].w};
             uint32_t o[F::P][4];
-            uint32_t pos = 0;
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {
-                uint32_t w[F::P];
-                const float r0 = x[2 * t] < 0.f ? 0.f : x[2 * t], r1 = x[2 * t + 1] < 0.f ? 0.f : x[2 * t + 1];  // NaN-propagating ReLU
-                pos |= (r0 > 0.f ? 1u : 0u) << (2 * t) | (r1 > 0.f ? 1u : 0u) << (2 * t + 1);
-                F::split2(r0 * s, r1 * s, w, amax);
-#pragma unroll
-                for (int p = 0; p < F::P; ++p) o[p][t] = w[p];
-            }
+            const uint32_t pos = pair_split8<FMT>(x, true, s, o, amax);
             const long long row = (long long)b * W + jb + q;
             const long long off = row * H + 8 * lane;
 #pragma unroll
@@ -2244,34 +2236,29 @@ extern "C" int morl_philox_advance(unsigned int* offset, unsigned int inc, void*
 
 
 namespace morl {
-// Launch of gemm_chain_resident_kernel.  g: k_first, store and (pair mode) u / v / W set by the caller; in[c]: planes-mode input of chain c
-// (nullptr in pair mode); acts[c (n_layers + 1) + l + 1]: output of job (c, l), needed when its store bit is set.
-static int launch_chain_resident(ResChainArgs& g, int n_chains, int n_layers, const void* const* in, const void* const* acts, long long act_plane_stride,
-                                 const float* act_scale, const void* const* w_planes, long long w_plane_stride, const float* const* w_scales,
-                                 const float* const* biases, int relu, const void* const* relu_bits_in, void* const* relu_bits_out, int M, int K,
-                                 const char* name, void* stream) {
-    constexpr int fmt = MORL_FMT_F16X2;
-    ResChainMaps maps;
-    memset(&maps, 0, sizeof(maps));
-    g.M = M; g.K = K; g.n_chains = n_chains; g.n_layers = n_layers; g.a_scale = act_scale; g.relu = relu ? 1 : 0;
-    for (int c = 0; c < n_chains; ++c) {
-        if (!g.u[0]) {
-            MORL_REQUIRE(in[c] && aligned16(in[c]), MORL_ERR_NULL, "%s: NULL or misaligned input planes (chain %d)", name, c);
-            // [P][M][k_first] (plane stride M * k_first), box P x 128 rows x 32
-            const int rc = make_plane_map(&maps.A[c], fmt, in[c], M, g.k_first, (long long)M * g.k_first, kGemmBM, ResPlan::BK);
-            MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "%s: cuTensorMapEncodeTiled(A) failed (%d)", name, rc);
-        }
+// The ChainArgs of a chain launch, and the weight and output tensor maps of its jobs.  Job (c, l) = layer l of chain c reads the weight
+// planes w_planes[job] ([P][256][K]; layer 0: [P][256][k_first]) and, when bit job of `store` is set, writes its output to
+// acts[c (n_layers + 1) + l + 1] ([P][M][256]).  f16x2 runs on gemm_chain_resident_kernel (weight boxes of 256 rows, output boxes of one
+// plane), bf16x3 on gemm_chain_kernel (weight boxes of 32 rows, output boxes of all planes).
+static int set_chain_args(ChainArgs& g, CUtensorMap* B, CUtensorMap* C, int fmt, int n_chains, int n_layers, int M, int K, int k_first,
+                          const void* const* acts, long long act_plane_stride, const float* act_scale, uint32_t store, const void* const* w_planes,
+                          long long w_plane_stride, const float* const* w_scales, const float* const* biases, int relu,
+                          const void* const* relu_bits_in, void* const* relu_bits_out, const char* name) {
+    const bool resident = fmt == MORL_FMT_F16X2;
+    const int BK = resident ? ResPlan::BK : fmt_bk(fmt);
+    g.M = M; g.K = K; g.k_first = k_first; g.n_chains = n_chains; g.n_layers = n_layers; g.a_scale = act_scale; g.relu = relu ? 1 : 0;
+    for (int c = 0; c < n_chains; ++c)
         for (int l = 0; l < n_layers; ++l) {
             const int job = c * n_layers + l;
-            const int kj = l == 0 ? g.k_first : K;
-            const long long w_stride = l == 0 ? (long long)256 * g.k_first : w_plane_stride;
+            const int kj = l == 0 ? k_first : K;
+            const long long w_stride = l == 0 ? (long long)256 * k_first : w_plane_stride;
             MORL_REQUIRE(w_planes[job] && aligned16(w_planes[job]), MORL_ERR_NULL, "%s: NULL or misaligned weight planes (chain %d, layer %d)", name, c, l);
-            int rc = make_plane_map(&maps.B[job], fmt, w_planes[job], 256, kj, w_stride, 256, ResPlan::BK, true);
+            int rc = make_plane_map(&B[job], fmt, w_planes[job], 256, kj, w_stride, resident ? 256 : kGemmBoxN, BK, true);
             MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "%s: cuTensorMapEncodeTiled(B) failed (%d)", name, rc);
-            if ((g.store >> job) & 1u) {
+            if ((store >> job) & 1u) {
                 const void* out = acts[c * (n_layers + 1) + l + 1];
                 MORL_REQUIRE(out && aligned16(out), MORL_ERR_NULL, "%s: NULL or misaligned output planes (chain %d, layer %d)", name, c, l);
-                rc = make_plane_map(&maps.C[job], fmt, out, M, 256, act_plane_stride, 16, 32, true);
+                rc = make_plane_map(&C[job], fmt, out, M, 256, act_plane_stride, 16, 32, resident);
                 MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "%s: cuTensorMapEncodeTiled(C) failed (%d)", name, rc);
             }
             g.bias[job] = biases ? biases[job] : nullptr;
@@ -2280,6 +2267,26 @@ static int launch_chain_resident(ResChainArgs& g, int n_chains, int n_layers, co
             g.bits_in[job] = relu_bits_in ? static_cast<const uint32_t*>(relu_bits_in[job]) : nullptr;
             MORL_REQUIRE(aligned16(g.bits_out[job]) && aligned16(g.bits_in[job]), MORL_ERR_ALIGN, "%s: ReLU bit masks must be 16-byte aligned", name);
         }
+    return MORL_OK;
+}
+
+// Launch of gemm_chain_resident_kernel.  g: store and (pair mode) u / v / W set by the caller; in[c]: planes-mode input of chain c
+// ([P][M][k_first], nullptr in pair mode); acts: as set_chain_args.
+static int launch_chain_resident(ResChainArgs& g, int n_chains, int n_layers, int k_first, const void* const* in, const void* const* acts,
+                                 long long act_plane_stride, const float* act_scale, const void* const* w_planes, long long w_plane_stride,
+                                 const float* const* w_scales, const float* const* biases, int relu, const void* const* relu_bits_in,
+                                 void* const* relu_bits_out, int M, int K, const char* name, void* stream) {
+    constexpr int fmt = MORL_FMT_F16X2;
+    ResChainMaps maps;
+    memset(&maps, 0, sizeof(maps));
+    const int rc = set_chain_args(g, maps.B, maps.C, fmt, n_chains, n_layers, M, K, k_first, acts, act_plane_stride, act_scale, g.store, w_planes,
+                                  w_plane_stride, w_scales, biases, relu, relu_bits_in, relu_bits_out, name);
+    if (rc) return rc;
+    for (int c = 0; c < n_chains && !g.u[0]; ++c) {
+        MORL_REQUIRE(in[c] && aligned16(in[c]), MORL_ERR_NULL, "%s: NULL or misaligned input planes (chain %d)", name, c);
+        // [P][M][k_first] (plane stride M * k_first), box P x 128 rows x 32
+        const int rca = make_plane_map(&maps.A[c], fmt, in[c], M, k_first, (long long)M * k_first, kGemmBM, ResPlan::BK);
+        MORL_REQUIRE(rca == 0, MORL_ERR_NO_DEVICE, "%s: cuTensorMapEncodeTiled(A) failed (%d)", name, rca);
     }
     static const bool want_stats = [] { const char* e = getenv("MORL_GEMM_STATS"); return e && e[0] == '1'; }();
     if (want_stats) {
@@ -2304,7 +2311,7 @@ extern "C" int morl_gemm_chain_supported(int fmt, int M, int K) {
 
 // Several 256-wide hidden layers (Linear + ReLU, planes in / planes out) of one or two networks in ONE persistent launch: job (c, l) computes
 // act[c][l+1] = relu(act[c][l] . W[c][l]^T + bias[c][l]) exactly as morl_gemm_planes_f32 does (bit-identical), but a CTA takes its row tiles
-// through all layers, so intermediate activations are re-read from L2 instead of HBM (csrc: gemm_chain_kernel).
+// through all layers (csrc: gemm_chain_resident_kernel for f16x2, gemm_chain_kernel for bf16x3).
 extern "C" int morl_gemm_chain_f32(int fmt, int n_chains, int n_layers, const void* const* act_planes, long long act_plane_stride, const float* act_scale,
                                    const void* const* w_planes, long long w_plane_stride, const float* const* w_scales, const float* const* biases,
                                    int relu, const void* const* relu_bits_in, void* const* relu_bits_out, int M, int K, int k_first, void* stream) {
@@ -2318,53 +2325,38 @@ extern "C" int morl_gemm_chain_f32(int fmt, int n_chains, int n_layers, const vo
     const int BK = fmt == MORL_FMT_F16X2 ? ResPlan::BK : fmt_bk(fmt);
     if (k_first <= 0) k_first = K;
     MORL_REQUIRE(k_first % BK == 0 && k_first <= K, MORL_ERR_SHAPE, "morl_gemm_chain_f32: k_first=%d must be a multiple of %d and <= K", k_first, BK);
+    const uint32_t every_output = (1u << (n_chains * n_layers)) - 1u;
     if (fmt == MORL_FMT_F16X2) {
         ResChainArgs g;
         memset(&g, 0, sizeof(g));
-        g.k_first = k_first;
-        g.store = (1u << (n_chains * n_layers)) - 1u;  // every output
+        g.store = every_output;
         const void* in[2] = {nullptr, nullptr};
         for (int c = 0; c < n_chains; ++c) in[c] = act_planes[c * (n_layers + 1)];
-        return launch_chain_resident(g, n_chains, n_layers, in, act_planes, act_plane_stride, act_scale, w_planes, w_plane_stride, w_scales, biases,
-                                     relu, relu_bits_in, relu_bits_out, M, K, "morl_gemm_chain_f32", stream);
+        return launch_chain_resident(g, n_chains, n_layers, k_first, in, act_planes, act_plane_stride, act_scale, w_planes, w_plane_stride, w_scales,
+                                     biases, relu, relu_bits_in, relu_bits_out, M, K, "morl_gemm_chain_f32", stream);
     }
     ChainMaps maps;  // (host staging of the 3 x 8 tensor maps on this thread's stack -- the entry point stays re-entrant; copied into the kernel
                      // parameters by the launch)
     ChainArgs g;
     memset(&g, 0, sizeof(g));
-    g.M = M; g.K = K; g.k_first = k_first; g.n_chains = n_chains; g.n_layers = n_layers; g.a_scale = act_scale; g.relu = relu ? 1 : 0;
+    const int rc = set_chain_args(g, maps.B, maps.C, fmt, n_chains, n_layers, M, K, k_first, act_planes, act_plane_stride, act_scale, every_output,
+                                  w_planes, w_plane_stride, w_scales, biases, relu, relu_bits_in, relu_bits_out, "morl_gemm_chain_f32");
+    if (rc) return rc;
+    g.n_stages = KPlan<MORL_FMT_BF16X3>::kStages;
     for (int c = 0; c < n_chains; ++c)
         for (int l = 0; l < n_layers; ++l) {
-            const int job = c * n_layers + l;
+            // the input of job (c, l) is the output of job (c, l - 1); layer 0 may read a narrower input [P][M][k_first] (plane stride M k_first)
             const void* a_in = act_planes[c * (n_layers + 1) + l];
-            const void* a_out = act_planes[c * (n_layers + 1) + l + 1];
-            MORL_REQUIRE(a_in && a_out && w_planes[job] && aligned16(a_in) && aligned16(a_out) && aligned16(w_planes[job]), MORL_ERR_NULL,
-                         "morl_gemm_chain_f32: NULL or misaligned plane pointer (chain %d, layer %d)", c, l);
-            // layer 0 may read a narrower input [P][M][k_first] (plane stride M * k_first) through weights [P][256][k_first]
-            const int kj = l == 0 ? k_first : K;
-            const long long a_stride = l == 0 ? (long long)M * k_first : act_plane_stride;
-            const long long w_stride = l == 0 ? (long long)256 * k_first : w_plane_stride;
-            int rc = make_plane_map(&maps.A[job], fmt, a_in, M, kj, a_stride, kGemmBM, BK);
-            MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "morl_gemm_chain_f32: cuTensorMapEncodeTiled(A) failed (%d)", rc);
-            rc = make_plane_map(&maps.B[job], fmt, w_planes[job], 256, kj, w_stride, kGemmBoxN, BK, true);
-            MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "morl_gemm_chain_f32: cuTensorMapEncodeTiled(B) failed (%d)", rc);
-            rc = make_plane_map(&maps.C[job], fmt, a_out, M, 256, act_plane_stride, 16, 32);
-            MORL_REQUIRE(rc == 0, MORL_ERR_NO_DEVICE, "morl_gemm_chain_f32: cuTensorMapEncodeTiled(C) failed (%d)", rc);
-            g.bias[job] = biases ? biases[job] : nullptr;
-            g.b_scale[job] = w_scales ? w_scales[job] : nullptr;
-            g.bits_out[job] = relu_bits_out ? static_cast<uint32_t*>(relu_bits_out[job]) : nullptr;
-            g.bits_in[job] = relu_bits_in ? static_cast<const uint32_t*>(relu_bits_in[job]) : nullptr;
-            MORL_REQUIRE(aligned16(g.bits_out[job]) && aligned16(g.bits_in[job]), MORL_ERR_ALIGN, "morl_gemm_chain_f32: ReLU bit masks must be 16-byte aligned");
+            MORL_REQUIRE(a_in && aligned16(a_in), MORL_ERR_NULL, "morl_gemm_chain_f32: NULL or misaligned input planes (chain %d, layer %d)", c, l);
+            const int rca = make_plane_map(&maps.A[c * n_layers + l], fmt, a_in, M, l == 0 ? k_first : K, l == 0 ? (long long)M * k_first : act_plane_stride,
+                                           kGemmBM, BK);
+            MORL_REQUIRE(rca == 0, MORL_ERR_NO_DEVICE, "morl_gemm_chain_f32: cuTensorMapEncodeTiled(A) failed (%d)", rca);
         }
     const int sms = sm_count();
     const int n_tiles = (M + kGemmBM - 1) / kGemmBM;
-    MORL_DISPATCH_FMT(fmt, {
-        constexpr size_t smem = KPlan<kFmt>::kBytes;
-        g.n_stages = KPlan<kFmt>::kStages;
-        set_smem_limit_once<gemm_chain_kernel<kFmt>>(smem);
-        launch_k_pdl(true, gemm_chain_kernel<kFmt>, dim3(n_tiles < sms ? n_tiles : sms), dim3(kGemmThreads), smem,
-                     static_cast<cudaStream_t>(stream), maps, g);
-    });
+    constexpr size_t smem = KPlan<MORL_FMT_BF16X3>::kBytes;
+    set_smem_limit_once<gemm_chain_kernel>(smem);
+    launch_k_pdl(true, gemm_chain_kernel, dim3(n_tiles < sms ? n_tiles : sms), dim3(kGemmThreads), smem, static_cast<cudaStream_t>(stream), maps, g);
     return check_launch("morl_gemm_chain_f32");
 }
 
@@ -2387,7 +2379,6 @@ extern "C" int morl_gemm_chain_pairs_f32(int n_chains, int n_layers, const float
     MORL_REQUIRE(store_mask == 0 || acts, MORL_ERR_NULL, "morl_gemm_chain_pairs_f32: stored outputs need their planes");
     ResChainArgs g;
     memset(&g, 0, sizeof(g));
-    g.k_first = 256;
     g.store = store_mask;
     g.W = W;
     const void* outs[2 * (kChainMaxJobs + 1)] = {};
@@ -2397,6 +2388,6 @@ extern "C" int morl_gemm_chain_pairs_f32(int n_chains, int n_layers, const float
         g.v[c] = v[c];
         for (int l = 0; l < n_layers; ++l) outs[c * (n_layers + 1) + l + 1] = acts ? acts[c * n_layers + l] : nullptr;
     }
-    return launch_chain_resident(g, n_chains, n_layers, nullptr, outs, act_plane_stride, act_scale, w_planes, w_plane_stride, w_scales, biases, 1, nullptr,
+    return launch_chain_resident(g, n_chains, n_layers, 256, nullptr, outs, act_plane_stride, act_scale, w_planes, w_plane_stride, w_scales, biases, 1, nullptr,
                                  relu_bits_out, B * W, 256, "morl_gemm_chain_pairs_f32", stream);
 }

@@ -5,20 +5,19 @@ CTA in layer order, and that the per-chain rotation balances the two-chain launc
 
 import itertools
 
+from tests.chain_tiles import chain_tiles
+
 
 def schedule(n_tiles, n_sms, n_chains, n_layers):
     """[(cta, [(chain, tile, layer), ...])] exactly as gemm_chain_resident_kernel enumerates them."""
     n_units = min(n_tiles, n_sms)
     out = []
     for unit in range(n_units):
-        cu = [unit, (unit + n_units // 2) % n_units]
-        mt = [(n_tiles - c + n_units - 1) // n_units if c < n_tiles else 0 for c in cu]
-        if n_chains == 1:
-            mt[1] = 0
+        tiles = chain_tiles(n_tiles, n_units, n_chains, unit)
         seq = []
-        for ti, c in itertools.product(range(max(mt)), range(n_chains)):
-            if ti < mt[c]:
-                seq += [(c, cu[c] + ti * n_units, l) for l in range(n_layers)]
+        for ti, c in itertools.product(range(max(map(len, tiles))), range(n_chains)):
+            if ti < len(tiles[c]):
+                seq += [(c, tiles[c][ti], l) for l in range(n_layers)]
         out.append((unit, seq))
     return out
 

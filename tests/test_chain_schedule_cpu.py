@@ -10,6 +10,8 @@ section 4.6 claims:
 
 import itertools
 
+from tests.chain_tiles import chain_tiles
+
 LANES = 4
 
 
@@ -19,16 +21,13 @@ def schedule(n_tiles, n_pairs, n_chains, n_layers, rotate=True):
     tpg = LANES // n_chains
     out = []
     for unit in range(n_units):
-        cu = [unit, (unit + n_units // 2) % n_units if rotate else unit]
-        mt = [(n_tiles - c + n_units - 1) // n_units if c < n_tiles else 0 for c in cu]
-        if n_chains == 1:
-            mt[1] = 0
-        n_groups = (max(mt) + tpg - 1) // tpg
+        tiles = chain_tiles(n_tiles, n_units, n_chains, unit, rotate)
+        n_groups = (max(map(len, tiles)) + tpg - 1) // tpg
         seq = []
         for gi, l, ln in itertools.product(range(n_groups), range(n_layers), range(LANES)):
             c, ti = ln % n_chains, gi * tpg + ln // n_chains
-            if ti < mt[c]:
-                seq.append((c, cu[c] + ti * n_units, l, ln))
+            if ti < len(tiles[c]):
+                seq.append((c, tiles[c][ti], l, ln))
         out.append((unit, seq))
     return out
 
