@@ -56,7 +56,7 @@
 extern "C" {
 #endif
 
-#define MORL_B200_VERSION 100 /* 0.1.0 */
+#define MORL_B200_VERSION 200 /* 0.2.0 */
 
 #if defined(__GNUC__)
 #define MORL_API __attribute__((visibility("default")))
@@ -334,9 +334,8 @@ MORL_API int morl_per_priority_f32(const float* raw, int n, float alpha, double*
  *                     K % 64 == 0 (f16x2) / K % 32 == 0 (bf16x3), N_pad % 32 == 0, N_pad <= 512 (wider than 256: two column units
  *                     [0, 256) and [256, N_pad) of a row tile, each bit-identical to a launch over that half).  The accumulator is multiplied by
  *                     1 / (a_scale * b_scale) before the bias.  Outputs: c_f32 [M, ldc] and/or c_planes [P][M][ldp] holding
- *                     c_scale * C (the operand format of the next layer).  relu != 0 applies max(x, 0); relu_mask_plane0 (plane 0 of
- *                     a forward activation, [M][ld_mask] 16-bit) zeroes the outputs where that activation was <= 0 (ReLU backward).
- *                     ReLU bit masks (the form the update uses; relu_mask_plane0 stays for callers that only hold planes):
+ *                     c_scale * C (the operand format of the next layer).  relu != 0 applies max(x, 0).
+ *                     ReLU bit masks (the only form of the ReLU-backward mask):
  *                     relu_bits_out [M][8] uint32 (N_pad <= 256) receives bit j of word (c & 1) * 4 + (c >> 1) = (C[m, 32 c + j] > 0) -- 32
  *                     bytes per row instead of the 512-byte activation row, words ordered so that the four chunks one epilogue thread
  *                     owns are one 16-byte load.  N_pad > 256: [M][16] words (the row pitch follows N_pad, not N: every 32-column
@@ -370,9 +369,8 @@ MORL_API int morl_split_planes(int fmt, const float* src, int rows, int cols, in
                                int ldp, long long plane_stride, const float* scale, void* stream);
 MORL_API int morl_gemm_planes_f32(int fmt, const void* a_planes, long long a_plane_stride, const float* a_scale, const void* b_planes,
                                   long long b_plane_stride, const float* b_scale, int M, int N, int N_pad, int K, const float* bias,
-                                  int relu, const void* relu_mask_plane0, int ld_mask, float* c_f32, int ldc, void* c_planes, int ldp,
-                                  long long c_plane_stride, const float* c_scale, int reverse_tiles, int split_accumulators,
-                                  const void* relu_bits_in, void* relu_bits_out, void* stream);
+                                  int relu, float* c_f32, int ldc, void* c_planes, int ldp, long long c_plane_stride, const float* c_scale,
+                                  int reverse_tiles, int split_accumulators, const void* relu_bits_in, void* relu_bits_out, void* stream);
 /* Hidden layer Linear -> Dropout(p) -> LayerNorm -> ReLU of GPI-PD's Q-network (reference gpi_pd.py:41-76, networks.py:10-48) as ONE
  * K-major GEMM whose epilogue computes, per output row,  y = relu(LN(dropout(A . B^T / (a_scale b_scale) + bias)))  (csrc/gemm_planes.cu,
  * gemm_planes_kernel<FMT, 0, kEpiLn>).  Operands, scales, reverse_tiles, c_f32 / c_planes as in morl_gemm_planes_f32 with N_pad = N; the
@@ -501,10 +499,6 @@ MORL_API size_t morl_gemm_mn_workspace_bytes(int M, int a_cols, int b_cols);
 MORL_API int morl_gemm_planes_mn_f32(int fmt, const void* g_planes, long long g_plane_stride, int ldg, int g_cols, const float* g_scale,
                                      const void* h_planes, long long h_plane_stride, int ldh, int h_cols, const float* h_scale, int M,
                                      int transpose_out, float* out, int ld_out, float* colsum_out, void* workspace, void* stream);
-/* out[n] = (1 / *scale) sum_m sum_p planes[p][m][n]  (bias gradients); workspace: morl_colsum_workspace_bytes(N) bytes */
-MORL_API size_t morl_colsum_workspace_bytes(int N);
-MORL_API int morl_colsum_planes(int fmt, const void* planes, long long plane_stride, const float* scale, int M, int ld, int N, float* out,
-                                void* workspace, void* stream);
 /* gradients of the separable first layer: dU[b,:] = sum_j G[b*W+j,:], dV[j,:] = sum_b G[b*W+j,:]  (G planes [P][B*W][H] scaled by
  * *scale, W <= 64 for the one-pass kernel); workspace: morl_pairs_grad_reduce_workspace_bytes(B, W, H) bytes */
 MORL_API size_t morl_pairs_grad_reduce_workspace_bytes(int B, int W, int H);

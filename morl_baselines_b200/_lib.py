@@ -9,9 +9,11 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import re
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "csrc", "libmorl_b200.so")
+HEADER = os.path.join(os.path.dirname(HERE), "include", "morl_b200.h")
 
 # constants of include/morl_b200.h
 DOT_UNFUSED, DOT_FMA, DOT_PAIRFMA = 0, 1, 2
@@ -22,88 +24,34 @@ MAX_D = 8
 PCN_MAX_BATCH = 4096
 FMT_BF16X3, FMT_F16X2 = 0, 1
 
-_vp, _i, _f, _d, _i64, _sz = C.c_void_p, C.c_int, C.c_float, C.c_double, C.c_int64, C.c_size_t
+_vp, _i = C.c_void_p, C.c_int
 
-# name -> (restype, argtypes); mirrors include/morl_b200.h one to one (checked by tests/test_abi.py)
-SIGNATURES = {
-    "morl_version": (_i, []),
-    "morl_last_error": (C.c_char_p, []),
-    "morl_device_sm_count": (_i, []),
-    "morl_envelope_td_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    "morl_greedy_td_f32": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _f, _i, _i, _i, _i, _vp, _vp, _vp]),
-    "morl_critic_min_td_f32": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _i, _f, _i, _i, _i, _i, _vp, _vp, _vp]),
-    "morl_gpi_envelope_f32": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _i, _f, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    "morl_actor_critic_td_f32": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _f, _f, _i, _i, _i, _vp, _vp]),
-    "morl_td_workspace_bytes": (_sz, [_i]),
-    "morl_td_mse_priority_f32": (_i, [_vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "morl_td_huber_priority_f32": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp, _i, _i, _f, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
-    "morl_discrete_sac_target_f32": (_i, [_vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _f, _i, _i, _i, _vp, _vp]),
-    "morl_discrete_sac_workspace_bytes": (_sz, [_i]),
-    "morl_discrete_sac_actor_loss_f32": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _vp, _f, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "morl_host_sumtree_walk": (_i, [_vp, _i, _vp, _i, _vp]),
-    "morl_host_sumtree_batch_set": (_i, [_vp, _i, _vp, _vp, _i]),
-    "morl_host_gather_rows": (_i, [_vp, C.c_longlong, _vp, _i, _vp]),
-    "morl_host_gather_u8_to_i32": (_i, [_vp, C.c_longlong, _vp, _i, _vp]),
-    "morl_sumtree_walk_f64": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp]),
-    "morl_sumtree_batch_set_f64": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp]),
-    "morl_sumtree_set_f64": (_i, [_vp, _i, C.c_longlong, _d, _i, _vp, _vp, _vp]),
-    "morl_per_priority_f32": (_i, [_vp, _i, _f, _vp, _vp, _vp, _vp]),
-    "morl_replay_gather": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "morl_pareto_mask_f32": (_i, [_vp, _i, _i, _i, _vp, _vp]),
-    "morl_pareto_mask_f64": (_i, [_vp, _i, _i, _i, _vp, _vp]),
-    "morl_front_pack_f64": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp]),
-    "morl_front_unpack_f64": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp]),
-    "morl_hypervolume_f64": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
-    "morl_corner_weights_f64": (_i, [_vp, _i, _i, _vp, _i, _vp, _vp]),
-    "morl_polyak_f32": (_i, [_vp, _vp, _vp, _i, _i64, _d, _vp]),
-    "morl_plane_overflow_count": (_i, [_i]),
-    "morl_amax_scale_f32": (_i, [_vp, C.c_longlong, _i, _vp, _vp, _vp]),
-    "morl_split_planes_multi": (_i, [_i, _vp, _i, _vp]),
-    "morl_split_planes": (_i, [_i, _vp, _i, _i, _i, _i, _vp, _i, _i, C.c_longlong, _vp, _vp]),
-    "morl_gemm_planes_f32": (_i, [_i, _vp, C.c_longlong, _vp, _vp, C.c_longlong, _vp, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _i, C.c_longlong,
-                                  _vp, _i, _i, _vp, _vp, _vp]),
-    "morl_gemm_planes_ln_f32": (_i, [_i, _vp, C.c_longlong, _vp, _vp, C.c_longlong, _vp, _i, _i, _i, _vp, _i, _vp, _vp, _f, _f, _vp, _vp, C.c_uint,
-                                     _vp, _i, _vp, _i, C.c_longlong, _vp, _i, _vp, _vp]),
-    "morl_philox_advance": (_i, [_vp, C.c_uint, _vp]),
-    "morl_gemm_chain_supported": (_i, [_i, _i, _i]),
-    "morl_gemm_chain_f32": (_i, [_i, _i, _i, _vp, C.c_longlong, _vp, _vp, C.c_longlong, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp]),
-    "morl_gemm_chain_pairs_f32": (_i, [_i, _i, _vp, _vp, _i, _i, _vp, C.c_longlong, _vp, _vp, C.c_longlong, _vp, _vp, _vp, C.c_uint, _vp]),
-    "morl_debug_gemm_stats": (_i, [_vp, _i]),
-    "morl_ensemble_sample_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    "morl_dyna_commit_workspace_bytes": (_sz, [_i]),
-    "morl_dyna_commit_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
-    "morl_qhead_envelope_supported": (_i, [_i, _i, _i, _i, _i, _i]),
-    "morl_qhead_gemm_supported": (_i, [_i, _i, _i, _i]),
-    "morl_qhead_gemm_f32": (_i, [_i, _vp, C.c_longlong, _vp, _vp, C.c_longlong, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
-    "morl_qhead_envelope_td_f32": (_i, [_i, _vp, _vp, C.c_longlong, _vp, _vp, _vp, _vp, C.c_longlong, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _f, _i, _i,
-                                        _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "morl_pairs_relu_split_planes": (_i, [_i, _vp, _vp, _i, _i, _i, _vp, C.c_longlong, _vp, _vp, _vp]),
-    "morl_pairs_product_split_planes": (_i, [_i, _vp, _vp, _i, _i, _i, _vp, C.c_longlong, _vp, _vp]),
-    "morl_gemm_mn_workspace_bytes": (_sz, [_i, _i, _i]),
-    "morl_gemm_planes_mn_f32": (_i, [_i, _vp, C.c_longlong, _i, _i, _vp, _vp, C.c_longlong, _i, _i, _vp, _i, _i, _vp, _i, _vp, _vp, _vp]),
-    "morl_colsum_workspace_bytes": (_sz, [_i]),
-    "morl_colsum_planes": (_i, [_i, _vp, C.c_longlong, _vp, _i, _i, _i, _vp, _vp, _vp]),
-    "morl_pairs_grad_reduce_workspace_bytes": (_sz, [_i, _i, _i]),
-    "morl_pairs_grad_reduce_planes": (_i, [_i, _vp, C.c_longlong, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    "morl_pair_layer1_uv_f32": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
-    "morl_product_layer1_uv_f32": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
-    "morl_pair_layer1_grad_workspace_bytes": (_sz, [_i, _i, _i]),
-    "morl_pair_layer1_grad_f32": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    "morl_adam_workspace_bytes": (_sz, [_i, _i64]),
-    "morl_adam_clip_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i64, _f, _f, _f, _f, _f, _vp, _vp]),
-    "morl_adam_clip_lr_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i64, _f, _vp, _f, _f, _f, _vp, _vp]),
-    "morl_vector_gae_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _d, _d, _i, _vp, _vp, _vp]),
-    "morl_ppo_loss_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _f, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "morl_pcn_supported": (_i, [_i, _i, _i, _i, _i]),
-    "morl_pcn_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
-    "morl_pcn_update_f32": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
-    "morl_pcn_forward_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
-    "morl_eupg_supported": (_i, [_i, _i, _vp, _i, _i]),
-    "morl_eupg_workspace_bytes": (_sz, [_i, _i, _vp, _i, _i]),
-    "morl_eupg_returns_f32": (_i, [_vp, _i, _i, _i, _f, _vp, _vp]),
-    "morl_eupg_update_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp]),
-    "morl_eupg_probs_f32": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _i, _vp, _vp]),
-}
+# value types of include/morl_b200.h and their ctypes equivalents (every pointer is passed as c_void_p)
+_SCALARS = {"int": _i, "float": C.c_float, "double": C.c_double, "long long": C.c_longlong, "int64_t": C.c_int64, "unsigned int": C.c_uint,
+            "size_t": C.c_size_t}
+_DECL = re.compile(r"MORL_API\s+([\w\s\*]+?)\s*\b(morl_\w+)\s*\(([^;]*?)\)\s*;", flags=re.S)
+
+
+def _ctype(decl: str, where: str, ret: bool = False):
+    words = decl.replace("*", " * ").split()
+    if "*" in words:
+        return C.c_char_p if ret and words == ["const", "char", "*"] else _vp
+    t = " ".join(words if ret else words[:-1])  # a parameter ends with its name
+    if t not in _SCALARS:
+        raise MorlB200Error(f"{where}: no ctypes mapping for the C type '{t}' (include/morl_b200.h)")
+    return _SCALARS[t]
+
+
+def signatures(header: str) -> dict:
+    """name -> (restype, argtypes) of every MORL_API declaration in the text of include/morl_b200.h."""
+    src = re.sub(r"/\*.*?\*/|//[^\n]*", "", header, flags=re.S)
+    sigs = {}
+    for m in _DECL.finditer(src):
+        ret, name, params = m.group(1), m.group(2), m.group(3).strip()
+        params = [] if params in ("", "void") else [p for p in params.split(",") if p.strip()]
+        sigs[name] = (_ctype(ret, name, ret=True), [_ctype(p, f"{name}({p.strip()})") for p in params])
+    return sigs
+
 
 SPLIT_MAX_JOBS = 16
 
@@ -132,8 +80,10 @@ def load():
             f"{LIB_PATH} not found: build it with `python -m morl_baselines_b200.csrc.build` (nvcc, sm_90a). "
             "morl_baselines_b200 has no CPU / eager fallback for its CUDA operators."
         )
+    with open(HEADER) as f:
+        sigs = signatures(f.read())
     lib = C.CDLL(LIB_PATH)
-    for name, (res, args) in SIGNATURES.items():
+    for name, (res, args) in sigs.items():
         fn = getattr(lib, name)  # AttributeError here == ABI drift between header and library
         fn.restype = res
         fn.argtypes = args

@@ -72,8 +72,6 @@ struct GemmArgs {
     void* c_planes;              // [P][M][ldp] or nullptr (re-split output: operand of the next layer)
     int ldp;                     // columns of a plane row (>= N, multiple of 32; columns [N, ldp) are written as zero)
     long long plane_stride;      // elements between planes
-    const uint16_t* mask;        // plane 0 of the forward activation [M][ld_mask] for the ReLU-backward mask, or nullptr
-    int ld_mask;
     const uint32_t* bits_in;     // ReLU-backward mask as BITS [M][relu_bits_words(N_pad)] words (see morl_b200.h "ReLU bit masks"), or nullptr
     uint32_t* bits_out;          // forward: bit = (output > 0) per column, same layout, or nullptr
     int bits_ld;                 // words per row of bits_in / bits_out: relu_bits_words(N_pad) (the epilogue visits every chunk below N_pad)
@@ -242,8 +240,6 @@ struct EpiArgs {
     const uint32_t* bits_in;
     uint32_t* bits_out;
     int bits_ld;                 // words per bit-mask row (relu_bits_words)
-    const uint16_t* mask;
-    int ld_mask;
     float* c_f32;
     int ldc;
     int planes;                  // re-split the output into planes through tmC
@@ -325,21 +321,6 @@ __device__ __forceinline__ void epilogue_chunk(const float (&a)[16], int col0, i
     const int l4 = lane & 3, lr = lane >> 2;
     float x[2][8];
     epilogue_values<PRE>(a, col0, rbase, lane, e, x);
-    if (e.mask) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int row = rbase + lr + 8 * h;
-            if (row < e.M) {
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const uint32_t mm = __ldg(reinterpret_cast<const uint32_t*>(e.mask + (size_t)row * e.ld_mask + col0 + 8 * q + 2 * l4));
-                    // (bf16 or fp16) > 0  <=>  sign bit clear and magnitude non-zero (NaN never occurs in a ReLU output)
-                    if ((mm & 0x8000u) || (mm & 0x7FFFu) == 0u) x[h][2 * q] = 0.f;
-                    if ((mm & 0x80000000u) || (mm & 0x7FFF0000u) == 0u) x[h][2 * q + 1] = 0.f;
-                }
-            }
-        }
-    }
     if (e.c_f32) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -581,8 +562,8 @@ gemm_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         e.M = g.M; e.N = g.N;
         e.k_acc = fold / (ld_scale(g.a_scale) * ld_scale(g.b_scale));
         e.c_mul = folded ? 1.0f : c_mul;
-        e.bias_s = s.bias; e.relu = g.relu; e.bits_in = g.bits_in; e.bits_out = g.bits_out; e.bits_ld = g.bits_ld; e.mask = g.mask;
-        e.ld_mask = g.ld_mask; e.c_f32 = g.c_f32; e.ldc = g.ldc; e.planes = g.c_planes != nullptr; e.ldp = g.ldp;
+        e.bias_s = s.bias; e.relu = g.relu; e.bits_in = g.bits_in; e.bits_out = g.bits_out; e.bits_ld = g.bits_ld;
+        e.c_f32 = g.c_f32; e.ldc = g.ldc; e.planes = g.c_planes != nullptr; e.ldp = g.ldp;
         uint32_t key0 = 0, key1 = 0, ctr0 = 0;
         if constexpr (EPI == kEpiLn) {
             if (g.drop_seed) {
@@ -749,7 +730,6 @@ gemm_chain_kernel(const __grid_constant__ ChainMaps maps, const ChainArgs g) {
                     e.k_acc = s_act / (s_act * ld_scale(g.b_scale[job]));
                     e.c_mul = 1.0f;
                     e.bias_s = s.bias; e.relu = g.relu; e.bits_in = g.bits_in[job]; e.bits_out = g.bits_out[job]; e.bits_ld = relu_bits_words(BN);
-                    e.mask = nullptr; e.ld_mask = 0;
                     e.c_f32 = nullptr; e.ldc = 0; e.planes = 1; e.ldp = BN;
                     const int rbase = row0 + wg * 64 + (warp & 3) * 16;
                     consume_unit<FMT, 0, false>(acc, s, ring, l == 0 ? n_kblk_first : n_kblk_full, 0, BN, rbase, wg, lane, nullptr, [] {}, e,
@@ -1010,7 +990,7 @@ gemm_chain_resident_kernel(const __grid_constant__ ResChainMaps maps, const ResC
                     e.k_acc = s_act / (s_act * ld_scale(g.b_scale[job]));  // as gemm_planes_kernel's folded epilogue
                     e.c_mul = 1.0f;
                     e.bias_s = s.bias; e.relu = g.relu; e.bits_in = g.bits_in[job]; e.bits_out = g.bits_out[job]; e.bits_ld = relu_bits_words(BN);
-                    e.mask = nullptr; e.ld_mask = 0; e.c_f32 = nullptr; e.ldc = 0; e.planes = 1; e.ldp = BN;
+                    e.c_f32 = nullptr; e.ldc = 0; e.planes = 1; e.ldp = BN;
                     const bool to_tile = !last || store;
                     if (to_tile) {
                         // the rows are overwritten: the stores of the previous layer (if any) must have read them
@@ -1894,7 +1874,6 @@ extern "C" int morl_gemm_planes_mn_f32(int fmt, const void* g_planes, long long 
 }
 
 // Row chunks of the split column sums: each chunk writes one row of partials to the workspace, reduced in a fixed order afterwards.
-constexpr int kColsumChunks = 296;     // morl_colsum_planes
 constexpr int kPgrFusedChunks = 296;   // morl_pairs_grad_reduce_planes, one-pass form
 constexpr int kPgrTwoPassChunks = 74;  // morl_pairs_grad_reduce_planes, two-pass form
 
@@ -1907,30 +1886,9 @@ static int pgr_fused_rows_per_chunk(int B, int W) {
     return (B + bpc - 1) / bpc <= kPgrFusedChunks ? bpc : 0;
 }
 
-extern "C" size_t morl_colsum_workspace_bytes(int N) { return N > 0 ? (size_t)kColsumChunks * N * sizeof(float) : 0; }
-
 extern "C" size_t morl_pairs_grad_reduce_workspace_bytes(int B, int W, int H) {
     if (B <= 0 || W <= 0 || H <= 0) return 0;
     return (size_t)(pgr_fused_rows_per_chunk(B, W) ? kPgrFusedChunks : kPgrTwoPassChunks) * W * H * sizeof(float);
-}
-
-extern "C" int morl_colsum_planes(int fmt, const void* planes, long long plane_stride, const float* scale, int M, int ld, int N, float* out,
-                                  void* workspace, void* stream) {
-    using namespace morl;
-    MORL_REQUIRE(fmt_ok(fmt), MORL_ERR_UNSUPPORTED, "morl_colsum_planes: unknown plane format %d", fmt);
-    MORL_REQUIRE(planes && out && workspace, MORL_ERR_NULL, "morl_colsum_planes: NULL pointer argument");
-    MORL_REQUIRE(M > 0 && N > 0 && ld >= N && ld % 8 == 0 && plane_stride % 8 == 0, MORL_ERR_SHAPE, "morl_colsum_planes: bad shape M=%d N=%d ld=%d", M, N, ld);
-    const int chunks = kColsumChunks;
-    const int rpc = (M + chunks - 1) / chunks;
-    const int nch = (M + rpc - 1) / rpc;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    float* part = static_cast<float*>(workspace);
-    MORL_DISPATCH_FMT(fmt, (colsum_planes_kernel<kFmt><<<dim3((unsigned)nch, (unsigned)((ld + 255) / 256)), dim3(32, 8), 0, st>>>(
-                               static_cast<const uint16_t*>(planes), plane_stride, M, ld, N, rpc, part)));
-    int rc = check_launch("morl_colsum_planes");
-    if (rc) return rc;
-    launch_k(reduce_partials_kernel, dim3((N + 31) / 32), dim3(dim3(32, 8)), 0, st, part, nch, 1, N, 1, N, 0, out, N, 1 << 30, nullptr, nullptr, scale, nullptr);
-    return check_launch("morl_colsum_planes(reduce)");
 }
 
 extern "C" int morl_pairs_grad_reduce_planes(int fmt, const void* planes, long long plane_stride, const float* scale, int B, int W, int H, float* dU,
@@ -2113,9 +2071,8 @@ struct LnDropArgs {
 
 static int gemm_planes_impl(int fmt, const void* a_planes, long long a_plane_stride, const float* a_scale, const void* b_planes,
                             long long b_plane_stride, const float* b_scale, int M, int N, int N_pad, int K, const float* bias, int relu,
-                            const void* relu_mask_plane0, int ld_mask, float* c_f32, int ldc, void* c_planes, int ldp, long long c_plane_stride,
-                            const float* c_scale, int reverse_tiles, int split_accumulators, const void* relu_bits_in, void* relu_bits_out,
-                            const LnDropArgs* lnd, const char* name, void* stream) {
+                            float* c_f32, int ldc, void* c_planes, int ldp, long long c_plane_stride, const float* c_scale, int reverse_tiles,
+                            int split_accumulators, const void* relu_bits_in, void* relu_bits_out, const LnDropArgs* lnd, const char* name, void* stream) {
     MORL_REQUIRE(fmt_ok(fmt), MORL_ERR_UNSUPPORTED, "%s: unknown plane format %d", name, fmt);
     MORL_REQUIRE(a_planes && b_planes && (c_f32 || c_planes), MORL_ERR_NULL, "%s: NULL pointer argument", name);
     MORL_REQUIRE(M > 0 && N > 0 && K > 0 && N_pad >= N, MORL_ERR_SHAPE, "%s: bad shape M=%d N=%d N_pad=%d K=%d", name, M, N, N_pad, K);
@@ -2143,7 +2100,7 @@ static int gemm_planes_impl(int fmt, const void* a_planes, long long a_plane_str
     g.M = M; g.N = N; g.N_pad = N_pad; g.K = K;
     g.bias = bias; g.c_f32 = c_f32; g.ldc = ldc;
     g.c_planes = c_planes; g.ldp = ldp; g.plane_stride = c_plane_stride;
-    g.mask = static_cast<const uint16_t*>(relu_mask_plane0); g.ld_mask = ld_mask; g.relu = relu;
+    g.relu = relu;
     g.bits_in = static_cast<const uint32_t*>(relu_bits_in); g.bits_out = static_cast<uint32_t*>(relu_bits_out);
     g.bits_ld = relu_bits_words(N_pad);  // every 32-column chunk below N_pad has its word, padding chunks included
     {
@@ -2156,8 +2113,6 @@ static int gemm_planes_impl(int fmt, const void* a_planes, long long a_plane_str
         const uint32_t room = fmt == MORL_FMT_F16X2 ? KPlan<MORL_FMT_F16X2>::kOffC : KPlan<MORL_FMT_BF16X3>::kOffC;
         int n_st = (int)(room / (a_box + b_box));
         if (n_st > 8) n_st = 8;
-        static const int st_env = [] { const char* e = getenv("MORL_GEMM_STAGES"); return e ? atoi(e) : 0; }();
-        if (st_env > 0 && st_env < n_st) n_st = st_env;  // A/B measurements
         g.n_stages = n_st;
         g.b_stage = b_box;
     }
@@ -2172,8 +2127,6 @@ static int gemm_planes_impl(int fmt, const void* a_planes, long long a_plane_str
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int sms = sm_count();
-    // accumulator mode (see gemm_planes_kernel): per call; MORL_GEMM_SPLIT_ACC=0 / 1 overrides every call (A/B measurements)
-    static const int split_env = [] { const char* e = getenv("MORL_GEMM_SPLIT_ACC"); return e ? (e[0] == '0' ? 0 : 1) : -1; }();
     if (lnd) {
         g.ln = lnd->ln; g.ln_eps = lnd->eps; g.ln_gamma = lnd->gamma; g.ln_beta = lnd->beta;
         g.drop_seed = lnd->seed; g.drop_offset = lnd->offset; g.drop_salt = lnd->salt; g.drop_thr = lnd->thr; g.drop_scale = lnd->scale;
@@ -2181,10 +2134,10 @@ static int gemm_planes_impl(int fmt, const void* a_planes, long long a_plane_str
         return fmt == MORL_FMT_F16X2 ? launch_gemm_planes<MORL_FMT_F16X2, 0, kEpiLn>(tmA, tmB, tmC, g, sms, st)
                                      : launch_gemm_planes<MORL_FMT_BF16X3, 0, kEpiLn>(tmA, tmB, tmC, g, sms, st);
     }
-    const bool split_acc = split_env >= 0 ? split_env != 0 : split_accumulators != 0;
+    // accumulator mode (see gemm_planes_kernel): per call
     if (fmt == MORL_FMT_F16X2)
-        return split_acc ? launch_gemm_planes<MORL_FMT_F16X2, 1>(tmA, tmB, tmC, g, sms, st) : launch_gemm_planes<MORL_FMT_F16X2, 0>(tmA, tmB, tmC, g, sms, st);
-    return split_acc ? launch_gemm_planes<MORL_FMT_BF16X3, 1>(tmA, tmB, tmC, g, sms, st) : launch_gemm_planes<MORL_FMT_BF16X3, 0>(tmA, tmB, tmC, g, sms, st);
+        return split_accumulators ? launch_gemm_planes<MORL_FMT_F16X2, 1>(tmA, tmB, tmC, g, sms, st) : launch_gemm_planes<MORL_FMT_F16X2, 0>(tmA, tmB, tmC, g, sms, st);
+    return split_accumulators ? launch_gemm_planes<MORL_FMT_BF16X3, 1>(tmA, tmB, tmC, g, sms, st) : launch_gemm_planes<MORL_FMT_BF16X3, 0>(tmA, tmB, tmC, g, sms, st);
 }
 
 __global__ void philox_advance_kernel(unsigned int* offset, unsigned int inc) {
@@ -2195,12 +2148,11 @@ __global__ void philox_advance_kernel(unsigned int* offset, unsigned int inc) {
 
 extern "C" int morl_gemm_planes_f32(int fmt, const void* a_planes, long long a_plane_stride, const float* a_scale, const void* b_planes,
                                     long long b_plane_stride, const float* b_scale, int M, int N, int N_pad, int K, const float* bias, int relu,
-                                    const void* relu_mask_plane0, int ld_mask, float* c_f32, int ldc, void* c_planes, int ldp, long long c_plane_stride,
-                                    const float* c_scale, int reverse_tiles, int split_accumulators, const void* relu_bits_in, void* relu_bits_out,
-                                    void* stream) {
-    return morl::gemm_planes_impl(fmt, a_planes, a_plane_stride, a_scale, b_planes, b_plane_stride, b_scale, M, N, N_pad, K, bias, relu, relu_mask_plane0,
-                                  ld_mask, c_f32, ldc, c_planes, ldp, c_plane_stride, c_scale, reverse_tiles, split_accumulators, relu_bits_in,
-                                  relu_bits_out, nullptr, "morl_gemm_planes_f32", stream);
+                                    float* c_f32, int ldc, void* c_planes, int ldp, long long c_plane_stride, const float* c_scale, int reverse_tiles,
+                                    int split_accumulators, const void* relu_bits_in, void* relu_bits_out, void* stream) {
+    return morl::gemm_planes_impl(fmt, a_planes, a_plane_stride, a_scale, b_planes, b_plane_stride, b_scale, M, N, N_pad, K, bias, relu, c_f32, ldc,
+                                  c_planes, ldp, c_plane_stride, c_scale, reverse_tiles, split_accumulators, relu_bits_in, relu_bits_out, nullptr,
+                                  "morl_gemm_planes_f32", stream);
 }
 
 extern "C" int morl_gemm_planes_ln_f32(int fmt, const void* a_planes, long long a_plane_stride, const float* a_scale, const void* b_planes,
@@ -2223,8 +2175,8 @@ extern "C" int morl_gemm_planes_ln_f32(int fmt, const void* a_planes, long long 
     a.thr = t >= 4294967295.0 ? 4294967295u : (unsigned int)t;
     a.scale = (float)(1.0 / (1.0 - (double)drop_p));
     a.bits = drop_bits_out;
-    return gemm_planes_impl(fmt, a_planes, a_plane_stride, a_scale, b_planes, b_plane_stride, b_scale, M, N, N, K, bias, 1, nullptr, 0, c_f32, ldc,
-                            c_planes, ldp, c_plane_stride, c_scale, reverse_tiles, 0, nullptr, nullptr, &a, "morl_gemm_planes_ln_f32", stream);
+    return gemm_planes_impl(fmt, a_planes, a_plane_stride, a_scale, b_planes, b_plane_stride, b_scale, M, N, N, K, bias, 1, c_f32, ldc, c_planes, ldp,
+                            c_plane_stride, c_scale, reverse_tiles, 0, nullptr, nullptr, &a, "morl_gemm_planes_ln_f32", stream);
 }
 
 extern "C" int morl_philox_advance(unsigned int* offset, unsigned int inc, void* stream) {

@@ -557,17 +557,17 @@ def _relu_bits(a, t, name, rows, width, out=False):
 
 
 def gemm_planes(a_planes: th.Tensor, b_planes: th.Tensor, n_out: int, bias: Optional[th.Tensor] = None, relu: bool = False,
-                relu_mask: Optional[th.Tensor] = None, out_f32: bool = True, out_planes: bool = False, c_f32: Optional[th.Tensor] = None,
-                c_planes: Optional[th.Tensor] = None, reverse_tiles: bool = False, a_scale: Optional[th.Tensor] = None,
-                b_scale: Optional[th.Tensor] = None, c_scale: Optional[th.Tensor] = None, split_acc: bool = False,
-                relu_bits_in: Optional[th.Tensor] = None, relu_bits_out: Optional[th.Tensor] = None):
+                out_f32: bool = True, out_planes: bool = False, c_f32: Optional[th.Tensor] = None, c_planes: Optional[th.Tensor] = None,
+                reverse_tiles: bool = False, a_scale: Optional[th.Tensor] = None, b_scale: Optional[th.Tensor] = None,
+                c_scale: Optional[th.Tensor] = None, split_acc: bool = False, relu_bits_in: Optional[th.Tensor] = None,
+                relu_bits_out: Optional[th.Tensor] = None):
     """C = act(A . B^T + bias) on the tensor cores (wgmma) with split operands (fp32-accurate).
     a_planes [P, M, K], b_planes [P, N_pad, K]; the scales are device floats the planes were multiplied by (None = 1);
     ``split_acc``: leading and correction products in separate accumulators (the tensor cores truncate their fp32 accumulation; ~2.5x
     smaller systematic error, ~20 % slower per launch); False (default): one double-buffered accumulator.
     ``relu_bits_out`` / ``relu_bits_in`` (:func:`empty_relu_bits`): the forward call records [C > 0] as one bit per column, the backward
-    call zeroes the outputs whose bit is clear (ReLU backward from 32 bytes per row instead of the activation planes; ``relu_mask`` is the
-    plane-based form of the same mask).  Their width is the padded output width N_pad = b_planes.shape[1]
+    call zeroes the outputs whose bit is clear (ReLU backward from 32 bytes per row instead of the activation planes).  Their width is the
+    padded output width N_pad = b_planes.shape[1]
     (``empty_relu_bits(M, device, N_pad)``): 8 words per row up to 256, 16 above.
     returns (c_f32 [M, n_out] or None, c_planes [P, M, ldp] holding c_scale * C, or None)."""
     a = _Args("gemm_planes")
@@ -576,9 +576,6 @@ def gemm_planes(a_planes: th.Tensor, b_planes: th.Tensor, n_out: int, bias: Opti
     a.planes(b_planes, "b_planes", fmt, ld=K)
     n_pad = b_planes.shape[1]
     bias = a.inp(bias, "bias", reshape=(n_out,), opt=True)
-    if relu_mask is not None:
-        a.planes(relu_mask, "relu_mask", fmt, M)
-    mask0 = None if relu_mask is None else relu_mask[0]
     c_f32 = a.out(c_f32, "c_f32", (M, n_out), alloc=out_f32, ld=True)
     if out_planes and c_planes is None:
         c_planes = empty_planes(fmt, M, _pad(n_out, 32), a.device)
@@ -587,9 +584,8 @@ def gemm_planes(a_planes: th.Tensor, b_planes: th.Tensor, n_out: int, bias: Opti
     # one bit-mask word per 32-column chunk of the padded output (the kernel visits them all)
     relu_bits_in, relu_bits_out = _relu_bits(a, relu_bits_in, "relu_bits_in", M, n_pad), _relu_bits(a, relu_bits_out, "relu_bits_out", M, n_pad, True)
     _launch("morl_gemm_planes_f32", fmt, a_planes, a_planes.stride(0), a.scalar(a_scale, "a_scale"), b_planes, b_planes.stride(0), a.scalar(b_scale, "b_scale"),
-            M, n_out, n_pad, K, bias, int(relu), mask0, 0 if mask0 is None else mask0.stride(0), c_f32, 0 if c_f32 is None else c_f32.stride(0), c_planes,
-            0 if c_planes is None else c_planes.shape[2], 0 if c_planes is None else c_planes.stride(0), a.scalar(c_scale, "c_scale"), int(reverse_tiles),
-            int(bool(split_acc)), relu_bits_in, relu_bits_out)
+            M, n_out, n_pad, K, bias, int(relu), c_f32, 0 if c_f32 is None else c_f32.stride(0), c_planes, 0 if c_planes is None else c_planes.shape[2],
+            0 if c_planes is None else c_planes.stride(0), a.scalar(c_scale, "c_scale"), int(reverse_tiles), int(bool(split_acc)), relu_bits_in, relu_bits_out)
     return c_f32, c_planes
 
 
@@ -976,23 +972,6 @@ def gemm_planes_mn(g_planes: th.Tensor, g_cols: int, h_planes: th.Tensor, h_cols
     workspace = a.ws(workspace, "workspace", gemm_mn_workspace_bytes(M, g_cols, h_cols))
     _launch("morl_gemm_planes_mn_f32", fmt, g_planes, g_planes.stride(0), ldg, g_cols, a.scalar(g_scale, "g_scale"), h_planes, h_planes.stride(0), ldh,
             h_cols, a.scalar(h_scale, "h_scale"), M, int(transpose_out), out, out.stride(0), colsum, workspace, launches=2)
-    return out
-
-
-def colsum_workspace(n_cols: int, device) -> th.Tensor:
-    nbytes = _lib.load().morl_colsum_workspace_bytes(int(n_cols))
-    return th.empty((nbytes + 3) // 4, device=device, dtype=th.float32)
-
-
-def colsum_planes(planes: th.Tensor, n_cols: int, out: Optional[th.Tensor] = None, workspace: Optional[th.Tensor] = None,
-                  scale: Optional[th.Tensor] = None) -> th.Tensor:
-    """Column sums over the rows and the planes, scale removed (bias gradients)."""
-    a = _Args("colsum_planes")
-    fmt = a.planes(planes, "planes")
-    _, M, ld = planes.shape
-    out = a.out(out, "out", (n_cols,))
-    workspace = a.ws(workspace, "workspace", _lib.load().morl_colsum_workspace_bytes(int(n_cols)))
-    _launch("morl_colsum_planes", fmt, planes, planes.stride(0), a.scalar(scale, "scale"), M, ld, n_cols, out, workspace, launches=2)
     return out
 
 

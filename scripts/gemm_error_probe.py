@@ -2,7 +2,7 @@
     bias  = mean of (c - ref) / (|A| . |B|^T)      (a systematic component: the tensor cores' fp32 accumulation TRUNCATES)
     rms   = rms of the same ratio
 and the error of a whole 4 x 256 Q-network forward (TCPairMlp) against a float64 forward of the same parameters.
-Run once per accumulator mode:  MORL_GEMM_SPLIT_ACC=1 / 0 python scripts/gemm_error_probe.py"""
+usage: gemm_error_probe.py [single|split]   (accumulator mode of the GEMMs and of the network's layers; default single)"""
 import os
 import sys
 
@@ -19,7 +19,8 @@ a = th.randn(M, K, device=dev, generator=g).relu_()
 b = th.randn(N, K, device=dev, generator=g) / 16
 ref = a.double() @ b.double().t()
 mag = a.abs().double() @ b.abs().double().t()
-print("accumulators:", "split" if os.environ.get("MORL_GEMM_SPLIT_ACC") == "1" else "single")
+split = len(sys.argv) > 1 and sys.argv[1] == "split"
+print("accumulators:", "split" if split else "single")
 
 
 def stats(name, c):
@@ -32,7 +33,7 @@ stats("cublas", a @ b.t())
 for fmt, name in ((ops.FMT_F16X2, "f16x2"), (ops.FMT_BF16X3, "bf16x3")):
     sa = ops.scale_tensor(8.0, dev) if fmt == ops.FMT_F16X2 else None
     sb = ops.scale_tensor(4096.0, dev) if fmt == ops.FMT_F16X2 else None
-    c, _ = ops.gemm_planes(ops.split_planes(a, fmt, scale=sa), ops.split_planes(b, fmt, scale=sb), N, a_scale=sa, b_scale=sb)
+    c, _ = ops.gemm_planes(ops.split_planes(a, fmt, scale=sa), ops.split_planes(b, fmt, scale=sb), N, a_scale=sa, b_scale=sb, split_acc=split)
     stats(name, c)
 
 # whole-network forward on the pair batch
@@ -56,7 +57,7 @@ with th.no_grad():
     print(f"  network forward vs float64: cublas fp32 max rel {float((q32.double() - q64).abs().max() / q64.abs().max()):.3e} "
           f"mean signed rel {float(((q32.double() - q64) / q64.abs().clamp_min(1e-3)).mean()):+.3e}")
     for fmt, name in ((ops.FMT_F16X2, "f16x2"), (ops.FMT_BF16X3, "bf16x3")):
-        plan = TCPairMlp(net, F, B, W, fmt=fmt)
+        plan = TCPairMlp(net, F, B, W, fmt=fmt, split_acc=split)
         plan.refresh_weights()
         q = plan.forward_pairs(feats, wset)
         e = q.double() - q64

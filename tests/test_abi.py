@@ -1,24 +1,17 @@
 """CPU-only checks of the drop-in boundary: libmorl_b200.so loads, exports exactly the symbols include/morl_b200.h
-declares, the ctypes signature table mirrors the header, and argument errors are reported without touching a device."""
+declares, the ctypes signatures read from the header are the declared ones, and argument errors are reported without touching a device."""
 
+import ctypes as C
 import os
-import re
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "morl_b200.h")
+from morl_baselines_b200 import _lib
 
 
 def _header_decls():
-    src = open(HEADER).read()
-    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    decls = {}
-    for m in re.finditer(r"MORL_API\s+([\w\s\*]+?)\s*\b(morl_\w+)\s*\(([^;]*?)\)\s*;", src, flags=re.S):
-        args = m.group(3).strip()
-        n = 0 if args in ("", "void") else len([a for a in args.split(",") if a.strip()])
-        decls[m.group(2)] = n
-    return decls
+    with open(_lib.HEADER) as f:
+        return _lib.signatures(f.read())
 
 
 def test_library_builds_and_loads():
@@ -26,29 +19,44 @@ def test_library_builds_and_loads():
 
     path = build.build()
     assert os.path.exists(path)
-    from morl_baselines_b200 import _lib
-
     lib = _lib.load()
-    assert lib.morl_version() == 100
+    assert lib.morl_version() == 200
 
 
 def test_header_and_library_export_the_same_symbols():
-    from morl_baselines_b200 import _lib
-
     decls = _header_decls()
     assert len(decls) >= 15
     lib = _lib.load()
-    for name in decls:
-        assert hasattr(lib, name), f"{name} declared in include/morl_b200.h but not exported by libmorl_b200.so"
-    assert set(decls) == set(_lib.SIGNATURES), set(decls) ^ set(_lib.SIGNATURES)
-    for name, nargs in decls.items():
-        assert len(_lib.SIGNATURES[name][1]) == nargs, f"{name}: header has {nargs} parameters, ctypes table {len(_lib.SIGNATURES[name][1])}"
+    for name, (res, args) in decls.items():
+        fn = getattr(lib, name, None)
+        assert fn is not None, f"{name} declared in include/morl_b200.h but not exported by libmorl_b200.so"
+        assert fn.restype is res and fn.argtypes == args, name
+
+
+def test_signatures_follow_the_declared_types():
+    """Every declaration parses, a few spelled out in full: pointers are c_void_p, value types their own ctypes type."""
+    vp, i, f, d, ll, i64, u, sz = C.c_void_p, C.c_int, C.c_float, C.c_double, C.c_longlong, C.c_int64, C.c_uint, C.c_size_t
+    decls = _header_decls()
+    assert decls["morl_last_error"] == (C.c_char_p, [])
+    assert decls["morl_version"] == (i, [])
+    assert decls["morl_polyak_f32"] == (i, [vp, vp, vp, i, i64, d, vp])
+    assert decls["morl_adam_workspace_bytes"] == (sz, [i, i64])
+    assert decls["morl_sumtree_set_f64"] == (i, [vp, i, ll, d, i, vp, vp, vp])
+    assert decls["morl_philox_advance"] == (i, [vp, u, vp])
+    assert decls["morl_gemm_planes_f32"] == (i, [i, vp, ll, vp, vp, ll, vp, i, i, i, i, vp, i, vp, i, vp, i, ll, vp, i, i, vp, vp, vp])
+    assert decls["morl_gemm_planes_ln_f32"] == (i, [i, vp, ll, vp, vp, ll, vp, i, i, i, vp, i, vp, vp, f, f, vp, vp, u, vp, i, vp, i, ll, vp, i,
+                                                   vp, vp])
+
+
+@pytest.mark.parametrize("decl", ["MORL_API int morl_x(int n, bool flag);", "MORL_API int morl_x(const int n);",
+                                  "MORL_API void morl_x(int n);", "MORL_API int morl_x(int);"])
+def test_signatures_refuse_unknown_types(decl):
+    with pytest.raises(_lib.MorlB200Error):
+        _lib.signatures(decl)
 
 
 def test_exported_symbols_are_only_the_abi():
     import subprocess
-
-    from morl_baselines_b200 import _lib
 
     out = subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH], capture_output=True, text=True).stdout
     exported = {l.split()[-1] for l in out.splitlines() if " T " in l}
@@ -56,8 +64,6 @@ def test_exported_symbols_are_only_the_abi():
 
 
 def test_argument_errors_need_no_device():
-    from morl_baselines_b200 import _lib
-
     lib = _lib.load()
     rc = lib.morl_envelope_td_f32(None, None, None, None, None, 0.99, 4, 4, 4, 3, 0, 0, None, None, None, None)
     assert rc == -1  # MORL_ERR_NULL
@@ -71,7 +77,7 @@ def test_argument_errors_need_no_device():
 def test_ops_refuse_cpu_tensors():
     import torch as th
 
-    from morl_baselines_b200 import _lib, ops
+    from morl_baselines_b200 import ops
 
     with pytest.raises(_lib.MorlB200Error):
         ops.pareto_mask(th.zeros(4, 2))
@@ -82,8 +88,6 @@ def test_ops_refuse_cpu_tensors():
 def test_fusion_coverage_predicates_need_no_device():
     """The `*_supported` predicates that decide between a fused kernel and the launches it replaces are pure host functions: their answers
     at the BASELINE shapes and just outside them (both sides are CUDA paths; an unsupported shape is refused by the fused entry point)."""
-    from morl_baselines_b200 import _lib
-
     lib = _lib.load()
     F16, BF16 = _lib.FMT_F16X2, _lib.FMT_BF16X3
     # fused output layers + envelope + Bellman: north-star, configs[1] (minecart: |W| 32, |A| 6, d 3), and what falls outside
@@ -106,12 +110,9 @@ def test_fusion_coverage_predicates_need_no_device():
 
 
 def test_reduction_workspaces_cover_the_chunk_partials():
-    """The column-sum reductions write one row of partials per row chunk: up to 296 chunks for morl_colsum_planes and the one-pass
-    pairs_grad_reduce (|W| <= 64, at most 8 transitions per chunk), up to 74 for the two-pass form (|W| > 64, or a batch too large for
-    296 chunks of 8).  The library's byte counts cover them, so no caller needs to know the chunk arithmetic."""
-    from morl_baselines_b200 import _lib
-
+    """The column-sum reductions write one row of partials per row chunk: up to 296 chunks for the one-pass pairs_grad_reduce (|W| <= 64,
+    at most 8 transitions per chunk), up to 74 for the two-pass form (|W| > 64, or a batch too large for 296 chunks of 8).  The library's
+    byte counts cover them, so no caller needs to know the chunk arithmetic."""
     lib = _lib.load()
-    assert lib.morl_colsum_workspace_bytes(24) >= 296 * 24 * 4
     for B, W, H, chunks in ((1024, 64, 256, 296), (6, 5, 64, 296), (3, 70, 64, 74), (256, 128, 256, 74), (4096, 8, 64, 74)):
         assert lib.morl_pairs_grad_reduce_workspace_bytes(B, W, H) >= chunks * W * H * 4, (B, W, H)

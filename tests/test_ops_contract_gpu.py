@@ -227,10 +227,10 @@ def _gemm_operands(M=256, K=128, N=64):
 @row("morl_gemm_planes_f32")
 def gemm_planes():
     ap, bp, sa, sw = _gemm_operands()
-    kw = dict(a_planes=ap, b_planes=bp, n_out=64, bias=rn(64), relu=True, relu_mask=planes(256, 64), out_f32=True, out_planes=True,
+    kw = dict(a_planes=ap, b_planes=bp, n_out=64, bias=rn(64), relu=True, out_f32=True, out_planes=True,
               c_f32=sentinel(256, 64), c_planes=ops.empty_planes(F16, 256, 64, DEV).fill_(-7), a_scale=sa, b_scale=sw, c_scale=sa,
               relu_bits_in=th.full((256, 8), -1, dtype=th.int32, device=DEV), relu_bits_out=sentinel(256, 8, dtype=th.int32))
-    kinds = dict(a_planes="planes", b_planes="planes", bias="in", relu_mask="planes", c_f32="out", c_planes="planes_out", a_scale="scalar",
+    kinds = dict(a_planes="planes", b_planes="planes", bias="in", c_f32="out", c_planes="planes_out", a_scale="scalar",
                  b_scale="scalar", c_scale="scalar", relu_bits_in="in", relu_bits_out="out")
     return ops.gemm_planes, kw, kinds
 
@@ -368,13 +368,6 @@ def gemm_planes_mn():
               out=sentinel(24, 128), workspace=ws_bytes(ops.gemm_mn_workspace_bytes(300, 24, 128)), colsum=sentinel(24), g_scale=sg, h_scale=sa)
     kinds = dict(g_planes="planes", h_planes="planes", out="out", workspace="ws", colsum="out", g_scale="scalar", h_scale="scalar")
     return ops.gemm_planes_mn, kw, kinds
-
-
-@row("morl_colsum_planes")
-def colsum_planes():
-    kw = dict(planes=planes(300, 64), n_cols=24, out=sentinel(24), workspace=ws_bytes(_lib.load().morl_colsum_workspace_bytes(24)),
-              scale=ops.scale_tensor(2.0, DEV))
-    return ops.colsum_planes, kw, dict(planes="planes", out="out", workspace="ws", scale="scalar")
 
 
 @row("morl_pairs_grad_reduce_planes")
