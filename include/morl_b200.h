@@ -564,6 +564,11 @@ MORL_API int morl_adam_clip_lr_f32(float* const* params, const float* const* gra
 MORL_API int morl_vector_gae_f32(const float* rewards, const float* values, const float* dones, const float* next_value, const float* next_done,
                                  const float* weights, int T, int E, int D, double gamma, double gae_lambda, int use_gae, float* returns,
                                  float* advantages, void* stream);
+/* morl_vector_gae_objectives_f32 (nl_mo_ppo.py:290-308): the use_gae = 1 recursion of morl_vector_gae_f32 with the same rounding, writing the
+ *   per-objective advantages [T, E, D] (lastgaelam) instead of their weighted sum; returns [T, E, D] as there.  D <= MORL_MAX_D. */
+MORL_API int morl_vector_gae_objectives_f32(const float* rewards, const float* values, const float* dones, const float* next_value,
+                                            const float* next_done, int T, int E, int D, double gamma, double gae_lambda, float* returns,
+                                            float* advantages, void* stream);
 MORL_API int morl_ppo_loss_f32(const float* mean, const float* logstd, const float* value, const float* actions, const float* old_logprob,
                                const float* advantages, const float* returns, const float* old_values, int M, int A, int D, float clip_coef,
                                float ent_coef, float vf_coef, int norm_adv, int clip_vloss, float* loss_out, float* dmean, float* dlogstd,
@@ -627,6 +632,51 @@ MORL_API int morl_eupg_update_f32(const float* const* params, float* const* grad
                                   float* loss_out, void* workspace, void* stream);
 MORL_API int morl_eupg_probs_f32(const float* const* params, const float* x, int N, int obs_dim, int d, const int* hidden, int n_hidden,
                                  int n_out, float* out, void* stream);
+
+
+/* ------------------------------------------------------------------------------------------------
+ * Non-linear MO-PPO (reference single_policy/ser/nl_mo_ppo.py), csrc/nl_ppo.cu.
+ *
+ * The reference's Agent (nl_mo_ppo.py:26-108): x = [obs (S) || accrued reward (d) || pref (Dp)] with Dp in {0, d} (pref: one device vector
+ *   [Dp] shared by every row; zeros when the learner has no preference), critic x -> tanh(64) -> tanh(64) -> d, actor x -> tanh(64) ->
+ *   tanh(64) -> A logits of a Categorical.  params / grads: HOST arrays of the 12 device pointers in the Agent's parameter order
+ *   (critic.0.weight [64, K], critic.0.bias, critic.2.weight [64, 64], critic.2.bias, critic.4.weight [d, 64], critic.4.bias, then the
+ *   same six of the actor with actor.4.weight [A, 64]); K = S + d + Dp.
+ * Supported range (morl_nl_ppo_supported, no device needed): 1 <= S, 1 <= d <= MORL_MAX_D, Dp in {0, d}, K <= 256, 1 <= A <= 32 and a
+ *   minibatch (batch) of 1 to 4096 rows; anything else returns MORL_ERR_UNSUPPORTED.
+ *
+ * morl_nl_ppo_update_f32 (nl_mo_ppo.py:344-393): one minibatch of M rows; row i is source row perm[i] (int64) of obs f32 [B, S],
+ *   acc f32 [B, d], actions int64 [B], old_logprob [B], advantages / returns / old_values f32 [B, d] (old_values may be NULL without
+ *   clip_vloss).  With norm_adv (refused for M < 2) each objective's advantages are normalised by their minibatch mean and unbiased std
+ *   + 1e-8.  pg_loss = sum_o w_o mean_i max(-adv_io r_i, -adv_io clamp(r_i, 1 -+ clip)), r = exp(logp - old); v_loss = 0.5 mean over M*d of
+ *   (v - R)^2 or, with clip_vloss, of max((v - R)^2, (clip(v) - R)^2); entropy = mean Categorical entropy;
+ *   loss_out[0] (nullable) = pg_loss - ent_coef * entropy + vf_coef * v_loss.  grads are OVERWRITTEN with d loss / d params, with torch's
+ *   backward rules (th.max splits a tie half and half, clamp passes on its closed interval).  stats f32 [6]: pg_loss, v_loss, entropy,
+ *   old_approx_kl, approx_kl written; stats[5] += the clip fraction.  loss_weights f32 [d] is read at run time.  A fixed number of CTAs each
+ *   folds a contiguous range of 16-row tiles into its own partial, a second launch sums them in CTA order: no float atomics, results depend
+ *   on neither the SM count nor the run.  workspace: morl_nl_ppo_workspace_bytes(...) bytes, independent of M.  Two launches.
+ * morl_nl_ppo_forward_f32 (nl_mo_ppo.py:90-108): rows [obs (N x S) || acc (N x d) || pref]; logits [N, A], values [N, d] and argmax_out int32
+ *   [N] (first occurrence of the row maximum) are each nullable, at least one given.  obs, acc and the outputs may be pinned host memory.
+ *   One launch.
+ * morl_nl_ppo_commit_f32 (nl_mo_ppo.py:251-275): one rollout step of E environments.  For each e: row `step` of obs_store [T, E, S],
+ *   acc_store [T, E, d] and done_store [T, E] takes the carried next_obs [E, S], next_acc [E, d] and next_done [E]; act_store int64 [T, E]
+ *   takes action[e]; logp_store [T, E] the log-softmax of logits [E, A] at it; rew_store [T, E, d] the staged reward.  staged f32
+ *   [E, S + d + 2] = obs | reward | terminated | truncated of the environment step; then next_obs = obs, next_done = terminated | truncated,
+ *   next_acc = (next_acc + powf((float)gamma, (float)t) * reward) * (1 - next_done) and timestep int32 [E] t = (t + 1) * (1 - next_done),
+ *   each operation rounded once as torch's device expression.  One launch. */
+MORL_API int morl_nl_ppo_supported(int obs_dim, int d, int pref_dim, int n_actions, int batch);
+MORL_API size_t morl_nl_ppo_workspace_bytes(int obs_dim, int d, int pref_dim, int n_actions);
+MORL_API int morl_nl_ppo_update_f32(const float* const* params, float* const* grads, const float* obs, const float* acc, const int64_t* actions,
+                                    const float* old_logprob, const float* advantages, const float* returns, const float* old_values,
+                                    const int64_t* perm, int M, int obs_dim, int d, int pref_dim, int n_actions, const float* pref,
+                                    const float* loss_weights, float clip_coef, float ent_coef, float vf_coef, int norm_adv, int clip_vloss,
+                                    float* loss_out, float* stats, void* workspace, void* stream);
+MORL_API int morl_nl_ppo_forward_f32(const float* const* params, const float* obs, const float* acc, int N, int obs_dim, int d, int pref_dim,
+                                     int n_actions, const float* pref, float* logits, float* values, int32_t* argmax_out, void* stream);
+MORL_API int morl_nl_ppo_commit_f32(const float* staged, const float* logits, const int64_t* action, int step, int E, int obs_dim, int d,
+                                    int n_actions, double gamma, float* obs_store, float* acc_store, float* done_store, float* rew_store,
+                                    int64_t* act_store, float* logp_store, float* next_obs, float* next_acc, float* next_done, int32_t* timestep,
+                                    void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,6 +1,7 @@
 // ppo.cu -- the device side of MO-PPO's update (reference single_policy/ser/mo_ppo.py).
 //
-// morl_vector_gae_f32 : the reverse GAE / discounted-return recursion of :439-476 in one launch
+// morl_vector_gae_f32            : the reverse GAE / discounted-return recursion of :439-476 in one launch
+// morl_vector_gae_objectives_f32 : the same recursion, keeping the per-objective advantages (nl_mo_ppo.py:290-308)
 // morl_ppo_loss_f32   : one minibatch's clipped PPO loss, its gradients w.r.t. the actor mean, actor_logstd and the vector value head,
 //                       and the logged statistics (:514-549) in one launch
 #include "common.cuh"
@@ -10,11 +11,13 @@ namespace morl {
 // ---- vector GAE ------------------------------------------------------------------------------------------------------------------
 // One lane per (env, objective), sequential over T from the last step back.  A CTA owns 32 / d whole environments, so the
 // scalarisation of its advantages needs no other CTA.  Chunks of kGaeChunk steps of rewards, values and dones are staged in shared
-// memory by the whole CTA before the lanes walk them, so the dependent chain never waits on a global load.
+// memory by the whole CTA before the lanes walk them, so the dependent chain never waits on a global load.  kScalarise = false writes
+// each lane's advantage to adv_out [T, E, D] as it is produced and skips the scalarisation.
 constexpr int kGaeThreads = 128;
 constexpr int kGaeLanes = 32;  // (env, objective) lanes per CTA; the lanes of one env are never split
 constexpr int kGaeChunk = 64;
 
+template <bool kScalarise>
 __global__ void __launch_bounds__(kGaeThreads) vector_gae_kernel(const float* __restrict__ rewards, const float* __restrict__ values,
                                                                  const float* __restrict__ dones, const float* __restrict__ next_value,
                                                                  const float* __restrict__ next_done, const float* __restrict__ w, int T, int E,
@@ -71,9 +74,13 @@ __global__ void __launch_bounds__(kGaeThreads) vector_gae_kernel(const float* __
                     returns[(size_t)(t0 + tt) * row + (size_t)e0 * D + lane] = carry;
                     a = __fsub_rn(carry, v);
                 }
-                s_a[tt][lane] = a;
+                if constexpr (kScalarise)
+                    s_a[tt][lane] = a;
+                else
+                    adv_out[(size_t)(t0 + tt) * row + (size_t)e0 * D + lane] = a;
             }
         }
+        if constexpr (!kScalarise) continue;
         __syncthreads();
         for (int k = threadIdx.x; k < n * ne; k += blockDim.x) {
             const int tt = k / ne, e = k - tt * ne;
@@ -255,9 +262,25 @@ extern "C" int morl_vector_gae_f32(const float* rewards, const float* values, co
     const int blocks = (E + envs_per_cta - 1) / envs_per_cta;
     // gamma and gamma * lambda are Python floats in the reference: gamma is rounded to fp32 by the tensor op, gamma * lambda is formed
     // in double and rounded once
-    vector_gae_kernel<<<blocks, kGaeThreads, 0, st>>>(rewards, values, dones, next_value, next_done, weights, T, E, D, envs_per_cta, (float)gamma,
+    vector_gae_kernel<true><<<blocks, kGaeThreads, 0, st>>>(rewards, values, dones, next_value, next_done, weights, T, E, D, envs_per_cta, (float)gamma,
                                                       (float)(gamma * gae_lambda), use_gae ? 1 : 0, returns, advantages);
     return check_launch("morl_vector_gae_f32");
+}
+
+extern "C" int morl_vector_gae_objectives_f32(const float* rewards, const float* values, const float* dones, const float* next_value,
+                                              const float* next_done, int T, int E, int D, double gamma, double gae_lambda, float* returns,
+                                              float* advantages, void* stream) {
+    using namespace morl;
+    MORL_REQUIRE(rewards && values && dones && next_value && next_done && returns && advantages, MORL_ERR_NULL,
+                 "morl_vector_gae_objectives_f32: NULL pointer argument");
+    MORL_REQUIRE(T > 0 && E > 0 && D > 0, MORL_ERR_SHAPE, "morl_vector_gae_objectives_f32: bad shape T=%d E=%d D=%d", T, E, D);
+    MORL_REQUIRE(D <= MORL_MAX_D, MORL_ERR_UNSUPPORTED, "morl_vector_gae_objectives_f32: D=%d > %d", D, MORL_MAX_D);
+    const int envs_per_cta = kGaeLanes / D;
+    const int blocks = (E + envs_per_cta - 1) / envs_per_cta;
+    vector_gae_kernel<false><<<blocks, kGaeThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+        rewards, values, dones, next_value, next_done, nullptr, T, E, D, envs_per_cta, (float)gamma, (float)(gamma * gae_lambda), 1, returns,
+        advantages);
+    return check_launch("morl_vector_gae_objectives_f32");
 }
 
 extern "C" int morl_ppo_loss_f32(const float* mean, const float* logstd, const float* value, const float* actions, const float* old_logprob,

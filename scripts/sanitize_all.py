@@ -2,7 +2,7 @@
 
     compute-sanitizer --tool memcheck|racecheck|synccheck|initcheck python scripts/sanitize_all.py [group ...]
 
-groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners ppo pcn eupg (default: all; dyna includes the fused Dyna commit).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
+groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners ppo pcn eupg nl_ppo (default: all; dyna includes the fused Dyna commit).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
 every code path: all envelope kernel families, both GEMM operand formats x CTA modes x accumulator modes, MN split-K GEMM with the fused
 column sums, every split / reduction helper, the loss kernels (discrete SAC's included), Adam, polyak, Pareto + front records, replay gather,
 the corner-weight enumeration, MO-PPO's vector GAE and loss (racecheck: the loss kernel's CTA reductions), PCN's update and forward,
@@ -24,7 +24,7 @@ if os.environ.get("SAN_ZERO_PLANES") == "1":
     # from a genuine read of memory nobody wrote.
     _empty = ops.empty_planes
     ops.empty_planes = lambda *a, **k: _empty(*a, **k).zero_()
-groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain", "corners", "ppo", "pcn", "eupg"}
+groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain", "corners", "ppo", "pcn", "eupg", "nl_ppo"}
 
 
 def rn(*s, scale=1.0):
@@ -275,4 +275,29 @@ if "eupg" in groups:
         ops.eupg_probs(knet, th.ones(1, S + d).pin_memory(), pin_out)
     th.cuda.synchronize()
     print("eupg ok")
+
+if "nl_ppo" in groups:
+    # non-linear MO-PPO (csrc/nl_ppo.cu, the objective GAE of csrc/ppo.cu): M = 2, a ragged last tile, M = 4096 (each CTA several tiles),
+    # Dp 0 and d, K = 256, A = 32; the forward on device and pinned rows; one commit step
+    from morl_baselines_b200 import nl_ppo_ops
+    from morl_baselines_b200.single_policy.ser.nl_mo_ppo import Agent
+    from tests.nl_ppo_standin import RingVecEnv
+
+    for S, d, Dp, A, M in [(2, 2, 2, 4, 2), (7, 3, 0, 6, 37), (240, 8, 8, 32, 4096)]:
+        ts = list(Agent(RingVecEnv(1, obs_dim=S, n_actions=A, d=d), d, Dp).to(dev).parameters())
+        knet = nl_ppo_ops.NlPpoNet(S, d, Dp, A, ts, [th.empty_like(t) for t in ts], rn(Dp) if Dp else None)
+        B = M + 5
+        perm = th.randperm(B, device=dev)[:M].contiguous()
+        nl_ppo_ops.nl_ppo_update(knet, rn(B, S), rn(B, d), th.randint(0, A, (B,), device=dev), rn(B), rn(B, d), rn(B, d), rn(B, d), perm, rn(d),
+                                 0.2, 0.01, 0.5, True, True, th.zeros(6, device=dev), knet.workspace(dev))
+        nl_ppo_ops.nl_ppo_forward(knet, rn(19, S), rn(19, d), th.zeros(19, A, device=dev), th.zeros(19, d, device=dev),
+                                  th.zeros(19, dtype=th.int32, device=dev))
+        nl_ppo_ops.nl_ppo_forward(knet, th.ones(1, S).pin_memory(), th.ones(1, d).pin_memory(), argmax_out=th.zeros(1, dtype=th.int32).pin_memory())
+        T, E = 3, 5
+        nl_ppo_ops.vector_gae_objectives(rn(T, E, d), rn(T, E, d), th.zeros(T, E, device=dev), rn(E, d), th.zeros(E, device=dev), 0.99, 0.95)
+        nl_ppo_ops.nl_ppo_commit(rn(E, S + d + 2), rn(E, A), th.randint(0, A, (E,), device=dev), 1, 0.99, rn(T, E, S), rn(T, E, d), rn(T, E),
+                                 rn(T, E, d), th.zeros(T, E, dtype=th.int64, device=dev), rn(T, E), rn(E, S), rn(E, d), th.zeros(E, device=dev),
+                                 th.zeros(E, dtype=th.int32, device=dev))
+    th.cuda.synchronize()
+    print("nl_ppo ok")
 print("sanitize run ok")
