@@ -269,6 +269,19 @@ MORL_API int morl_front_unpack_f64(const double* gathered, int world, int d, int
  * `ref` in every objective contribute nothing; dominated points are harmless (the volume is that of the union of boxes). */
 MORL_API int morl_hypervolume_f64(const double* pts, const uint8_t* keep, int n, int d, const double* ref, double* out, void* stream);
 
+/* Batched exact hypervolume (maximisation, float64) of "a base set plus one candidate" for every candidate, in one launch (one block per
+ * candidate): IPRO's hypervolume improvements of its sampled lower points (multi_policy/ipro/ipro.py:212-226) and its other volumes.
+ *   n_cand >= 1 : out[k] = volume of base [n_base, d] U { cand[k] } (cand [n_cand, d]) above ref [d], k < n_cand
+ *   n_cand == 0 : out[0] = volume of base alone (cand may be NULL)
+ * Points count as in morl_hypervolume_f64: q = p - ref clipped at 0; a point that does not exceed ref in every objective, or holds a NaN,
+ * spans nothing.  d = 4 slices over the fourth objective, each slab a 3-D volume by the same sweep (O(n^3) per set); results do not depend
+ * on the grid (fixed-shape reductions, no atomics), and with n_cand == 0 and d <= 3 they equal morl_hypervolume_f64's bit for bit.
+ * Supported range (morl_hypervolume_batch_supported, no device needed: 1 if supported, else 0): 1 <= d <= 4 and 0 <= n_base <= 2048 for
+ * d <= 3, <= 512 for d = 4; anything else returns MORL_ERR_UNSUPPORTED (compute on the host instead). */
+MORL_API int morl_hypervolume_batch_supported(int n, int d);
+MORL_API int morl_hypervolume_batch_f64(const double* base, int n_base, const double* cand, int n_cand, int d, const double* ref, double* out,
+                                        void* stream);
+
 /* Corner weights of a convex coverage set (OLS / GPI-LS weight selection).  Replaces compute_corner_weights
  * (multi_policy/linear_support/linear_support.py:295-349), which enumerates with cdd the vertices of
  *   { (w, u) : V w <= u 1,  w >= 0,  sum w = 1 }.

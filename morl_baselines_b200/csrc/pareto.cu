@@ -152,75 +152,120 @@ __global__ void __launch_bounds__(256) front_unpack_kernel(const double* __restr
     }
 }
 
-// ---- exact hypervolume (maximisation) of <= kHvMaxN points in d <= 3 objectives w.r.t. a reference point, one block ---------------------
+// ---- exact hypervolume (maximisation) of one set, or of a batch of sets "base plus one candidate", above a reference point -----------------
 // Replaces the host-side exact sweep behind `hypervolume(ref_point, points)` (reference common/performance_indicators.py:15-25, which
-// delegates to pymoo's exact HV) for fronts that already live on the device (the output of the global prune of an evaluation round).
-// q_i = p_i - ref clipped at 0 (a point that does not exceed ref in some objective spans no volume); volume of the union of the boxes
-// [0, q_i]:  d = 1: max q.   d = 2: sum over points in x-descending order of (x_(i) - x_(i+1)) * max_{j <= i} y_(j).   d = 3: slabs in
-// z-descending order: thread k integrates the 2-D staircase of the points with z-rank <= k over the x-descending order (an O(n) loop
-// per thread, n threads' worth of work in parallel -- n^2 total, no scans, no atomics) and multiplies by the slab height z_(k) - z_(k+1);
-// the n slab volumes are added by a fixed-shape tree reduction (deterministic).  Ranks come from counting (ties by index).
-constexpr int kHvMaxN = 2048;
+// delegates to pymoo's exact HV) for fronts that already live on the device, and IPRO's hypervolume improvements of the sampled lower points
+// (reference multi_policy/ipro/ipro.py:212-226: one exact volume per candidate, all of them in one launch here).
+// q_i = p_i - ref clipped at 0 (a point that does not exceed ref in some objective spans no volume; nor does a NaN); missing objectives get
+// a unit extent, so every set is treated as 4-D.  Volume of the union of the boxes [0, q_i]: slabs in w-descending order (only one slab of
+// height 1 when d <= 3), each slab a 3-D volume of the points with w-rank <= j; that volume is a sum over z-descending slabs of the 2-D
+// staircase area of the points with z-rank <= k (and w-rank <= j), integrated over the x-descending order.  Thread t of the block takes the
+// (w-slab, z-slab) pairs t, t + blockDim, ... (an O(n) loop each: n^2 work for d <= 3, n^3 for d = 4, no scans, no atomics); the slab
+// volumes are added by a fixed-shape tree reduction (deterministic).  Ranks come from counting (ties by index).
+constexpr int kHvMaxN = 2048;     // points per set, d <= 3
+constexpr int kHvMaxN4 = 512;     // points per set, d = 4 (O(n^3) per set)
 constexpr int kHvThreads = 1024;
 
-__global__ void __launch_bounds__(kHvThreads) hypervolume_kernel(const double* __restrict__ pts, const uint8_t* __restrict__ keep, int n, int d,
-                                                                 const double* __restrict__ ref, double* __restrict__ out) {
-    extern __shared__ double hv_smem[];  // (everything dynamic: 7 n + 1 + 1024 doubles + n shorts -- up to ~127 KB at n = 2048)
-    double* red = hv_smem;                       // [kHvThreads] tree reduction
-    double* rx = red + kHvThreads;               // [3][n] staging (x, y, z of point i, input order)
-    double* ry = rx + n;
-    double* rz = ry + n;
-    double* qx = rz + n;                         // shifted, clipped coordinates in x-descending order
-    double* qy = qx + n;
-    double* qz = qy + n;
-    double* zs = qz + n;                         // [n + 1] z values in z-descending order, then 0
-    short* zr = reinterpret_cast<short*>(zs + n + 1);  // z-rank (0 = largest z) of the point at x-position i
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        const bool k = keep == nullptr || keep[i] != 0;
-        double c[3] = {0.0, 1.0, 1.0};  // missing objectives: unit extent (the product then is the lower-dimensional volume)
-        bool ok = k;
-        for (int r = 0; r < d; ++r) {
-            const double v = pts[(size_t)i * d + r] - ref[r];
+// shared-memory carve for sets of up to n points: red [kHvThreads] | rx ry rz rw [n] (input order) | qx qy [n] (x-descending order) |
+// zs ws [n + 1] (descending, then 0) | zr wr [n] shorts (z- and w-rank of the point at x-position i)
+struct HvSmem {
+    double *red, *rx, *ry, *rz, *rw, *qx, *qy, *zs, *ws;
+    short *zr, *wr;
+};
+
+__host__ __device__ constexpr size_t hv_smem_bytes(int n) { return ((size_t)kHvThreads + 8 * (size_t)n + 2) * sizeof(double) + 2 * (size_t)n * sizeof(short); }
+
+__device__ __forceinline__ HvSmem hv_carve(double* smem, int n) {
+    HvSmem s;
+    s.red = smem;
+    s.rx = s.red + kHvThreads; s.ry = s.rx + n; s.rz = s.ry + n; s.rw = s.rz + n;
+    s.qx = s.rw + n; s.qy = s.qx + n;
+    s.zs = s.qy + n; s.ws = s.zs + n + 1;
+    s.zr = reinterpret_cast<short*>(s.ws + n + 1); s.wr = s.zr + n;
+    return s;
+}
+
+// stage point i: its clipped offsets from ref (all zero unless it exceeds ref in every objective and `keep`)
+__device__ __forceinline__ void hv_stage(const HvSmem& s, int i, const double* __restrict__ p, bool keep, int d, const double* __restrict__ ref) {
+    double c[4] = {0.0, 1.0, 1.0, 1.0};
+    bool ok = keep;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        if (r < d) {
+            const double v = p[r] - ref[r];
             c[r] = v > 0.0 ? v : 0.0;  // (NaN fails the comparison: contributes nothing)
             ok = ok && (v > 0.0);
         }
-        rx[i] = ok ? c[0] : 0.0; ry[i] = ok ? c[1] : 0.0; rz[i] = ok ? c[2] : 0.0;
     }
-    __syncthreads();
-    // rank by counting: position of point i in x-descending order (ties by index), and its z-descending rank
+    s.rx[i] = ok ? c[0] : 0.0; s.ry[i] = ok ? c[1] : 0.0; s.rz[i] = ok ? c[2] : 0.0; s.rw[i] = ok ? c[3] : 0.0;
+}
+
+// the volume of the n staged points (every thread returns it); `sliced_w`: the w-slabs of d = 4, else one slab of height 1
+__device__ __forceinline__ double hv_sweep(const HvSmem& s, int n, bool sliced_w) {
+    // rank by counting: position of point i in x-descending order (ties by index), its z- and w-descending ranks
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        const double xi = rx[i], zi = rz[i];
-        int px = 0, pz = 0;
+        const double xi = s.rx[i], zi = s.rz[i], wi = s.rw[i];
+        int px = 0, pz = 0, pw = 0;
         for (int j = 0; j < n; ++j) {
-            px += (rx[j] > xi || (rx[j] == xi && j < i)) ? 1 : 0;
-            pz += (rz[j] > zi || (rz[j] == zi && j < i)) ? 1 : 0;
+            px += (s.rx[j] > xi || (s.rx[j] == xi && j < i)) ? 1 : 0;
+            pz += (s.rz[j] > zi || (s.rz[j] == zi && j < i)) ? 1 : 0;
+            if (sliced_w) pw += (s.rw[j] > wi || (s.rw[j] == wi && j < i)) ? 1 : 0;
         }
-        qx[px] = xi; qy[px] = ry[i]; qz[px] = zi; zr[px] = (short)pz;
-        zs[pz] = zi;
+        s.qx[px] = xi; s.qy[px] = s.ry[i]; s.zr[px] = (short)pz; s.wr[px] = (short)pw;
+        s.zs[pz] = zi; s.ws[pw] = wi;
     }
-    if (threadIdx.x == 0) zs[n] = 0.0;
+    if (threadIdx.x == 0) { s.zs[n] = 0.0; s.ws[n] = 0.0; }
     __syncthreads();
+    const int nw = sliced_w ? n : 1;
     double acc = 0.0;
-    for (int k = threadIdx.x; k < n; k += blockDim.x) {
-        const double height = zs[k] - zs[k + 1];  // slab between the k-th and (k+1)-th largest z
-        if (height > 0.0) {
+    for (int t = threadIdx.x; t < nw * n; t += blockDim.x) {
+        const int j = t / n, k = t - j * n;           // w-slab j, z-slab k
+        const double zh = s.zs[k] - s.zs[k + 1];      // slab between the k-th and (k+1)-th largest z
+        const double wh = sliced_w ? s.ws[j] - s.ws[j + 1] : 1.0;
+        if (zh > 0.0 && wh > 0.0) {
             double m = 0.0, area = 0.0;
             for (int i = 0; i < n; ++i) {
-                if ((int)zr[i] <= k) m = fmax(m, qy[i]);
-                const double xn = i + 1 < n ? qx[i + 1] : 0.0;
-                area += (qx[i] - xn) * m;
+                if ((int)s.zr[i] <= k && (int)s.wr[i] <= j) m = fmax(m, s.qy[i]);
+                const double xn = i + 1 < n ? s.qx[i + 1] : 0.0;
+                area = __fma_rn(s.qx[i] - xn, m, area);
             }
-            acc += area * height;
+            acc = __fma_rn(__dmul_rn(area, wh), zh, acc);  // (wh = 1 is exact: the d <= 3 sum is area * zh)
         }
     }
-    red[threadIdx.x] = acc;
+    s.red[threadIdx.x] = acc;
     __syncthreads();
     for (int off = kHvThreads / 2; off > 0; off >>= 1) {
-        if (threadIdx.x < off) red[threadIdx.x] += red[threadIdx.x + off];
+        if (threadIdx.x < off) s.red[threadIdx.x] += s.red[threadIdx.x + off];
         __syncthreads();
     }
-    if (threadIdx.x == 0) *out = red[0];
+    return s.red[0];
 }
+
+// one set: the points with keep[i] != 0 (keep NULL = all), d <= 3
+__global__ void __launch_bounds__(kHvThreads, 1) hypervolume_kernel(const double* __restrict__ pts, const uint8_t* __restrict__ keep, int n, int d,
+                                                                 const double* __restrict__ ref, double* __restrict__ out) {
+    extern __shared__ double hv_smem[];
+    const HvSmem s = hv_carve(hv_smem, n);
+    for (int i = threadIdx.x; i < n; i += blockDim.x) hv_stage(s, i, pts + (size_t)i * d, keep == nullptr || keep[i] != 0, d, ref);
+    __syncthreads();
+    const double v = hv_sweep(s, n, false);
+    if (threadIdx.x == 0) *out = v;
+}
+
+// block b: the set base [n_base] plus cand[b] (cand NULL: base alone), d <= 4
+__global__ void __launch_bounds__(kHvThreads, 1) hypervolume_batch_kernel(const double* __restrict__ base, int n_base, const double* __restrict__ cand,
+                                                                       int d, const double* __restrict__ ref, double* __restrict__ out) {
+    extern __shared__ double hv_smem[];
+    const int n = n_base + (cand != nullptr ? 1 : 0);
+    const HvSmem s = hv_carve(hv_smem, n);
+    for (int i = threadIdx.x; i < n; i += blockDim.x)
+        hv_stage(s, i, i < n_base ? base + (size_t)i * d : cand + (size_t)blockIdx.x * d, true, d, ref);
+    __syncthreads();
+    const double v = hv_sweep(s, n, d == 4);
+    if (threadIdx.x == 0) out[blockIdx.x] = v;
+}
+
+static int hv_batch_cap(int d) { return d >= 1 && d <= 3 ? kHvMaxN : d == 4 ? kHvMaxN4 : -1; }
 
 }  // namespace morl
 
@@ -258,13 +303,35 @@ extern "C" int morl_hypervolume_f64(const double* pts, const uint8_t* keep, int 
     MORL_REQUIRE(ref && out && (pts || n == 0), MORL_ERR_NULL, "morl_hypervolume_f64: NULL pointer argument");
     MORL_REQUIRE(n >= 0 && d >= 1 && d <= 3, MORL_ERR_UNSUPPORTED, "morl_hypervolume_f64: exact device hypervolume supports 1 <= d <= 3 (got d=%d)", d);
     MORL_REQUIRE(n <= kHvMaxN, MORL_ERR_UNSUPPORTED, "morl_hypervolume_f64: at most %d points (got %d): prune the set first", kHvMaxN, n);
-    const size_t smem = ((size_t)kHvThreads + 7 * (size_t)n + 1) * sizeof(double) + (size_t)n * sizeof(short) + 16;
     static bool configured = false;
     if (!configured) {
-        cudaFuncSetAttribute(hypervolume_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)(((size_t)kHvThreads + 7 * (size_t)kHvMaxN + 1) * sizeof(double) + (size_t)kHvMaxN * sizeof(short) + 16));
+        cudaFuncSetAttribute(hypervolume_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hv_smem_bytes(kHvMaxN));
         configured = true;
     }
-    hypervolume_kernel<<<1, kHvThreads, smem, static_cast<cudaStream_t>(stream)>>>(pts, keep, n, d, ref, out);
+    hypervolume_kernel<<<1, kHvThreads, hv_smem_bytes(n), static_cast<cudaStream_t>(stream)>>>(pts, keep, n, d, ref, out);
     return check_launch("morl_hypervolume_f64");
+}
+
+extern "C" int morl_hypervolume_batch_supported(int n, int d) {
+    const int cap = morl::hv_batch_cap(d);
+    return cap > 0 && n >= 0 && n <= cap ? 1 : 0;
+}
+
+extern "C" int morl_hypervolume_batch_f64(const double* base, int n_base, const double* cand, int n_cand, int d, const double* ref, double* out,
+                                          void* stream) {
+    using namespace morl;
+    MORL_REQUIRE(ref && out && (base || n_base == 0) && (cand || n_cand == 0), MORL_ERR_NULL, "morl_hypervolume_batch_f64: NULL pointer argument");
+    MORL_REQUIRE(n_base >= 0 && n_cand >= 0, MORL_ERR_SHAPE, "morl_hypervolume_batch_f64: bad shape n_base=%d n_cand=%d", n_base, n_cand);
+    MORL_REQUIRE(morl_hypervolume_batch_supported(n_base, d), MORL_ERR_UNSUPPORTED,
+                 "morl_hypervolume_batch_f64: supports 1 <= d <= 4 with at most %d (d <= 3) or %d (d = 4) base points (got d=%d, n_base=%d)",
+                 kHvMaxN, kHvMaxN4, d, n_base);
+    static bool configured = false;
+    if (!configured) {
+        cudaFuncSetAttribute(hypervolume_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hv_smem_bytes(kHvMaxN + 1));
+        configured = true;
+    }
+    const int n = n_base + (n_cand > 0 ? 1 : 0);
+    hypervolume_batch_kernel<<<n_cand > 0 ? n_cand : 1, kHvThreads, hv_smem_bytes(n), static_cast<cudaStream_t>(stream)>>>(
+        base, n_base, n_cand > 0 ? cand : nullptr, d, ref, out);
+    return check_launch("morl_hypervolume_batch_f64");
 }

@@ -2,7 +2,7 @@
 
     compute-sanitizer --tool memcheck|racecheck|synccheck|initcheck python scripts/sanitize_all.py [group ...]
 
-groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners ppo pcn eupg nl_ppo (default: all; dyna includes the fused Dyna commit).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
+groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners ppo pcn eupg nl_ppo hv_batch (default: all; dyna includes the fused Dyna commit).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
 every code path: all envelope kernel families, both GEMM operand formats x CTA modes x accumulator modes, MN split-K GEMM with the fused
 column sums, every split / reduction helper, the loss kernels (discrete SAC's included), Adam, polyak, Pareto + front records, replay gather,
 the corner-weight enumeration, MO-PPO's vector GAE and loss (racecheck: the loss kernel's CTA reductions), PCN's update and forward,
@@ -24,7 +24,7 @@ if os.environ.get("SAN_ZERO_PLANES") == "1":
     # from a genuine read of memory nobody wrote.
     _empty = ops.empty_planes
     ops.empty_planes = lambda *a, **k: _empty(*a, **k).zero_()
-groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain", "corners", "ppo", "pcn", "eupg", "nl_ppo"}
+groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain", "corners", "ppo", "pcn", "eupg", "nl_ppo", "hv_batch"}
 
 
 def rn(*s, scale=1.0):
@@ -300,4 +300,14 @@ if "nl_ppo" in groups:
                                  th.zeros(E, dtype=th.int32, device=dev))
     th.cuda.synchronize()
     print("nl_ppo ok")
+if "hv_batch" in groups:
+    # batched exact hypervolume (csrc/pareto.cu): every d, an empty base, base alone, one and several candidates, the d = 4 cap
+    from morl_baselines_b200 import hv_ops
+
+    for d, n_base, n_cand in [(1, 0, 3), (2, 17, 0), (3, 33, 5), (3, 2048, 1), (4, 9, 4), (4, 512, 1)]:
+        base = th.rand(n_base, d, device=dev, dtype=th.float64, generator=g)
+        cand = th.rand(n_cand, d, device=dev, dtype=th.float64, generator=g) if n_cand else None
+        hv_ops.hypervolume_batch(base, cand, th.zeros(d, device=dev, dtype=th.float64))
+    th.cuda.synchronize()
+    print("hv_batch ok")
 print("sanitize run ok")
