@@ -144,6 +144,36 @@ __device__ __forceinline__ void warp_argmax(float& v, int& i) {
     }
 }
 
+// ---- warp and block reductions (butterfly trees: every lane gets the same value) ------------------------------------------------
+__device__ __forceinline__ float warp_sum_f32(float v) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+    return v;
+}
+
+__device__ __forceinline__ float warp_max_f32(float v) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, off));
+    return v;
+}
+
+// Sum of one double per thread of a kThreads-thread block in a fixed order: the warp tree, then the warp sums in warp order.  `red`
+// holds kThreads / 32 doubles of shared memory; the first barrier frees it from a previous call.  Every thread gets the same value.
+template <int kThreads>
+__device__ __forceinline__ double block_sum_f64(double v, double* red) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double t = 0.0;
+#pragma unroll
+    for (int i = 0; i < kThreads / 32; ++i) t += red[i];
+    return t;
+}
+
+__device__ __forceinline__ float sigmoid_f32(float z) { return 1.0f / (1.0f + expf(-z)); }
+
 }  // namespace morl
 
 // Dispatch helpers: D in 1..8, dot mode in 0..2.

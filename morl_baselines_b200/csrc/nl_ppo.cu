@@ -13,13 +13,10 @@
 // morl_nl_ppo_commit_f32  : one rollout step's bookkeeping (nl_mo_ppo.py:251-275) for every environment in one launch
 //
 // The networks are tiny (hidden 64, K = S + d + Dp <= 256), so CUDA cores, activations in shared memory, no float atomics.
-#include "common.cuh"
+#include "tile_mlp.cuh"
 
 namespace morl {
 
-constexpr int kNlThreads = 256;
-constexpr int kNlWarps = kNlThreads / 32;
-constexpr int kNlRows = 16;     // rows per tile
 constexpr int kNlCtas = 128;    // CTAs of the update, whatever M and the card (the reduction order depends on it)
 constexpr int kNlHidden = 64;   // the reference Agent's hidden width
 constexpr int kNlMaxK = 256;    // S + d + Dp
@@ -27,134 +24,59 @@ constexpr int kNlMaxA = 32;
 constexpr int kNlMaxBatch = 4096;
 constexpr int kNlStats = MORL_MAX_D + 5;  // per CTA: pg sum per objective | value-loss sum | entropy | -logratio | kl | clipped rows
 
-#define MORL_NL_ROWS(i) _Pragma("unroll") for (int i = 0; i < kNlRows; ++i) if (i < rpj)
+using NlParams = ParamTable<12>;
+using NlGrads = GradTable<12>;
+using NlLayout = ParamLayout<12>;
 
 struct NlShape {
     int S, d, Dp, A;
     __host__ __device__ int K() const { return S + d + Dp; }
     // tensor t in the Agent's parameter order: critic W0 b0 W2 b2 W4 b4, then actor W0 b0 W2 b2 W4 b4
-    __host__ __device__ int size(int t) const {
-        const int l = (t % 6) >> 1;
-        const int out = l < 2 ? kNlHidden : (t < 6 ? d : A);
-        const int in = l == 0 ? K() : kNlHidden;
-        return (t & 1) ? out : out * in;
+    NlLayout layout() const {
+        NlLayout lay{12, {}};
+        for (int t = 0; t < 12; ++t) {
+            const int l = (t % 6) >> 1;
+            const int out = l < 2 ? kNlHidden : (t < 6 ? d : A);
+            const int in = l == 0 ? K() : kNlHidden;
+            lay.size[t] = (t & 1) ? out : out * in;
+        }
+        return lay;
     }
-    __host__ __device__ int offset(int t) const {
-        int o = 0;
-        for (int i = 0; i < t; ++i) o += size(i);
-        return o;
-    }
-    __host__ __device__ int total() const { return offset(12); }
-};
-
-struct NlParams {
-    const float* p[12];
-};
-struct NlGrads {
-    float* g[12];
 };
 
 // The activations of one tile in shared memory: input, both networks' hidden layers, outputs, and the backward's two buffers.
 struct NlTile {
-    float x[kNlRows * kNlMaxK];
-    float h1[2][kNlRows * kNlHidden];  // [0] critic, [1] actor
-    float h2[2][kNlRows * kNlHidden];
-    float z[kNlRows * kNlMaxA];        // logits, then d loss / d logits
-    float v[kNlRows * MORL_MAX_D];     // values, then d loss / d values
-    float dh[2][kNlRows * kNlHidden];
+    float x[kTileRows * kNlMaxK];
+    float h1[2][kTileRows * kNlHidden];  // [0] critic, [1] actor
+    float h2[2][kTileRows * kNlHidden];
+    float z[kTileRows * kNlMaxA];        // logits, then d loss / d logits
+    float v[kTileRows * MORL_MAX_D];     // values, then d loss / d values
+    float dh[2][kTileRows * kNlHidden];
 };
 
-// groups of rows per job for a layer with n outputs: the largest power of two <= 256 / n, at most kNlRows
-__device__ __forceinline__ int nl_groups(int n) {
-    int g = kNlThreads / n;
-    g = g > kNlRows ? kNlRows : g;
-    return 1 << (31 - __clz(g));
-}
-
-// out[r, j] = act(b[j] + sum_k W[j, k] in[r, k]) for the tile's rows.  Job (j, g) walks weight row j once and applies it to its rows.
-// Not inlined: the six layers of the update inlined with their unrolled row loops take 202 registers, called they take 80.
-__device__ __noinline__ void nl_linear(const float* __restrict__ W, const float* __restrict__ b, const float* in, int K, float* out, int N, bool tanh_act) {
-    const int groups = nl_groups(N), rpj = kNlRows / groups;
-    const int job = threadIdx.x;
-    if (job < N * groups) {
-        const int j = job % N, g = job / N;
-        float acc[kNlRows];
-        MORL_NL_ROWS(i) acc[i] = 0.f;
-        const float* wr = W + (size_t)j * K;
-        for (int k = 0; k < K; ++k) {
-            const float wv = __ldg(wr + k);
-            MORL_NL_ROWS(i) acc[i] = fmaf(wv, in[(g + groups * i) * K + k], acc[i]);
-        }
-        const float bj = __ldg(b + j);
-        MORL_NL_ROWS(i) {
-            const float v = acc[i] + bj;
-            out[(g + groups * i) * N + j] = tanh_act ? tanhf(v) : v;
-        }
-    }
-    __syncthreads();
-}
-
-// Network `net` (0 critic, 1 actor) on the staged tile; its outputs go to `out` [kNlRows, N].
+// Network `net` (0 critic, 1 actor) on the staged tile; its outputs go to `out` [kTileRows, N].
 __device__ void nl_forward(const NlParams& P, const NlShape& sh, NlTile& m, int net, float* out, int N) {
     const float* const* p = P.p + 6 * net;
-    nl_linear(p[0], p[1], m.x, sh.K(), m.h1[net], kNlHidden, true);
-    nl_linear(p[2], p[3], m.h1[net], kNlHidden, m.h2[net], kNlHidden, true);
-    nl_linear(p[4], p[5], m.h2[net], kNlHidden, out, N, false);
+    tile_linear(p[0], p[1], m.x, sh.K(), m.h1[net], kNlHidden, Act::Tanh);
+    tile_linear(p[2], p[3], m.h1[net], kNlHidden, m.h2[net], kNlHidden, Act::Tanh);
+    tile_linear(p[4], p[5], m.h2[net], kNlHidden, out, N, Act::None);
 }
 
-// Gradient of one Linear layer folded into the partial (init: first tile of the CTA), and, with `dnext`, the gradient w.r.t. its tanh
-// input a: dnext[r, k] = (sum_j W[j, k] dz[r, j]) (1 - a[r, k]^2).
-__device__ __noinline__ void nl_backward_layer(const float* __restrict__ W, const float* a, int K, const float* dz, int N, float* gw, float* gb, bool init,
-                                  float* dnext) {
-    for (int idx = threadIdx.x; idx < N * K; idx += kNlThreads) {
-        const int j = idx / K, k = idx % K;
-        float s = 0.f;
-#pragma unroll
-        for (int r = 0; r < kNlRows; ++r) s = fmaf(dz[r * N + j], a[r * K + k], s);
-        gw[idx] = init ? s : gw[idx] + s;
-    }
-    for (int j = threadIdx.x; j < N; j += kNlThreads) {
-        float s = 0.f;
-#pragma unroll
-        for (int r = 0; r < kNlRows; ++r) s += dz[r * N + j];
-        gb[j] = init ? s : gb[j] + s;
-    }
-    if (dnext) {
-        const int groups = nl_groups(K), rpj = kNlRows / groups;
-        const int job = threadIdx.x;
-        if (job < K * groups) {
-            const int k = job % K, g = job / K;
-            float s[kNlRows];
-            MORL_NL_ROWS(i) s[i] = 0.f;
-            for (int j = 0; j < N; ++j) {
-                const float wv = __ldg(W + (size_t)j * K + k);
-                MORL_NL_ROWS(i) s[i] = fmaf(wv, dz[(g + groups * i) * N + j], s[i]);
-            }
-            MORL_NL_ROWS(i) {
-                const int r = g + groups * i;
-                const float y = a[r * K + k];
-                dnext[r * K + k] = s[i] * (1.0f - y * y);
-            }
-        }
-    }
-    __syncthreads();
-}
-
-// Backward of network `net` from d loss / d outputs `dz` [kNlRows, N] (the tile's forward activations still in place).
-__device__ void nl_backward(const NlParams& P, const NlShape& sh, NlTile& m, int net, const float* dz, int N, float* part, bool init) {
+// Backward of network `net` from d loss / d outputs `dz` [kTileRows, N] (the tile's forward activations still in place).
+__device__ void nl_backward(const NlParams& P, const NlShape& sh, const NlLayout& lay, NlTile& m, int net, const float* dz, int N, float* g,
+                            bool init) {
     const int t0 = 6 * net;
-    float* g = part;
-    nl_backward_layer(P.p[t0 + 4], m.h2[net], kNlHidden, dz, N, g + sh.offset(t0 + 4), g + sh.offset(t0 + 5), init, m.dh[0]);
-    nl_backward_layer(P.p[t0 + 2], m.h1[net], kNlHidden, m.dh[0], kNlHidden, g + sh.offset(t0 + 2), g + sh.offset(t0 + 3), init, m.dh[1]);
-    nl_backward_layer(P.p[t0 + 0], m.x, sh.K(), m.dh[1], kNlHidden, g + sh.offset(t0 + 0), g + sh.offset(t0 + 1), init, nullptr);
+    tile_backward(P.p[t0 + 4], m.h2[net], kNlHidden, dz, N, g + lay.offset(t0 + 4), g + lay.offset(t0 + 5), init, m.dh[0], Act::Tanh);
+    tile_backward(P.p[t0 + 2], m.h1[net], kNlHidden, m.dh[0], kNlHidden, g + lay.offset(t0 + 2), g + lay.offset(t0 + 3), init, m.dh[1], Act::Tanh);
+    tile_backward(P.p[t0 + 0], m.x, sh.K(), m.dh[1], kNlHidden, g + lay.offset(t0 + 0), g + lay.offset(t0 + 1), init, nullptr, Act::Tanh);
 }
 
-// Stages rows [r0, r0 + kNlRows) as x = [obs || acc || pref], zero past n.  Row r reads source row src(r).
+// Stages rows [r0, r0 + kTileRows) as x = [obs || acc || pref], zero past n.  Row r reads source row src(r).
 template <typename Src>
 __device__ __forceinline__ void nl_stage(NlTile& m, const NlShape& sh, const float* obs, const float* acc, const float* __restrict__ pref, int r0,
                                          int n, Src src) {
     const int K = sh.K(), S = sh.S, d = sh.d;
-    for (int idx = threadIdx.x; idx < kNlRows * K; idx += kNlThreads) {
+    for (int idx = threadIdx.x; idx < kTileRows * K; idx += kTileThreads) {
         const int r = idx / K, k = idx % K, row = r0 + r;
         float v = 0.f;
         if (row < n) {
@@ -166,38 +88,14 @@ __device__ __forceinline__ void nl_stage(NlTile& m, const NlShape& sh, const flo
     __syncthreads();
 }
 
-__device__ __forceinline__ float nl_warp_max(float v) {
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, off));
-    return v;
-}
-__device__ __forceinline__ float nl_warp_sum(float v) {
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-    return v;
-}
-
-// Block-wide sum of one double per thread in a fixed order (the same value in every thread).
-__device__ __forceinline__ double nl_block_sum(double v, double* red) {
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-    __syncthreads();  // red is free
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double t = 0.0;
-#pragma unroll
-    for (int i = 0; i < kNlWarps; ++i) t += red[i];
-    return t;
-}
-
-__global__ void __launch_bounds__(kNlThreads) nl_update_kernel(
-    const __grid_constant__ NlParams P, const __grid_constant__ NlShape sh, const float* __restrict__ obs, const float* __restrict__ acc,
+__global__ void __launch_bounds__(kTileThreads) nl_update_kernel(
+    const __grid_constant__ NlParams P, const __grid_constant__ NlShape sh, const __grid_constant__ NlLayout lay, const float* __restrict__ obs, const float* __restrict__ acc,
     const int64_t* __restrict__ actions, const float* __restrict__ old_logp, const float* __restrict__ adv, const float* __restrict__ ret,
     const float* __restrict__ old_v, const int64_t* __restrict__ perm, int M, const float* __restrict__ pref, const float* __restrict__ w,
     float clip_coef, float ent_coef, float vf_coef, int norm_adv, int clip_vloss, float* __restrict__ part, double* __restrict__ stat_part) {
     __shared__ NlTile m;
-    __shared__ double red[kNlWarps];
-    __shared__ double red_lane[kNlWarps][32];
+    __shared__ double red[kTileWarps];
+    __shared__ double red_lane[kTileWarps][32];
     __shared__ float s_mu[MORL_MAX_D], s_den[MORL_MAX_D], s_w[MORL_MAX_D];
     const int d = sh.d, A = sh.A;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -211,14 +109,14 @@ __global__ void __launch_bounds__(kNlThreads) nl_update_kernel(
     if (norm_adv) {
         for (int o = 0; o < d; ++o) {
             double s = 0.0;
-            for (int i = threadIdx.x; i < M; i += kNlThreads) s += (double)__ldg(adv + (size_t)__ldg(perm + i) * d + o);
-            const double mean = nl_block_sum(s, red) / (double)M;
+            for (int i = threadIdx.x; i < M; i += kTileThreads) s += (double)__ldg(adv + (size_t)__ldg(perm + i) * d + o);
+            const double mean = block_sum_f64<kTileThreads>(s, red) / (double)M;
             double s2 = 0.0;
-            for (int i = threadIdx.x; i < M; i += kNlThreads) {
+            for (int i = threadIdx.x; i < M; i += kTileThreads) {
                 const double c = (double)__ldg(adv + (size_t)__ldg(perm + i) * d + o) - mean;
                 s2 += c * c;
             }
-            const double var = nl_block_sum(s2, red) / (double)(M - 1);
+            const double var = block_sum_f64<kTileThreads>(s2, red) / (double)(M - 1);
             if (threadIdx.x == 0) {
                 s_mu[o] = (float)mean;
                 s_den[o] = __fadd_rn((float)sqrt(var), 1e-8f);
@@ -227,11 +125,10 @@ __global__ void __launch_bounds__(kNlThreads) nl_update_kernel(
     }
     __syncthreads();
 
-    const int n_all = (M + kNlRows - 1) / kNlRows;
-    const int q = n_all / kNlCtas, rem = n_all % kNlCtas;
     const int c = blockIdx.x;
-    const int first = c * q + min(c, rem), count = q + (c < rem ? 1 : 0);
-    float* out = part + (size_t)c * sh.total();
+    int first, count;
+    tile_range((M + kTileRows - 1) / kTileRows, c, first, count);
+    float* out = part + (size_t)c * lay.total();
     const float inv_m = 1.0f / (float)M;
     const float g_v = (float)(0.5 / ((double)M * d)) * vf_coef;
     const float g_ent = __fmul_rn(ent_coef, inv_m);
@@ -241,23 +138,23 @@ __global__ void __launch_bounds__(kNlThreads) nl_update_kernel(
 
     for (int tile = first; tile < first + count; ++tile) {
         const bool init = tile == first;
-        const int r0 = tile * kNlRows;
+        const int r0 = tile * kTileRows;
         nl_stage(m, sh, obs, acc, pref, r0, M, [&](int row) { return (size_t)__ldg(perm + row); });
         nl_forward(P, sh, m, 0, m.v, d);
         nl_forward(P, sh, m, 1, m.z, A);
 
         // one warp per row; lane a holds logit a, lane o objective o
-        for (int r = warp; r < kNlRows; r += kNlWarps) {
+        for (int r = warp; r < kTileRows; r += kTileWarps) {
             const int row = r0 + r;
             const bool valid = row < M;
             const size_t src = valid ? (size_t)__ldg(perm + row) : 0;
             const float z = lane < A ? m.z[r * A + lane] : -INFINITY;
-            const float mx = nl_warp_max(z);
+            const float mx = warp_max_f32(z);
             const float e = lane < A ? expf(__fsub_rn(z, mx)) : 0.f;
-            const float lse = __fadd_rn(logf(nl_warp_sum(e)), mx);
+            const float lse = __fadd_rn(logf(warp_sum_f32(e)), mx);
             const float l = __fsub_rn(z, lse);  // log-probability of action `lane`
             const float p = lane < A ? expf(l) : 0.f;
-            const float ent = -nl_warp_sum(lane < A ? __fmul_rn(l, p) : 0.f);
+            const float ent = -warp_sum_f32(lane < A ? __fmul_rn(l, p) : 0.f);
             const int a = valid ? (int)__ldg(actions + src) : 0;
             const float logratio = __fsub_rn(__shfl_sync(0xffffffffu, l, a & 31), valid ? __ldg(old_logp + src) : 0.f);
             const float ratio = expf(logratio);
@@ -291,7 +188,7 @@ __global__ void __launch_bounds__(kNlThreads) nl_update_kernel(
                 }
                 dv = __fmul_rn(g_v, g);
             }
-            const float dlp = __fmul_rn(nl_warp_sum(dratio_o), ratio);  // d loss / d log p_a
+            const float dlp = __fmul_rn(warp_sum_f32(dratio_o), ratio);  // d loss / d log p_a
             if (valid && lane == 0) {
                 ent_acc += (double)ent;
                 okl_acc += (double)(-logratio);
@@ -305,8 +202,8 @@ __global__ void __launch_bounds__(kNlThreads) nl_update_kernel(
             if (lane < d) m.v[r * d + lane] = dv;
         }
         __syncthreads();
-        nl_backward(P, sh, m, 1, m.z, A, out, init);
-        nl_backward(P, sh, m, 0, m.v, d, out, init);
+        nl_backward(P, sh, lay, m, 1, m.z, A, out, init);
+        nl_backward(P, sh, lay, m, 0, m.v, d, out, init);
     }
 
     // statistics partial of this CTA, summed over its warps in order
@@ -315,14 +212,14 @@ __global__ void __launch_bounds__(kNlThreads) nl_update_kernel(
     double* sp = stat_part + (size_t)c * kNlStats;
     if (threadIdx.x < d) {
         double t = 0.0;
-        for (int i = 0; i < kNlWarps; ++i) t += red_lane[i][threadIdx.x];
+        for (int i = 0; i < kTileWarps; ++i) t += red_lane[i][threadIdx.x];
         sp[threadIdx.x] = t;
     }
-    const double vs = nl_block_sum(v_acc, red);
-    const double es = nl_block_sum(ent_acc, red);
-    const double os = nl_block_sum(okl_acc, red);
-    const double ks = nl_block_sum(kl_acc, red);
-    const double cs = nl_block_sum(clip_acc, red);
+    const double vs = block_sum_f64<kTileThreads>(v_acc, red);
+    const double es = block_sum_f64<kTileThreads>(ent_acc, red);
+    const double os = block_sum_f64<kTileThreads>(okl_acc, red);
+    const double ks = block_sum_f64<kTileThreads>(kl_acc, red);
+    const double cs = block_sum_f64<kTileThreads>(clip_acc, red);
     if (threadIdx.x == 0) {
         sp[MORL_MAX_D + 0] = vs;
         sp[MORL_MAX_D + 1] = es;
@@ -332,74 +229,61 @@ __global__ void __launch_bounds__(kNlThreads) nl_update_kernel(
     }
 }
 
-// Fixed-order sum of the CTAs' partials into the .grad storages; block 0 also finishes the loss and the statistics.
-__global__ void __launch_bounds__(kNlThreads) nl_reduce_kernel(const __grid_constant__ NlGrads G, const __grid_constant__ NlShape sh,
-                                                               const float* __restrict__ part, const double* __restrict__ stat_part, int n_parts,
-                                                               int M, const float* __restrict__ w, float ent_coef, float vf_coef,
-                                                               float* __restrict__ loss_out, float* __restrict__ stats) {
-    const int total = sh.total();
-    int off = 0;
-#pragma unroll
-    for (int t = 0; t < 12; ++t) {  // unrolled: G.g[t] stays a kernel parameter, not a stack array
-        const int n = sh.size(t);
-        for (int q = blockIdx.x * kNlThreads + threadIdx.x; q < n; q += gridDim.x * kNlThreads) {
-            float s = 0.f;
-            for (int c = 0; c < n_parts; ++c) s += __ldg(part + (size_t)c * total + off + q);
-            G.g[t][q] = s;
+// Block 0 of the partial sum: the loss and the statistics from the CTAs' statistics partials.
+struct NlFinish {
+    const double* stat_part;
+    int M, d;
+    const float* w;
+    float ent_coef, vf_coef;
+    float* loss_out;
+    float* stats;
+    __device__ void operator()(int n_parts) const {
+        __shared__ double acc[kNlStats];
+        if (threadIdx.x < kNlStats) {
+            double t = 0.0;
+            for (int c = 0; c < n_parts; ++c) t += stat_part[(size_t)c * kNlStats + threadIdx.x];
+            acc[threadIdx.x] = t;
         }
-        off += n;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            const double inv_m = 1.0 / (double)M;
+            float pg = 0.f;  // (per-objective mean surrogate * w).sum()
+            for (int o = 0; o < d; ++o) pg = __fadd_rn(pg, __fmul_rn((float)(acc[o] * inv_m), __ldg(w + o)));
+            const float v = (float)(0.5 * acc[MORL_MAX_D] / ((double)M * d));
+            const float ent = (float)(acc[MORL_MAX_D + 1] * inv_m);
+            if (loss_out) loss_out[0] = __fadd_rn(__fsub_rn(pg, __fmul_rn(ent_coef, ent)), __fmul_rn(vf_coef, v));
+            stats[0] = pg;
+            stats[1] = v;
+            stats[2] = ent;
+            stats[3] = (float)(acc[MORL_MAX_D + 2] * inv_m);
+            stats[4] = (float)(acc[MORL_MAX_D + 3] * inv_m);
+            stats[5] = __fadd_rn(stats[5], (float)(acc[MORL_MAX_D + 4] * inv_m));
+        }
     }
-    if (blockIdx.x != 0) return;
-    __shared__ double acc[kNlStats];
-    if (threadIdx.x < kNlStats) {
-        double t = 0.0;
-        for (int c = 0; c < n_parts; ++c) t += stat_part[(size_t)c * kNlStats + threadIdx.x];
-        acc[threadIdx.x] = t;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        const double inv_m = 1.0 / (double)M;
-        float pg = 0.f;  // (per-objective mean surrogate * w).sum()
-        for (int o = 0; o < sh.d; ++o) pg = __fadd_rn(pg, __fmul_rn((float)(acc[o] * inv_m), __ldg(w + o)));
-        const float v = (float)(0.5 * acc[MORL_MAX_D] / ((double)M * sh.d));
-        const float ent = (float)(acc[MORL_MAX_D + 1] * inv_m);
-        if (loss_out) loss_out[0] = __fadd_rn(__fsub_rn(pg, __fmul_rn(ent_coef, ent)), __fmul_rn(vf_coef, v));
-        stats[0] = pg;
-        stats[1] = v;
-        stats[2] = ent;
-        stats[3] = (float)(acc[MORL_MAX_D + 2] * inv_m);
-        stats[4] = (float)(acc[MORL_MAX_D + 3] * inv_m);
-        stats[5] = __fadd_rn(stats[5], (float)(acc[MORL_MAX_D + 4] * inv_m));
-    }
-}
+};
 
 // Both networks (as asked) on N rows [obs || acc || pref]; obs, acc and the outputs may live in mapped pinned host memory.
-__global__ void __launch_bounds__(kNlThreads) nl_forward_kernel(const __grid_constant__ NlParams P, const __grid_constant__ NlShape sh,
+__global__ void __launch_bounds__(kTileThreads) nl_forward_kernel(const __grid_constant__ NlParams P, const __grid_constant__ NlShape sh,
                                                                 const float* obs, const float* acc, const float* __restrict__ pref, int N,
                                                                 float* logits, float* values, int32_t* argmax) {
     __shared__ NlTile m;
-    const int r0 = blockIdx.x * kNlRows;
-    const int nr = min(kNlRows, N - r0);
+    const int r0 = blockIdx.x * kTileRows;
+    const int nr = min(kTileRows, N - r0);
     const int d = sh.d, A = sh.A;
     nl_stage(m, sh, obs, acc, pref, r0, N, [](int row) { return (size_t)row; });
     if (values) {
         nl_forward(P, sh, m, 0, m.v, d);
-        for (int idx = threadIdx.x; idx < nr * d; idx += kNlThreads) values[(size_t)r0 * d + idx] = m.v[idx];
+        for (int idx = threadIdx.x; idx < nr * d; idx += kTileThreads) values[(size_t)r0 * d + idx] = m.v[idx];
     }
     if (logits || argmax) {
         nl_forward(P, sh, m, 1, m.z, A);
-        for (int idx = threadIdx.x; logits && idx < nr * A; idx += kNlThreads) logits[(size_t)r0 * A + idx] = m.z[idx];
+        for (int idx = threadIdx.x; logits && idx < nr * A; idx += kTileThreads) logits[(size_t)r0 * A + idx] = m.z[idx];
         const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-        for (int r = warp; argmax && r < nr; r += kNlWarps) {
+        for (int r = warp; argmax && r < nr; r += kTileWarps) {
             // first occurrence of the row maximum (torch.argmax)
             float best = lane < A ? m.z[r * A + lane] : -INFINITY;
             int bi = lane < A ? lane : kNlMaxA;
-#pragma unroll
-            for (int off = 16; off > 0; off >>= 1) {
-                const float ob = __shfl_xor_sync(0xffffffffu, best, off);
-                const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
-                if (ob > best || (ob == best && oi < bi)) best = ob, bi = oi;
-            }
+            warp_argmax(best, bi);
             if (lane == 0) argmax[r0 + r] = bi;
         }
     }
@@ -468,7 +352,7 @@ extern "C" size_t morl_nl_ppo_workspace_bytes(int obs_dim, int d, int pref_dim, 
     using namespace morl;
     NlShape sh;
     if (!nl_shape(obs_dim, d, pref_dim, n_actions, &sh)) return 0;
-    return (size_t)kNlCtas * kNlStats * sizeof(double) + (size_t)kNlCtas * (size_t)sh.total() * sizeof(float);
+    return (size_t)kNlCtas * kNlStats * sizeof(double) + (size_t)kNlCtas * (size_t)sh.layout().total() * sizeof(float);
 }
 
 extern "C" int morl_nl_ppo_update_f32(const float* const* params, float* const* grads, const float* obs, const float* acc, const int64_t* actions,
@@ -488,19 +372,15 @@ extern "C" int morl_nl_ppo_update_f32(const float* const* params, float* const* 
     MORL_REQUIRE(!norm_adv || M >= 2, MORL_ERR_SHAPE, "morl_nl_ppo_update_f32: advantage normalisation needs M >= 2 rows (unbiased std), got M=%d", M);
     NlParams P;
     NlGrads G;
-    for (int t = 0; t < 12; ++t) {
-        MORL_REQUIRE(params[t] && grads[t], MORL_ERR_NULL, "morl_nl_ppo_update_f32: NULL parameter or gradient pointer %d", t);
-        P.p[t] = params[t];
-        G.g[t] = grads[t];
-    }
-    const int ctas = min(kNlCtas, (M + kNlRows - 1) / kNlRows);
+    if (int rc = load_tables("morl_nl_ppo_update_f32", 12, params, P, grads, &G)) return rc;
+    const NlLayout lay = sh.layout();
+    const int ctas = min(kNlCtas, (M + kTileRows - 1) / kTileRows);
     double* stat_part = static_cast<double*>(workspace);
     float* part = reinterpret_cast<float*>(stat_part + (size_t)kNlCtas * kNlStats);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    nl_update_kernel<<<ctas, kNlThreads, 0, st>>>(P, sh, obs, acc, actions, old_logprob, advantages, returns, old_values, perm, M, pref, loss_weights,
+    nl_update_kernel<<<ctas, kTileThreads, 0, st>>>(P, sh, lay, obs, acc, actions, old_logprob, advantages, returns, old_values, perm, M, pref, loss_weights,
                                                   clip_coef, ent_coef, vf_coef, norm_adv ? 1 : 0, clip_vloss ? 1 : 0, part, stat_part);
-    const int rblocks = min((sh.total() + kNlThreads - 1) / kNlThreads, 4 * sm_count());
-    nl_reduce_kernel<<<rblocks, kNlThreads, 0, st>>>(G, sh, part, stat_part, ctas, M, loss_weights, ent_coef, vf_coef, loss_out, stats);
+    launch_partial_sum(G, lay, part, ctas, NlFinish{stat_part, M, d, loss_weights, ent_coef, vf_coef, loss_out, stats}, st);
     return check_launch("morl_nl_ppo_update_f32");
 }
 
@@ -514,11 +394,8 @@ extern "C" int morl_nl_ppo_forward_f32(const float* const* params, const float* 
     MORL_REQUIRE(nl_shape(obs_dim, d, pref_dim, n_actions, &sh), MORL_ERR_UNSUPPORTED,
                  "morl_nl_ppo_forward_f32: unsupported configuration S=%d d=%d Dp=%d A=%d (morl_nl_ppo_supported)", obs_dim, d, pref_dim, n_actions);
     NlParams P;
-    for (int t = 0; t < 12; ++t) {
-        MORL_REQUIRE(params[t], MORL_ERR_NULL, "morl_nl_ppo_forward_f32: NULL parameter pointer %d", t);
-        P.p[t] = params[t];
-    }
-    nl_forward_kernel<<<(N + kNlRows - 1) / kNlRows, kNlThreads, 0, static_cast<cudaStream_t>(stream)>>>(P, sh, obs, acc, pref, N, logits, values,
+    if (int rc = load_tables("morl_nl_ppo_forward_f32", 12, params, P)) return rc;
+    nl_forward_kernel<<<(N + kTileRows - 1) / kTileRows, kTileThreads, 0, static_cast<cudaStream_t>(stream)>>>(P, sh, obs, acc, pref, N, logits, values,
                                                                                                          argmax_out);
     return check_launch("morl_nl_ppo_forward_f32");
 }

@@ -98,19 +98,6 @@ constexpr int kPpoThreads = 256;
 constexpr int kPpoMaxA = 32;
 constexpr float kHalfLog2Pi = 0.918938533204672742f;  // 0.5 * log(2 pi)
 
-__device__ __forceinline__ double ppo_block_sum(double v, double* red) {
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    __syncthreads();  // red is free (its previous use has been read by every thread)
-    if (lane == 0) red[warp] = v;
-    __syncthreads();
-    double t = 0.0;
-#pragma unroll
-    for (int i = 0; i < kPpoThreads / 32; ++i) t += red[i];
-    return t;  // the same value in every thread
-}
-
 // Normal(mean, exp(logstd)).log_prob(action).sum(-1) for one row
 __device__ __forceinline__ float row_logprob(const float* __restrict__ mean, const float* __restrict__ act, const float* s_ls,
                                              const float* s_ivar, int A) {
@@ -150,10 +137,10 @@ __global__ void __launch_bounds__(kPpoThreads) ppo_loss_kernel(const float* __re
         s_kl += (double)__fsub_rn(__fsub_rn(ratio, 1.0f), lr);
         s_clip += (fabsf(__fsub_rn(ratio, 1.0f)) > clip_coef) ? 1.0 : 0.0;
     }
-    const double adv_mean = ppo_block_sum(s_adv, red) * inv_m;
-    const double okl = ppo_block_sum(s_okl, red) * inv_m;
-    const double kl = ppo_block_sum(s_kl, red) * inv_m;
-    const double clipfrac = ppo_block_sum(s_clip, red) * inv_m;
+    const double adv_mean = block_sum_f64<kPpoThreads>(s_adv, red) * inv_m;
+    const double okl = block_sum_f64<kPpoThreads>(s_okl, red) * inv_m;
+    const double kl = block_sum_f64<kPpoThreads>(s_kl, red) * inv_m;
+    const double clipfrac = block_sum_f64<kPpoThreads>(s_clip, red) * inv_m;
 
     // pass 2: unbiased standard deviation (torch's Tensor.std())
     float a_mu = 0.f, a_den = 1.f;
@@ -163,7 +150,7 @@ __global__ void __launch_bounds__(kPpoThreads) ppo_loss_kernel(const float* __re
             const double c = (double)__ldg(advantages + i) - adv_mean;
             s2 += c * c;
         }
-        const double var = ppo_block_sum(s2, red) / (double)(M - 1);
+        const double var = block_sum_f64<kPpoThreads>(s2, red) / (double)(M - 1);
         a_mu = (float)adv_mean;
         a_den = __fadd_rn((float)sqrt(var), 1e-8f);
     }
@@ -224,15 +211,15 @@ __global__ void __launch_bounds__(kPpoThreads) ppo_loss_kernel(const float* __re
             dvalue[k] = __fmul_rn(g_v, g);
         }
     }
-    const float pg_loss = (float)(ppo_block_sum(s_pg, red) * inv_m);
-    const float v_loss = (float)(0.5 * ppo_block_sum(s_v, red) / ((double)M * D));
+    const float pg_loss = (float)(block_sum_f64<kPpoThreads>(s_pg, red) * inv_m);
+    const float v_loss = (float)(0.5 * block_sum_f64<kPpoThreads>(s_v, red) / ((double)M * D));
     // Normal entropy summed over action dims (the same for every row): sum_j 0.5 + 0.5 log(2 pi) + logstd_j
     float ent = 0.f;
     for (int j = 0; j < A; ++j) ent = __fadd_rn(ent, __fadd_rn(0.5f + kHalfLog2Pi, s_ls[j]));
 #pragma unroll
     for (int j = 0; j < kPpoMaxA; ++j) {
         if (j < A) {  // uniform across the CTA
-            const double sj = ppo_block_sum(acc[j], red);
+            const double sj = block_sum_f64<kPpoThreads>(acc[j], red);
             if (threadIdx.x == 0) dlogstd[j] = __fsub_rn((float)sj, ent_coef);
         }
     }

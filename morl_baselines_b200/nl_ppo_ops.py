@@ -12,7 +12,7 @@ from typing import Optional
 import torch as th
 
 from . import _lib
-from .ops import _Args, _launch, _pointer_table
+from .ops import _Args, _launch, _param_table, _workspace
 
 N_TENSORS = 12
 N_STATS = 6  # pg_loss, v_loss, entropy, old_approx_kl, approx_kl, clip-fraction sum
@@ -35,22 +35,16 @@ class NlPpoNet:
             a.fail("shape", f"is unsupported: obs_dim={obs_dim} d={d} pref_dim={pref_dim} n_actions={n_actions}")
         K, H = self.obs_dim + self.d + self.pref_dim, 64
         self.shapes = [(H, K), (H,), (H, H), (H,), (self.d, H), (self.d,), (H, K), (H,), (H, H), (H,), (self.n_actions, H), (self.n_actions,)]
-        self.params = self._table(a, params, "params")
-        self.grads = None if grads is None else self._table(a, grads, "grads")
+        self.params = _param_table(a, params, "params", N_TENSORS, "tensors of the Agent", self.shapes)
+        self.grads = None if grads is None else _param_table(a, grads, "grads", N_TENSORS, "tensors of the Agent", self.shapes)
         self.pref = a.inp(pref, "pref", (self.pref_dim,), inplace=True) if self.pref_dim else None
-
-    def _table(self, a, tensors, what):
-        ts = list(tensors)
-        if len(ts) != N_TENSORS:
-            a.fail(what, f"must hold the {N_TENSORS} tensors of the Agent, got {len(ts)}")
-        return _pointer_table([a.inp(t, f"{what}[{i}]", s, inplace=True) for i, (t, s) in enumerate(zip(ts, self.shapes))])
 
     @property
     def workspace_bytes(self) -> int:
         return int(_lib.load().morl_nl_ppo_workspace_bytes(self.obs_dim, self.d, self.pref_dim, self.n_actions))
 
     def workspace(self, device) -> th.Tensor:
-        return th.empty((self.workspace_bytes + 7) // 8, device=device, dtype=th.float64)
+        return _workspace(self.workspace_bytes, device)
 
 
 def vector_gae_objectives(rewards, values, dones, next_value, next_done, gamma: float, gae_lambda: float,

@@ -55,6 +55,20 @@ def _pointer_table(tensors):
     return (ctypes.c_void_p * max(1, len(tensors)))(*[None if t is None else t.data_ptr() for t in tensors])
 
 
+def _param_table(a, tensors, what: str, count: int, holds: str, shapes=None):
+    """Pointer table of the ``count`` parameter (or gradient) tensors of one network, each checked as an in-place input ``what[i]`` of
+    ``shapes[i]`` (any shape when None); ``holds`` names them in the error for a wrong count."""
+    ts = list(tensors)
+    if len(ts) != count:
+        a.fail(what, f"must hold the {count} {holds}, got {len(ts)}")
+    return _pointer_table([a.inp(t, f"{what}[{i}]", None if shapes is None else shapes[i], inplace=True) for i, t in enumerate(ts)])
+
+
+def _workspace(nbytes: int, device) -> th.Tensor:
+    """A workspace of ``nbytes`` (the library's count) on ``device``, 8-byte aligned for the double partials the kernels keep in it."""
+    return th.empty((nbytes + 7) // 8, device=device, dtype=th.float64)
+
+
 class _Args:
     """The argument contract of one binding call.  Each check raises MorlB200Error naming the binding and the argument:
 
@@ -1007,15 +1021,12 @@ def _pcn_workspace_bytes(obs_dim: int, d: int, hidden: int, n_out: int, batch: i
 
 
 def pcn_workspace(obs_dim: int, d: int, hidden: int, n_out: int, batch: int, device) -> th.Tensor:
-    return th.empty((_pcn_workspace_bytes(obs_dim, d, hidden, n_out, batch) + 7) // 8, device=device, dtype=th.float64)
+    return _workspace(_pcn_workspace_bytes(obs_dim, d, hidden, n_out, batch), device)
 
 
 def pcn_pointer_table(tensors) -> "ctypes.Array":
     """Host array of the 8 device pointers (Ls, bs, Lc, bc, W1, b1, W2, b2) the PCN kernels take; build it once per set of storages."""
-    a, ts = _Args("pcn_pointer_table"), list(tensors)
-    if len(ts) != 8:
-        a.fail("tensors", f"must hold the 8 parameter tensors of the PCN kernels, got {len(ts)}")
-    return _pointer_table([a.inp(t, f"tensors[{i}]", inplace=True) for i, t in enumerate(ts)])
+    return _param_table(_Args("pcn_pointer_table"), tensors, "tensors", 8, "parameter tensors of the PCN kernels")
 
 
 def pcn_update(params, grads, scaling: th.Tensor, store: th.Tensor, obs_dim: int, d: int, rows: th.Tensor, horizons: th.Tensor, batch: int,
@@ -1076,21 +1087,16 @@ class EupgNet:
         a = _Args("EupgNet")
         if not _lib.load().morl_eupg_supported(self.obs_dim, self.d, self.hidden, self.n_hidden, self.n_out):
             a.fail("hidden", f"is an unsupported configuration obs_dim={obs_dim} d={d} hidden={list(hidden)} n_out={n_out}")
-        self.params = self._table(a, params, "params")
-        self.grads = None if grads is None else self._table(a, grads, "grads")
-
-    def _table(self, a, tensors, what):
-        ts = list(tensors)
-        if len(ts) != 2 * (self.n_hidden + 1):
-            a.fail(what, f"must hold the {2 * (self.n_hidden + 1)} tensors of the EUPG kernels, got {len(ts)}")
-        return _pointer_table([a.inp(t, f"{what}[{i}]", inplace=True) for i, t in enumerate(ts)])
+        n = 2 * (self.n_hidden + 1)
+        self.params = _param_table(a, params, "params", n, "tensors of the EUPG kernels")
+        self.grads = None if grads is None else _param_table(a, grads, "grads", n, "tensors of the EUPG kernels")
 
     @property
     def workspace_bytes(self) -> int:
         return int(_lib.load().morl_eupg_workspace_bytes(self.obs_dim, self.d, self.hidden, self.n_hidden, self.n_out))
 
     def workspace(self, device) -> th.Tensor:
-        return th.empty((self.workspace_bytes + 7) // 8, device=device, dtype=th.float64)
+        return _workspace(self.workspace_bytes, device)
 
 
 def eupg_workspace_bytes(obs_dim: int, d: int, hidden, n_out: int) -> int:
