@@ -282,6 +282,35 @@ MORL_API int morl_hypervolume_batch_supported(int n, int d);
 MORL_API int morl_hypervolume_batch_f64(const double* base, int n_base, const double* cand, int n_cand, int d, const double* ref, double* out,
                                         void* stream);
 
+/* Pareto Q-learning's set table (multi_policy/pareto_q_learning/pql.py), caller-owned device tensors for S states, A actions, set
+ * capacity K and d objectives:  nd f64 [S, A, K, d] and nd_count int32 [S, A] (the stored set ND[s][a]: its first nd_count rows; start
+ * with count 1 and the zero vector), avg_reward f64 [S, A, d], counts f64 [S, A], status int32 [3] (zeroed by the caller).
+ * Q-set(s, a) = { avg_reward[s, a] + gamma * v : v in ND[s][a] }, each coordinate rounded as numpy does (gamma * v, then the add).
+ * morl_pql_update_f64 : one reference step (pql.py:260-262), one CTA:  counts[s, a] += 1;  ND[s][a] = ND(U_a' Q-set(s_next, a'));
+ *   avg_reward[s, a] += (reward - avg_reward[s, a]) / counts[s, a] (subtract, divide, add: one IEEE operation each).  ND keeps a point
+ *   iff no distinct point is >= it in every coordinate, and one copy of equal points (within and across actions).  The set is stored in
+ *   canonical order: descending coordinate sum (added left to right), ties lexicographically descending, so equal sets are equal bytes.
+ *   The union is staged on chip before anything is written, so s_next == s is safe.  If more than K points survive, nothing is written
+ *   but status: { needed size, s, a } when status[0] was 0 (the first overflow is kept).  reward: HOST pointer to d doubles, passed to
+ *   the kernel by value (no copy to the device).  s, s_next in [0, S), a in [0, A), else MORL_ERR_SHAPE.
+ * morl_pql_score_f64 : scores f64 [A] of `state`, one CTA per action.
+ *   mode MORL_PQL_HYPERVOLUME (pql.py:143-154): scores[a] = exact volume of Q-set(state, a) above ref (HOST pointer to d doubles, passed
+ *     by value), counted as morl_hypervolume_batch_f64 counts it: a point that does not exceed ref in every objective spans nothing.  Equal
+ *     sets give bit-identical volumes.
+ *   mode MORL_PQL_CARDINALITY (pql.py:122-141): scores[a] = number of points of ND(U_a' Q-set(state, a')) equal to a point of
+ *     Q-set(state, a) (a point shared by several actions counts for each); ref may be NULL.
+ *   Integer counts and fixed-shape reductions: no atomics, results do not depend on the grid.
+ * Supported range (morl_pql_supported, no device needed: 1 if supported, else 0): 1 <= A <= 16, 1 <= K <= 256, A * K <= 2048 and
+ *   1 <= d <= MORL_MAX_D, with d <= 4 for MORL_PQL_HYPERVOLUME; the update needs the MORL_PQL_CARDINALITY range.  Anything else returns
+ *   MORL_ERR_UNSUPPORTED. */
+#define MORL_PQL_HYPERVOLUME 0
+#define MORL_PQL_CARDINALITY 1
+MORL_API int morl_pql_supported(int n_actions, int cap, int d, int mode);
+MORL_API int morl_pql_update_f64(double* nd, int* nd_count, double* avg_reward, double* counts, int* status, int S, int A, int K, int d, int s,
+                                 int a, int s_next, double gamma, const double* reward, void* stream);
+MORL_API int morl_pql_score_f64(const double* nd, const int* nd_count, const double* avg_reward, int S, int A, int K, int d, int state,
+                                double gamma, int mode, const double* ref, double* scores, void* stream);
+
 /* Corner weights of a convex coverage set (OLS / GPI-LS weight selection).  Replaces compute_corner_weights
  * (multi_policy/linear_support/linear_support.py:295-349), which enumerates with cdd the vertices of
  *   { (w, u) : V w <= u 1,  w >= 0,  sum w = 1 }.

@@ -41,6 +41,16 @@ class MultiBinary(_Space):
         return self._rng.integers(0, 2, size=self.n)
 
 
+class MultiDiscrete(_Space):
+    def __init__(self, nvec):
+        super().__init__()
+        self.nvec = np.asarray(nvec, dtype=np.int64)
+        self.shape = self.nvec.shape
+
+    def sample(self):
+        return self._rng.integers(0, self.nvec)
+
+
 class Box(_Space):
     def __init__(self, low=-1.0, high=1.0, shape=None, dtype=np.float32):
         super().__init__()
@@ -50,6 +60,10 @@ class Box(_Space):
         self.low = np.broadcast_to(np.asarray(low, dtype=dtype), self.shape).copy()
         self.high = np.broadcast_to(np.asarray(high, dtype=dtype), self.shape).copy()
         self.dtype = dtype
+
+    def is_bounded(self, manner="both"):
+        below, above = bool(np.all(np.isfinite(self.low))), bool(np.all(np.isfinite(self.high)))
+        return {"both": below and above, "below": below, "above": above}[manner]
 
     def sample(self):
         if not (np.all(np.isfinite(self.low)) and np.all(np.isfinite(self.high))):

@@ -2,7 +2,7 @@
 
     compute-sanitizer --tool memcheck|racecheck|synccheck|initcheck python scripts/sanitize_all.py [group ...]
 
-groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners ppo pcn eupg nl_ppo hv_batch (default: all; dyna includes the fused Dyna commit).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
+groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners ppo pcn eupg nl_ppo hv_batch pql (default: all; dyna includes the fused Dyna commit).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
 every code path: all envelope kernel families, both GEMM operand formats x CTA modes x accumulator modes, MN split-K GEMM with the fused
 column sums, every split / reduction helper, the loss kernels (discrete SAC's included), Adam, polyak, Pareto + front records, replay gather,
 the corner-weight enumeration, MO-PPO's vector GAE and loss (racecheck: the loss kernel's CTA reductions), PCN's update and forward,
@@ -24,7 +24,7 @@ if os.environ.get("SAN_ZERO_PLANES") == "1":
     # from a genuine read of memory nobody wrote.
     _empty = ops.empty_planes
     ops.empty_planes = lambda *a, **k: _empty(*a, **k).zero_()
-groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain", "corners", "ppo", "pcn", "eupg", "nl_ppo", "hv_batch"}
+groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain", "corners", "ppo", "pcn", "eupg", "nl_ppo", "hv_batch", "pql"}
 
 
 def rn(*s, scale=1.0):
@@ -310,4 +310,20 @@ if "hv_batch" in groups:
         hv_ops.hypervolume_batch(base, cand, th.zeros(d, device=dev, dtype=th.float64))
     th.cuda.synchronize()
     print("hv_batch ok")
+if "pql" in groups:
+    # Pareto Q-learning's set table (csrc/pql.cu): an update with s' == s, one with an overflow, both score modes at d 2 and 4, cardinality
+    # at d 8, the A = 16 range
+    from morl_baselines_b200 import pql_ops
+
+    for S, A, K, d in [(3, 4, 8, 2), (3, 16, 64, 4), (3, 2, 4, 8)]:
+        t = pql_ops.PqlTable(S, A, K, d, dev)
+        t.nd.copy_(th.rand(S, A, K, d, device=dev, dtype=th.float64, generator=g))
+        t.nd_count.fill_(K)
+        pql_ops.pql_update(t, 0, A - 1, 0, np.ones(d), 0.9)
+        pql_ops.pql_update(t, 1, 0, 2, np.ones(d), 1.0)
+        pql_ops.pql_score(t, 0, pql_ops.CARDINALITY, 0.9)
+        if d <= 4:
+            pql_ops.pql_score(t, 1, pql_ops.HYPERVOLUME, 0.9, np.zeros(d))
+    th.cuda.synchronize()
+    print("pql ok")
 print("sanitize run ok")
