@@ -311,6 +311,38 @@ MORL_API int morl_pql_update_f64(double* nd, int* nd_count, double* avg_reward, 
 MORL_API int morl_pql_score_f64(const double* nd, const int* nd_count, const double* avg_reward, int S, int A, int K, int d, int state,
                                 double gamma, int mode, const double* ref, double* scores, void* stream);
 
+/* Multi-policy scalarised Q-learning (multi_policy/multi_policy_moqlearning/mp_mo_q_learning.py with single_policy/ser/mo_q_learning.py and
+ * common/model_based/tabular_model.py), caller-owned device tensors for S states, P policy slots, A actions, d objectives, M model pairs and
+ * K outcomes per pair:  q f64 [S, P, A, d] (zero where a policy never visited a state), visited u8 [S, P], pairs int32 [M, 3] (state,
+ * action, number of outcomes; zeroed), outcomes int32 [M, K, 2] (next state, terminal), counts int64 [M, K] (zeroed), out_reward
+ * f64 [M, K, d], tree f64 [2^18 - 1] (the reference's SumTree(max_size=1e5), zeroed), status int32 [2] (zeroed).  w . v adds the products
+ * left to right, one IEEE operation each; every update is numpy's expression order with no FMA contraction.
+ * morl_moq_act_f64 : n rows (HOST arrays, passed by value: no copy to the device), one block per row.  policy[i] >= 0: argmax over actions
+ *   of w . q[state, policy]; policy[i] == -1: GPI, argmax over the stacked [n_policies, A] values in row-major order.  First maximum wins
+ *   (numpy's argmax, a NaN first); a state the policy never visited, and state -1, scores 0.  out int32 [n, 2] = (action, visited) where
+ *   visited is 1 iff an own-policy row's state is in the policy's table; value f64 [n] (may be NULL) = the winning value.
+ * morl_moq_step_f64 : one environment step of policy p (mo_q_learning.py:173-208) in one block: visit s and s_next, greedy action at
+ *   s_next (GPI over the first n_policies with MORL_MOQ_GPI), td = r + ((1 - terminal) * gamma) * q[s_next, p, a'] - q[s, p, a],
+ *   q[s, p, a] += lr * td.  With MORL_MOQ_MODEL the transition enters the model as outcome `outcome` of pair `pair` (the caller keys both;
+ *   pair < n_pairs), then n_updates Dyna updates follow, each on a pair drawn uniformly (pick[j], HOST) or, with MORL_MOQ_PRIORITIZE, by
+ *   the tree walk of query root * u[j] (HOST), an outcome drawn as random.choices does with random() = choice[j] (HOST), and the same TD
+ *   update.  With MORL_MOQ_PRIORITIZE every update also sets the pair's leaf to max(|r.w + ((1 - terminal) gamma) max_scalar_q(s', w)
+ *   - q[s, p, a].w|, min_priority) ** alpha.  w and reward: HOST pointers to d doubles, passed by value.  A walk that lands on a leaf
+ *   >= n_pairs (the reference's IndexError) writes status = {1, leaf} and stops; while status[0] != 0 the call changes nothing.  More than
+ *   64 Dyna updates run as consecutive launches.
+ * Supported range (morl_moq_supported, no device needed): 1 <= A <= 64, 1 <= d <= MORL_MAX_D; else MORL_ERR_UNSUPPORTED. */
+#define MORL_MOQ_GPI 1
+#define MORL_MOQ_MODEL 2
+#define MORL_MOQ_PRIORITIZE 4
+MORL_API int morl_moq_supported(int n_actions, int d);
+MORL_API int morl_moq_act_f64(const double* q, const unsigned char* visited, int S, int P, int A, int d, int n_policies, const int* state,
+                              const int* policy, const double* w, int n, int* out, double* value, void* stream);
+MORL_API int morl_moq_step_f64(double* q, unsigned char* visited, int* pairs, int* outcomes, long long* counts, double* out_reward, double* tree,
+                               int* status, int S, int P, int A, int d, int M, int K, int n_policies, int p, int s, int a, int s_next, int terminal,
+                               int pair, int outcome, int n_pairs, const double* w, const double* reward, int flags, double gamma, double lr,
+                               double min_priority, double alpha, int n_updates, const int* pick, const double* u, const double* choice,
+                               void* stream);
+
 /* Corner weights of a convex coverage set (OLS / GPI-LS weight selection).  Replaces compute_corner_weights
  * (multi_policy/linear_support/linear_support.py:295-349), which enumerates with cdd the vertices of
  *   { (w, u) : V w <= u 1,  w >= 0,  sum w = 1 }.

@@ -19,8 +19,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 BUILD = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libmorl_b200.so")
-SOURCES = ["api.cu", "envelope_td.cu", "gpi_td.cu", "td_loss.cu", "pareto.cu", "replay.cu", "optim.cu", "gemm_planes.cu", "pair_layer1.cu", "host_replay.cu", "sumtree.cu", "qhead_envelope.cu", "dyna.cu", "discrete_sac.cu", "linear_support.cu", "ppo.cu", "pcn.cu", "eupg.cu", "nl_ppo.cu", "pql.cu"]
-HEADERS = ["common.cuh", "gemm_tc.cuh", "envelope_wp.cuh", "tile_mlp.cuh", "hv.cuh", os.path.join(ROOT, "include", "morl_b200.h")]
+SOURCES = ["api.cu", "envelope_td.cu", "gpi_td.cu", "td_loss.cu", "pareto.cu", "replay.cu", "optim.cu", "gemm_planes.cu", "pair_layer1.cu", "host_replay.cu", "sumtree.cu", "qhead_envelope.cu", "dyna.cu", "discrete_sac.cu", "linear_support.cu", "ppo.cu", "pcn.cu", "eupg.cu", "nl_ppo.cu", "pql.cu", "moq.cu"]
+HEADERS = ["common.cuh", "gemm_tc.cuh", "envelope_wp.cuh", "tile_mlp.cuh", "hv.cuh", "sumtree.cuh", os.path.join(ROOT, "include", "morl_b200.h")]
 
 NVCC_FLAGS = [
     "-gencode",

@@ -18,27 +18,16 @@
 //   priorities: p = fl32(fl32(|w . td| + min_p) ** alpha)  and  min_p = max(min_p, max p)                                 (envelope.py:329-334,
 //               prioritized_buffer.py:194); the power is evaluated in float64 and rounded once to float32 (numpy's float32 power is
 //               within 1 ulp of that, but not reproducible across its own SIMD / libm back ends).
-#include "common.cuh"
+#include "sumtree.cuh"
 
 namespace morl {
-
-__device__ __forceinline__ double* st_level(double* tree, int l) { return tree + (((size_t)1) << l) - 1; }
-__device__ __forceinline__ const double* st_level(const double* tree, int l) { return tree + (((size_t)1) << l) - 1; }
 
 __global__ void __launch_bounds__(256) sumtree_walk_kernel(const double* __restrict__ tree, int n_levels, const double* __restrict__ u, int n,
                                                            int scale_by_root, long long* __restrict__ out) {
     pdl_enter();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    double q = scale_by_root ? __dmul_rn(tree[0], u[i]) : u[i];
-    long long node = 0;
-    for (int l = 1; l < n_levels; ++l) {
-        const double left = st_level(tree, l)[2 * node];
-        const bool right = q > left;
-        node = 2 * node + (right ? 1 : 0);
-        q = __dsub_rn(q, __dmul_rn(left, right ? 1.0 : 0.0));  // query -= left_sum * is_greater
-    }
-    out[i] = node;
+    out[i] = st_walk(tree, n_levels, scale_by_root ? __dmul_rn(tree[0], u[i]) : u[i]);
 }
 
 constexpr int kStMaxBatch = 2048;  // (44 KB of static shared memory)
@@ -134,13 +123,7 @@ __global__ void __launch_bounds__(32) sumtree_set_kernel(double* __restrict__ tr
         if (threadIdx.x == 0) *err = 1;
         return;
     }
-    const double p = use_min ? *min_priority : priority;
-    const double d = __dsub_rn(p, st_level(tree, n_levels - 1)[index]);  // (every lane reads the old leaf before any lane writes it)
-    __syncwarp();
-    for (int l = threadIdx.x; l < n_levels; l += 32) {
-        double* node = st_level(tree, l) + (index >> (n_levels - 1 - l));
-        *node = __dadd_rn(*node, d);
-    }
+    st_set_warp(tree, n_levels, index, use_min ? *min_priority : priority);
 }
 
 // p32[i] = fl32( (fl32(raw[i] + fl32(min_p))) ** alpha ), p64 = (double) p32, then min_p = max(min_p, max_i p32[i]).  One block.

@@ -2,7 +2,7 @@
 
     compute-sanitizer --tool memcheck|racecheck|synccheck|initcheck python scripts/sanitize_all.py [group ...]
 
-groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners ppo pcn eupg nl_ppo hv_batch pql (default: all; dyna includes the fused Dyna commit).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
+groups: envelope td gemm optim pareto replay layer1 qhead dyna chain corners ppo pcn eupg nl_ppo hv_batch pql moq (default: all; dyna includes the fused Dyna commit).  Shapes are small (sanitizer slows kernels 10-100x) but exercise
 every code path: all envelope kernel families, both GEMM operand formats x CTA modes x accumulator modes, MN split-K GEMM with the fused
 column sums, every split / reduction helper, the loss kernels (discrete SAC's included), Adam, polyak, Pareto + front records, replay gather,
 the corner-weight enumeration, MO-PPO's vector GAE and loss (racecheck: the loss kernel's CTA reductions), PCN's update and forward,
@@ -24,7 +24,7 @@ if os.environ.get("SAN_ZERO_PLANES") == "1":
     # from a genuine read of memory nobody wrote.
     _empty = ops.empty_planes
     ops.empty_planes = lambda *a, **k: _empty(*a, **k).zero_()
-groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain", "corners", "ppo", "pcn", "eupg", "nl_ppo", "hv_batch", "pql"}
+groups = set(sys.argv[1:]) or {"envelope", "td", "gemm", "optim", "pareto", "replay", "layer1", "qhead", "dyna", "chain", "corners", "ppo", "pcn", "eupg", "nl_ppo", "hv_batch", "pql", "moq"}
 
 
 def rn(*s, scale=1.0):
@@ -326,4 +326,17 @@ if "pql" in groups:
             pql_ops.pql_score(t, 1, pql_ops.HYPERVOLUME, 0.9, np.zeros(d))
     th.cuda.synchronize()
     print("pql ok")
+if "moq" in groups:
+    # multi-policy MO Q-learning (csrc/moq.cu): GPI and own-policy rows with state -1, a prioritised step with 70 Dyna updates (two launches)
+    # and s' == s, a uniform step
+    from morl_baselines_b200 import moq_ops
+
+    for A, d, prio in [(4, 2, True), (16, 8, False)]:
+        t = moq_ops.MoqTable(A, d, dev, True, S=8, P=3, M=8, K=2)
+        flags = moq_ops.GPI | moq_ops.MODEL | (moq_ops.PRIORITIZE if prio else 0)
+        moq_ops.moq_step(t, 3, 1, 0, A - 1, 0, False, np.ones(d) / d, np.ones(d), flags, 0.9, 0.1, pair=0, outcome=1, n_pairs=1,
+                         pick=[0] * 70, u=[0.5] * 70, choice=[0.3] * 70)
+        moq_ops.moq_act(t, 3, [0, -1, 7], [-1, 0, 2], np.ones((3, d)))
+    th.cuda.synchronize()
+    print("moq ok")
 print("sanitize run ok")
